@@ -1,8 +1,8 @@
-# Builds the product library (sm_100a only) and the CPU oracle.
+# Builds the product library (sm_90a only) and the CPU oracle.
 #   make            -> f2nerf_b200/libf2nerf_b200.so + oracle/libf2oracle.so
 #   make ref        -> oracle/_ref/ref_driver (the unmodified reference, ~25 min; needs /root/reference)
 NVCC    ?= /usr/local/cuda/bin/nvcc
-ARCH    := -gencode arch=compute_100a,code=sm_100a
+ARCH    := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xptxas -v
 CSRC    := f2nerf_b200/csrc
 SRCS    := $(wildcard $(CSRC)/*.cu)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — training rays/s of the F2-NeRF per-ray rendering hot path on B200.
+"""bench.py — training rays/s of the F2-NeRF per-ray rendering hot path on H100.
 
 One "step" = one pass of the hot path over one batch: Renderer.Render (perspective-warp ray march,
 early-stop pass, hash encode, density + colour MLPs, composite) + the trainer's loss + backward down
@@ -16,6 +16,8 @@ big20, big22, synthetic.
 
   python bench.py --gpus N --steps K --warmup W [--config C]      (torchrun launches N > 1)
   python bench.py --impl reference ...     the path's CPU port (oracle/) on the same config, all host threads, rank 0 only
+  --dump-outputs DIR                        also write what the last step of the first timed run computed (RenderResult
+                                            fields, loss, parameter gradients) as DIR/<name>.npy, to compare two builds
 """
 import argparse
 import json
@@ -47,7 +49,7 @@ def config_dict(args, world):
                         "Render + loss + backward",
             "name": args.config, "rays_per_gpu": per_gpu, "global_rays": per_gpu * world, "log2_table_size": cfg["log2_table"],
             "parallelism": f"dp{world} (rays sharded, params replicated)",
-            "l2": "per-step working set (>=100 MB of samples + the table) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "per-step working set (>=100 MB of samples + the table) exceeds the 50 MB L2; no explicit flush"}
 
 
 def load_peaks():
@@ -55,7 +57,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=float(d["hbm_gbs"]), tf=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), src="measured")
-    return dict(hbm=6650.0, tf=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf=989.0, src="fallback: H100 SXM data sheet (HBM3, dense FP16)")
 
 
 class ClockSampler(threading.Thread):
@@ -271,10 +273,9 @@ def run_ours(args):
     if world > 1:
         from f2nerf_b200.dist import install_grad_overlap, install_vote_sync
         install_vote_sync(prob["sampler"])
-        # F2B_DP_OVERLAP=1: table-gradient all-reduce per level slab behind a per-slab scatter (dist.install_grad_overlap).  Measured
-        # on B200 (profiles/r02f_*, r02g_*): the four per-slab scatter launches cost +0.17 ms against the single 16-level launch,
-        # more than the overlapped all-reduce saves at N = 2 and 4 (4.64 / 4.73 vs 4.48 / 4.64 ms) — so the default is ONE
-        # all-reduce of the live 34 MB behind the single scatter launch.
+        # F2B_DP_OVERLAP=1: table-gradient all-reduce per level slab behind a per-slab scatter (dist.install_grad_overlap).  The
+        # default is ONE all-reduce of the live 34 MB behind the single 16-level scatter launch (four per-slab scatter launches cost
+        # more than the overlap saves).
         if os.environ.get("F2B_DP_OVERLAP", "0") == "1":
             install_grad_overlap(prob["renderer"])
     o, d, cam, gt = prob["host"]
@@ -305,6 +306,8 @@ def run_ours(args):
         finally:
             gc.enable()
 
+    dumped = []
+
     def _timed_loop():
         barrier()
         l0 = _lib.LAUNCHES
@@ -320,6 +323,8 @@ def run_ours(args):
             w.append(round((time.perf_counter() - w0) * 1e3, 2))
         eb.record()
         barrier()
+        if args.dump_outputs and not dumped:      # the first run: what precedes it does not depend on re-timing
+            dumped.append(step_outputs(prob, loss, res))
         return ea.elapsed_time(eb), w, ns, nk, _lib.LAUNCHES - l0
 
     # A step whose host wall time is far off the median (seen on fresh boxes: one NVML poll of the clock sampler
@@ -474,9 +479,44 @@ def run_ours(args):
         cpp = cpp_host_timing(args)
         if cpp is not None:
             line["cpp_host"] = cpp
+        if args.dump_outputs:
+            line["dumped_outputs"] = dump_outputs(args.dump_outputs, dumped[0])
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_MAX_ELEMS = 1 << 22     # per array: a larger one is written as a fixed, seeded sample of this many elements (16 MB)
+
+
+def step_outputs(prob, loss, res):
+    """What a caller of the timed path receives from one step, as host float arrays: the RenderResult fields, the loss and the
+    parameter gradients the backward left behind."""
+    out = {"loss": loss.detach().reshape(1), "colors": res.colors, "first_oct_dis": res.first_oct_dis, "disparity": res.disparity,
+           "depth": res.depth, "weights": res.weights, "idx_start_end": res.idx_start_end, "edge_feats": res.edge_feats,
+           "grad_feat_pool": prob["field"].feat_pool_.grad, "grad_field_mlp": prob["field"].mlp_.params_.grad,
+           "grad_shader_mlp": prob["shader"].mlp_.params_.grad, "grad_app_emb": prob["renderer"].app_emb_.grad}
+    host = {}
+    for k, v in out.items():
+        if v is None:
+            continue
+        a = v.detach().cpu().numpy()
+        host[k] = a.astype(np.float64 if a.dtype in (np.int32, np.int64, np.float64) else np.float32)
+    return host
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes ``arrays`` as out_dir/<name>.npy; an array above DUMP_MAX_ELEMS elements becomes <name>_sample.npy, its flattened
+    values at sorted indices drawn with a seed fixed per name and size (the same elements in every run)."""
+    os.makedirs(out_dir, exist_ok=True)
+    written = {}
+    for k, a in sorted(arrays.items()):
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng([a.size, len(k)]).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a, k = a.reshape(-1)[idx], k + "_sample"
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+        written[k] = list(a.shape)
+    return written
 
 
 def forward_only_timing(prob, d_o, d_d, args, iters=20):
@@ -617,7 +657,7 @@ def cpp_host_timing(args):
         if r.returncode != 0:
             return {"unavailable": ("ref_driver_b200 rc %d: " % r.returncode) + r.stderr[-160:]}
         t = json.load(open(os.path.join(out_dir, "ref_timing.json")))
-        t["note"] = "the reference's program with the B200 C++ host linked in as Renderer::Render (no march pipelining in this harness)"
+        t["note"] = "the reference's program with this library's C++ host linked in as Renderer::Render (no march pipelining in this harness)"
         return t
     except Exception as e:  # noqa: BLE001
         return {"unavailable": str(e)[:200]}
@@ -643,7 +683,7 @@ def reference_gpu_timing(args):
             return {"unavailable": ("ref_driver rc %d: " % r.returncode) + r.stderr[-160:]}
         t = json.load(open(os.path.join(out_dir, "ref_timing.json")))
         t["config_yaml"] = cfg["ref_yaml"]
-        t["note"] = "unmodified Totoro97/f2-nerf + tiny-cuda-nn compiled for sm_100a; same scene / rays / parameters as the product arm"
+        t["note"] = "unmodified Totoro97/f2-nerf + tiny-cuda-nn compiled for sm_90a; same scene / rays / parameters as the product arm"
         return t
     except Exception as e:  # noqa: BLE001
         return {"unavailable": str(e)[:200]}
@@ -749,6 +789,8 @@ def main():
                     help="march every batch at the start of its own Render (default: the next batch's march runs behind this step's backward)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last step of the first timed run as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""f2nerf_b200 — B200-native (sm_100a) implementation of F2-NeRF's per-ray rendering hot path.
+"""f2nerf_b200 — H100-native (sm_90a) implementation of F2-NeRF's per-ray rendering hot path.
 
 The product is ``libf2nerf_b200.so`` (hand-written CUDA behind the C ABI in ``include/f2nerf_b200.h``);
 this package is the thin host-side mirror of the reference's operator surface

@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/f2nerf_b200.h (libf2nerf_b200.so, sm_100a only).
+"""ctypes binding of the C ABI in include/f2nerf_b200.h (libf2nerf_b200.so, sm_90a only).
 
 The product path has no CPU fallback: if the shared library is missing or does not load, importing
 this module raises.  Tensors cross the boundary as raw device pointers (``Tensor.data_ptr()``) plus

@@ -1,11 +1,11 @@
 // api.cu — implementation selection for the MLP entry points of the C ABI.
-// impl 0 = CUDA-core twin (mlp.cu), impl 1 = tcgen05/TMEM kernels (mlp_tc.cu).  The default is the
+// impl 0 = CUDA-core twin (mlp.cu), impl 1 = wgmma tensor-core kernels (mlp_tc.cu).  The default is the
 // tensor-core path; F2B_MLP_IMPL=0 in the environment (or f2b_set_mlp_impl) selects the twin.
 #include "common.cuh"
 #include <stdlib.h>
 
 #ifndef F2B_TC_BWD_DEFAULT
-#define F2B_TC_BWD_DEFAULT 1   // mlp_tc_bwd.cu validated on B200 (tests/test_gpu_parity.py::test_mlp_fwd_bwd[tc-*])
+#define F2B_TC_BWD_DEFAULT 1   // mlp_tc_bwd.cu validated on H100 (tests/test_gpu_parity.py::test_mlp_fwd_bwd[tc-*])
 #endif
 
 extern "C" int f2b_mlp_fwd_v0(const void*, const void*, int, int, void*, void*, void*);
@@ -49,7 +49,7 @@ static int mlp_impl() {
 
 extern "C" int f2b_set_mlp_impl(int impl) {
 #ifndef F2B_HAVE_TC
-  if (impl != 0) { f2b::set_error("f2b_set_mlp_impl: tcgen05 path not built"); return F2B_EUNSUPPORTED; }
+  if (impl != 0) { f2b::set_error("f2b_set_mlp_impl: tensor-core path not built"); return F2B_EUNSUPPORTED; }
 #endif
   g_mlp_impl = impl;
   g_mlp_bwd_impl = impl ? F2B_TC_BWD_DEFAULT : 0;
@@ -91,6 +91,6 @@ extern "C" int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void
 #ifdef F2B_HAVE_TC
   if (mlp_bwd_impl() == 1) return f2b_mlp_bwd2_tc(dout_f16, in_f16, hidden0_f16, hidden1_f16, params_f16, n_hidden_matmuls, n_pts, din_f16, dparams_f32, stream);
 #endif
-  if (!hidden0_f16 && n_pts > 0) { f2b::set_error("f2b_mlp_bwd2: recompute (hidden0 == NULL) needs the tcgen05 implementation"); return F2B_EUNSUPPORTED; }
+  if (!hidden0_f16 && n_pts > 0) { f2b::set_error("f2b_mlp_bwd2: recompute (hidden0 == NULL) needs the tensor-core implementation"); return F2B_EUNSUPPORTED; }
   return f2b_mlp_bwd2_v0(dout_f16, in_f16, hidden0_f16, hidden1_f16, params_f16, n_hidden_matmuls, n_pts, din_f16, dparams_f32, stream);
 }

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the f2nerf_b200 sm_100a kernels (no torch, no Eigen).
+// common.cuh — shared helpers for the f2nerf_b200 sm_90a kernels (no torch, no Eigen).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -22,6 +22,13 @@ int  check_launch(const char* what);   // cudaGetLastError -> F2B_ECUDA + messag
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 static inline int div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+// CTAs of a persistent kernel that are resident on one SM at once (registers and shared memory decide), at least 1
+template <class Kernel>
+static inline int resident_per_sm(Kernel kernel, int threads, size_t smem_bytes) {
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, smem_bytes) != cudaSuccess) n = 1;
+  return n > 0 ? n : 1;
+}
 
 // ---- reference POD layouts (PersSampler.h:15-37), restated without Eigen -------------------
 struct __align__(32) TreeNode {      // 64 B

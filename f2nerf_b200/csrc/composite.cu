@@ -1,5 +1,5 @@
 // composite.cu — front-to-back alpha compositing, early-stop compaction and the per-ray
-// segmented ops, one warp per ray, for sm_100a.
+// segmented ops, one warp per ray, for sm_90a.
 //
 // Replaces the tail of Renderer::Render (src/Renderer/Renderer.cpp:107-150 early-stop pass,
 // :196-208 composite), TruncExp (src/Utils/CustomOps/CustomOps.cpp:9-18), FlexOps::Sum /
@@ -8,7 +8,7 @@
 // GradientScaling backward (CustomOps.cu:68-80) and WeightVarLoss (CustomOps.cu:12-66).
 //
 // The reference spends ~25 ATen launches (each a full pass over all samples) plus thread-per-ray
-// serial kernels here.  On B200 this is pure HBM streaming: one kernel reads 24 B/sample once and
+// serial kernels here.  This is pure HBM streaming: one kernel reads 24 B/sample once and
 // writes 4 B/sample.  Lanes load 32 consecutive samples (coalesced); the per-ray prefix/sums are
 // then chained IN THE REFERENCE'S serial left-to-right order through warp shuffles, so forward
 // values (and the early-stop mask / compacted indices that depend on them) round exactly like

@@ -1,10 +1,10 @@
 // field.cu — Hash3DAnchored::AnchoredQuery as ONE kernel: 16-level hash encode fused in front of the
-// tcgen05 field MLP (32 -> 64 -> 16).
+// wgmma field MLP (32 -> 64 -> 16).
 //
 // Replaces, per call, the reference's chain  (pts+1)/2 [ATen]  ->  Hash3DAnchoredForwardKernel x16 grid.y
 // passes  ->  fp16->fp32 cast  ->  pad  ->  fp32->fp16 identity encoding  ->  kernel_mlp_fused  ->  slice +
 // fp16->fp32 cast (src/Field/Hash3DAnchored.cpp:84-99, Hash3DAnchored.cu:160-197, TCNNWP.cpp:102-113).
-// The 32 encoded halfs of a sample go from registers straight into the UMMA operand tile in shared
+// The 32 encoded halfs of a sample go from registers straight into the wgmma operand tile in shared
 // memory (SWIZZLE_64B K-major row of thread i == sample i); they reach HBM only when the backward pass
 // needs them (feat_save).  Modes:
 //   logit_only  — the no-grad early-stop pass (Renderer.cpp:107-126) needs only channel 0: 4 B/sample out
@@ -21,7 +21,6 @@ namespace f2b {
 using namespace tc;
 
 constexpr int kFT = 128;
-constexpr int kFieldTmemCols = 64;
 constexpr int kFieldDefaultMinB = 4;   // see DESIGN.md: 4 = max loads in flight per thread, 6 = max resident warps
 
 struct FieldSmem {
@@ -29,8 +28,8 @@ struct FieldSmem {
   static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB
   static constexpr int W0 = 24576;      // [64 x 32]  SW64       4 KB
   static constexpr int WO = 28672;      // [16 x 64]  SW128      2 KB
-  static constexpr int BAR = 30720;     // mbarrier + tmem slot + 16 level scales
-  static constexpr int BYTES = 30720 + 128 + 1024;
+  static constexpr int SCALE = 30720;   // 16 level scales
+  static constexpr int BYTES = 30720 + 64 + 1024;
 };
 
 template <bool LOGIT_ONLY, int MINB>
@@ -42,10 +41,9 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
                  float* __restrict__ out, __half* __restrict__ feat_save, __half* __restrict__ hidden_save) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(sm + FieldSmem::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + FieldSmem::BAR + 8);
-  float* s_scale = reinterpret_cast<float*>(sm + FieldSmem::BAR + 16);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  float* s_scale = reinterpret_cast<float*>(sm + FieldSmem::SCALE);
+  float* s_rows = reinterpret_cast<float*>(sm + FieldSmem::A1);     // output rows [128][20] fp32 (A1 is dead by then)
+  const int tid = threadIdx.x;
 
   for (int i = tid; i < 64 * 4; i += kFT) {                       // W0 [64 x 32] -> SW64
     const int r = i >> 2, c = i & 3;
@@ -56,18 +54,11 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
     *reinterpret_cast<uint4*>(sm + FieldSmem::WO + sw128_off(r, c)) = *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
   }
   if (tid < F2B_N_LEVELS) s_scale[tid] = level_scale(tid);        // run-time MUFU.EX2, like the reference
-  if (tid == 0) mbar_init(mbar, 1);
-  if (warp == 0) tmem_alloc(tmem_slot, kFieldTmemCols);
-  fence_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_row = tmem + (uint32_t(warp * 32) << 16);
   const uint32_t a0 = smem_u32(sm + FieldSmem::A0), a1 = smem_u32(sm + FieldSmem::A1);
   const uint32_t w0 = smem_u32(sm + FieldSmem::W0), wo = smem_u32(sm + FieldSmem::WO);
-  constexpr uint32_t idesc64 = idesc_f16_f32(128, 64), idesc16 = idesc_f16_f32(128, 16);
-  uint32_t phase = 0;
+  Acc<64> acc;
+  Acc<16> acc_out;
 
   const int n_tiles = (n_pts + kFT - 1) / kFT;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -93,14 +84,11 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
     for (int c = 0; c < 4; c++)
       *reinterpret_cast<uint4*>(sm + FieldSmem::A0 + sw64_off(tid, c)) = make_uint4(enc[4 * c], enc[4 * c + 1], enc[4 * c + 2], enc[4 * c + 3]);
     fence_async_smem();
-    __syncthreads();
+    __syncthreads();                                              // (also: the previous tile's output rows have been read)
     // ---- layer 0 on the tensor pipe -------------------------------------------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < 2; k++) mma_f16(tmem, kmajor_desc(a0 + 32 * k, 64), kmajor_desc(w0 + 32 * k, 64), idesc64, k);
-      mma_commit(mbar);
-    }
+    wg_fence();
+    mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
+    wg_commit();
     if (feat_save) {                                              // whole-line copy-out of the tile while the MMA reads it
       const int rows = min(kFT, n_pts - tile * kFT);
       uint4* dst = reinterpret_cast<uint4*>(feat_save + size_t(tile) * kFT * 32);
@@ -110,33 +98,14 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
         if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A0 + sw64_off(r, c & 3));
       }
     }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + 16 * q, r);
-      tmem_ld_wait();
-      uint4 v[2];
-      uint32_t* vw = reinterpret_cast<uint32_t*>(v);
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        const __half2 h = __floats2half2_rn(fmaxf(__uint_as_float(r[2 * e]), 0.f), fmaxf(__uint_as_float(r[2 * e + 1]), 0.f));
-        vw[e] = *reinterpret_cast<const uint32_t*>(&h);
-      }
-      *reinterpret_cast<uint4*>(sm + FieldSmem::A1 + sw128_off(tid, 2 * q)) = v[0];
-      *reinterpret_cast<uint4*>(sm + FieldSmem::A1 + sw128_off(tid, 2 * q + 1)) = v[1];
-    }
-    fence_before_sync();
+    wg_wait();
+    acc_relu_to_tile(acc, sm + FieldSmem::A1, tid);
     fence_async_smem();
     __syncthreads();
     // ---- output layer -------------------------------------------------------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < 4; k++) mma_f16(tmem, kmajor_desc(a1 + 32 * k, 128), kmajor_desc(wo + 32 * k, 128), idesc16, k);
-      mma_commit(mbar);
-    }
+    wg_fence();
+    mma_m128<16, 0, 4>(acc_out, a1, 128, wo, 128, false);
+    wg_commit();
     if (!LOGIT_ONLY && hidden_save) {
       const int rows = min(kFT, n_pts - tile * kFT);
       uint4* dst = reinterpret_cast<uint4*>(hidden_save + size_t(tile) * kFT * 64);
@@ -146,12 +115,13 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
         if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A1 + sw128_off(r, c & 7));
       }
     }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
+    wg_wait();
+    __syncthreads();                                              // every warp is done with A1 (operand / copy-out)
+    acc_to_rows(acc_out, s_rows, kRowLd16, tid);
+    __syncthreads();
     {
       uint32_t r[16];
-      tmem_ld16(tmem_row, r);
-      tmem_ld_wait();
+      row_ld16(s_rows, kRowLd16, tid, r);
       if (valid) {
         if (LOGIT_ONLY) {
           out[p] = __half2float(__float2half_rn(__uint_as_float(r[0])));
@@ -164,10 +134,7 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
         }
       }
     }
-    fence_before_sync();
-    __syncthreads();
   }
-  if (warp == 0) tmem_dealloc(tmem, kFieldTmemCols);
 }
 
 }  // namespace f2b
@@ -206,7 +173,7 @@ static int field_fwd_launch(const void* table_f16, const int* prim_pool, const f
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(table_f16 && prim_pool && bias_pool && mlp_params_f16 && pts && vol && out_f32, "f2b_field_fwd: null pointer");
   F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_field_fwd: bad n_volumes/local_size");
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kFT);
   static int minb = -1;                                           // resident CTAs per SM the kernel is compiled for

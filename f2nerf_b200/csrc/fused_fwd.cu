@@ -7,14 +7,14 @@
 // between the march's output and the per-ray result.  Nothing per-sample goes to HBM: a sample costs 28 B read from the march's
 // slots + its 128 table gathers (SURVEY.md §8d "fused forward pipeline": 512 B/pt of gathers is the whole traffic).
 //
-// Shape: a "walker" (128 threads, thread i == sample i == TMEM lane i) walks ONE RAY front to back, a 128-sample tile at a
+// Shape: a "walker" (128 threads = one warpgroup, thread i == sample i) walks ONE RAY front to back, a 128-sample tile at a
 // time, and carries the ray's optical depth across tiles; a CTA holds one walker (optionally two independent ones sharing the weights).  Because the reference's early-stop mask `T_i > 1e-4`
 // (Renderer.cpp:125) is a prefix of the ray (tau >= 0 => T non-increasing), the walk simply ENDS at the first tile whose
 // leading sample is already opaque: the samples behind it are never encoded (the unfused path encodes every marched sample,
 // then drops them).  No occupancy votes are taken in VALIDATE mode, so nothing downstream needs those samples.
 // Rays are handed out through an atomic ticket (ray lengths differ by 10x).
 //
-// Arithmetic is the unfused path's, operation for operation: encode_point (hash.cuh), the two tcgen05 MLPs with the same
+// Arithmetic is the unfused path's, operation for operation: encode_point (hash.cuh), the two wgmma MLPs with the same
 // operand tiles (row results do not depend on which other rows share the tile), shade_row / shade_act (shader.cuh), and the
 // composite's SERIAL left-to-right sums (FlexOps.cu:5-73 order, as composite.cu) — colours / depth / disparity / weights come
 // out bit-identical to f2b_render_phase1 + _phase2_fwd (tests/test_gpu_render.py::test_fused_forward_matches_unfused).
@@ -47,7 +47,8 @@ struct FusedSmem {
   static constexpr int TAU = H0;          // float tau[128]          (inside H0)
   static constexpr int ACC = H0 + 512;    // float acc[129]
   static constexpr int ADD = H0 + 2048;   // float add[5][128]
-  static constexpr int BAR = WALK0 + NW * WALK;   // per walker 16 B: mbarrier (8) | ray ticket (4); then tmem slot (4) | 16 level scales
+  static constexpr int ROWS = H0 + 4608;  // float rows[128][20]     (inside H0) an MLP's 16 outputs per sample
+  static constexpr int BAR = WALK0 + NW * WALK;   // per walker 16 B: ray ticket (4); then 16 B | 16 level scales
   static constexpr int BYTES = BAR + 16 * NW + 16 + 64 + 1024;   // + alignment slack (the tiles need 1024-byte alignment)
 };
 
@@ -57,25 +58,6 @@ __device__ __forceinline__ void stage_w_fused(const __half* __restrict__ w, int 
   for (int i = threadIdx.x; i < rows * chunks; i += blockDim.x) {
     const int r = i / chunks, c = i % chunks;
     *reinterpret_cast<uint4*>(dst + (K == 64 ? sw128_off(r, c) : sw64_off(r, c))) = *reinterpret_cast<const uint4*>(w + r * K + c * 8);
-  }
-}
-
-// accumulator row (64 fp32 in TMEM) -> ReLU -> fp16 -> my row of the H tile
-__device__ __forceinline__ void relu_row(uint32_t tmem_row, unsigned char* h_tile, int row) {
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    uint32_t r[16];
-    tmem_ld16(tmem_row + 16 * q, r);
-    tmem_ld_wait();
-    uint4 v[2];
-    uint32_t* vw = reinterpret_cast<uint32_t*>(v);
-#pragma unroll
-    for (int e = 0; e < 8; e++) {
-      const __half2 h = __floats2half2_rn(fmaxf(__uint_as_float(r[2 * e]), 0.f), fmaxf(__uint_as_float(r[2 * e + 1]), 0.f));
-      vw[e] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q)) = v[0];
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q + 1)) = v[1];
   }
 }
 
@@ -95,11 +77,11 @@ __device__ __forceinline__ int walker_sync_count(int w, bool pred) {
   return n;
 }
 
-// NW = 1 (default): the CTA is one walker (4 CTAs per SM); NW = 2: two walkers share the 20 KB of weights, so SIX walkers fit an SM
-// (three CTAs, <= 80 registers) instead of four — more walkers to keep the gather pipe busy during each other's MLP / composite
-// phases, but fewer gathers in flight per thread: measured slower (see the launcher).
+// NW = 1 (default): the CTA is one walker (3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers); NW = 2: two
+// walkers share the 20 KB of weights (two CTAs, <= 128 registers, with spills) — more walkers to keep the gather pipe busy during each
+// other's MLP / composite phases, but fewer gathers in flight per thread.
 template <int NW>
-__global__ void __launch_bounds__(kRT * NW, NW == 2 ? 3 : 4)
+__global__ void __launch_bounds__(kRT * NW, NW == 2 ? 2 : 3)
 render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool,
                         int n_volumes, int local_size, const __half* __restrict__ fparams, const __half* __restrict__ sparams,
                         const float* __restrict__ s_pts, const float* __restrict__ s_dt, const float* __restrict__ s_t,
@@ -111,15 +93,14 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int wk = threadIdx.x >> 7;                               // my walker
-  const int tid = threadIdx.x & 127, warp = tid >> 5;            // thread within the walker == sample == TMEM lane
+  const int tid = threadIdx.x & 127;                             // thread within the walker == sample
   unsigned char* wsm = sm + S::WALK0 + wk * S::WALK;
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(sm + S::BAR + 16 * wk);
-  int* s_ray = reinterpret_cast<int*>(sm + S::BAR + 16 * wk + 8);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + S::BAR + 16 * NW);
+  int* s_ray = reinterpret_cast<int*>(sm + S::BAR + 16 * wk);
   float* s_scale = reinterpret_cast<float*>(sm + S::BAR + 16 * NW + 16);
   float* s_tau = reinterpret_cast<float*>(wsm + S::TAU);
   float* s_acc = reinterpret_cast<float*>(wsm + S::ACC);         // exclusive optical depth per sample, [128] = inclusive end
   float* s_add = reinterpret_cast<float*>(wsm + S::ADD);         // [5][128] addends of the five per-ray sums
+  float* s_rows = reinterpret_cast<float*>(wsm + S::ROWS);
 
   stage_w_fused<32>(fparams, 64, sm + S::FW0);
   stage_w_fused<64>(fparams + 64 * 32, 16, sm + S::FWO);
@@ -127,32 +108,30 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   stage_w_fused<64>(sparams + 64 * 32, 64, sm + S::SWH);
   stage_w_fused<64>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO);
   if (threadIdx.x < F2B_N_LEVELS) s_scale[threadIdx.x] = level_scale(threadIdx.x);
-  if (tid == 0) mbar_init(mbar, 1);
-  if (threadIdx.x < 32) tmem_alloc(tmem_slot, 64 * NW);
   fence_async_smem();
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot + 64 * wk;                    // my walker's 64 accumulator columns
-  const uint32_t tmem_row = tmem + (uint32_t(warp * 32) << 16);
   const uint32_t a0 = smem_u32(wsm + S::A0), h0 = smem_u32(wsm + S::H0);
   const uint32_t fw0 = smem_u32(sm + S::FW0), fwo = smem_u32(sm + S::FWO);
   const uint32_t sw0 = smem_u32(sm + S::SW0), swh = smem_u32(sm + S::SWH), swo = smem_u32(sm + S::SWO);
-  constexpr uint32_t idesc64 = idesc_f16_f32(128, 64), idesc16 = idesc_f16_f32(128, 16);
-  uint32_t phase = 0;
+  Acc<64> acc;
+  Acc<16> acc_out;
   const bool empty_batch = total_all && (__ldg(total_all) <= 0);   // Renderer.cpp:83-97: no sample in the WHOLE batch
 
-  // one MMA group issued by the walker's thread 0 + the walker waits for it
-#define F2B_MMA_STAGE(...)                         \
-  do {                                             \
-    if (tid == 0) {                                \
-      fence_after_sync();                          \
-      __VA_ARGS__;                                 \
-      mma_commit(mbar);                            \
-    }                                              \
-    mbar_wait(mbar, phase);                        \
-    phase ^= 1;                                    \
-    fence_after_sync();                            \
+  // one MMA group issued by the walker's warpgroup, which waits for it
+#define F2B_MMA_STAGE(...) \
+  do {                     \
+    wg_fence();            \
+    __VA_ARGS__;           \
+    wg_commit();           \
+    wg_wait();             \
+  } while (0)
+  // the walker's 16 outputs per sample -> my row (the rows sit in H0, the operand of the MMA just completed)
+#define F2B_OUT_ROW(r)                               \
+  do {                                               \
+    walker_sync(wk);                                 \
+    acc_to_rows(acc_out, s_rows, kRowLd16, tid);     \
+    walker_sync(wk);                                 \
+    row_ld16(s_rows, kRowLd16, tid, r);              \
   } while (0)
 
   for (;;) {
@@ -185,21 +164,18 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
 #pragma unroll
       for (int c = 0; c < 4; c++)
         *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = make_uint4(enc[4 * c], enc[4 * c + 1], enc[4 * c + 2], enc[4 * c + 3]);
-      fence_before_sync();                                       // (previous tile's TMEM reads are done)
       fence_async_smem();
       walker_sync(wk);                                           // (also: the previous tile's sums have been read out of H0)
       // ---- field MLP: 32 -> 64 (ReLU) -> 16 -------------------------------------------------------------------------
-      F2B_MMA_STAGE(for (int k = 0; k < 2; k++) mma_f16(tmem, kmajor_desc(a0 + 32 * k, 64), kmajor_desc(fw0 + 32 * k, 64), idesc64, k));
-      relu_row(tmem_row, wsm + S::H0, tid);
-      fence_before_sync();
+      F2B_MMA_STAGE(mma_m128<64, 0, 2>(acc, a0, 64, fw0, 64, false));
+      acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
       walker_sync(wk);
-      F2B_MMA_STAGE(for (int k = 0; k < 4; k++) mma_f16(tmem, kmajor_desc(h0 + 32 * k, 128), kmajor_desc(fwo + 32 * k, 128), idesc16, k));
+      F2B_MMA_STAGE(mma_m128<16, 0, 4>(acc_out, h0, 128, fwo, 128, false));
       float feat[16];
       {
         uint32_t r[16];
-        tmem_ld16(tmem_row, r);
-        tmem_ld_wait();
+        F2B_OUT_ROW(r);
 #pragma unroll
         for (int k = 0; k < 16; k++) feat[k] = h16(r[k]);        // the fp16-rounded outputs TCNNWP::Query returns
       }
@@ -233,24 +209,21 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
 #pragma unroll
         for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = row[c];
       }
-      fence_before_sync();
       fence_async_smem();
       walker_sync(wk);                                           // (thread 0 has read acc[nk]: H0 may be overwritten again)
-      F2B_MMA_STAGE(for (int k = 0; k < 2; k++) mma_f16(tmem, kmajor_desc(a0 + 32 * k, 64), kmajor_desc(sw0 + 32 * k, 64), idesc64, k));
-      relu_row(tmem_row, wsm + S::H0, tid);
-      fence_before_sync();
+      F2B_MMA_STAGE(mma_m128<64, 0, 2>(acc, a0, 64, sw0, 64, false));
+      acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
       walker_sync(wk);
-      F2B_MMA_STAGE(for (int k = 0; k < 4; k++) mma_f16(tmem, kmajor_desc(h0 + 32 * k, 128), kmajor_desc(swh + 32 * k, 128), idesc64, k));
-      relu_row(tmem_row, wsm + S::H0, tid);                      // in place: the hidden layer's MMA has completed
-      fence_before_sync();
+      F2B_MMA_STAGE(mma_m128<64, 0, 4>(acc, h0, 128, swh, 128, false));
+      walker_sync(wk);                                           // in place: every warp's part of the hidden layer's MMA has completed
+      acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
       walker_sync(wk);
-      F2B_MMA_STAGE(for (int k = 0; k < 4; k++) mma_f16(tmem, kmajor_desc(h0 + 32 * k, 128), kmajor_desc(swo + 32 * k, 128), idesc16, k));
+      F2B_MMA_STAGE(mma_m128<16, 0, 4>(acc_out, h0, 128, swo, 128, false));
       {                                                          // (H0 is dead again: the five addend rows live in it)
         uint32_t r[16];
-        tmem_ld16(tmem_row, r);
-        tmem_ld_wait();
+        F2B_OUT_ROW(r);
         float w = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, ts = 1.f;
         if (keep) {
           cr = shade_act(h16(r[0])); cg = shade_act(h16(r[1])); cb = shade_act(h16(r[2]));
@@ -285,9 +258,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
     }
   }
 #undef F2B_MMA_STAGE
-  fence_before_sync();
-  __syncthreads();                                               // both walkers are out of work
-  if (threadIdx.x < 32) tmem_dealloc(*tmem_slot, 64 * NW);
+#undef F2B_OUT_ROW
 }
 
 // weights of the kept samples out of the slot layout into the reference's packed layout (RenderResult.weights, Renderer.h:24)
@@ -318,25 +289,24 @@ extern "C" int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool,
               "f2b_render_fwd_fused: null pointer");
   F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_render_fwd_fused: bad n_volumes/local_size");
   F2B_REQUIRE(slot_size > 0 && int64_t(n_rays) * slot_size < (int64_t(1) << 31), "f2b_render_fwd_fused: n_rays * slot_size overflows int32");
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("f2b_render_fwd_fused: memset failed"); return F2B_ECUDA; }
-  // ray walkers per CTA (F2B_FUSED_WALKERS).  Measured on B200 (profiles/r02i_bench_w1.json / _w2.json, forward-only Render of the
-  // headline batch): one walker per CTA (4 per SM, 110 registers) 2.11 ms, two (6 per SM, 80 registers: fewer gathers in flight per
-  // thread) 2.57 ms — the default is one.
+  // ray walkers per CTA (F2B_FUSED_WALKERS): the default is one.
   static int walkers = -1;
   if (walkers < 0) { const char* e = getenv("F2B_FUSED_WALKERS"); walkers = (e && atoi(e) == 2) ? 2 : 1; }
-#define F2B_FUSED_LAUNCH(NW, PER_SM)                                                                                              \
+#define F2B_FUSED_LAUNCH(NW)                                                                                                      \
   {                                                                                                                               \
-    const int want = div_up(n_rays, NW);                                                                                          \
-    const int grid = want < sms * PER_SM ? want : sms * PER_SM;                                                                   \
     cudaFuncSetAttribute(render_fwd_fused_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem<NW>::BYTES);        \
+    const int per_sm = resident_per_sm(render_fwd_fused_kernel<NW>, kRT * NW, FusedSmem<NW>::BYTES);                              \
+    const int want = div_up(n_rays, NW);                                                                                          \
+    const int grid = want < sms * per_sm ? want : sms * per_sm;                                                                   \
     render_fwd_fused_kernel<NW><<<grid, kRT * NW, FusedSmem<NW>::BYTES, as_stream(stream)>>>(                                     \
         (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,                  \
         (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,    \
         total_all, ticket, colors, disparity, depth, kept_counts, weights_slots);                                                 \
   }
-  if (walkers == 2) F2B_FUSED_LAUNCH(2, 3) else F2B_FUSED_LAUNCH(1, 4)
+  if (walkers == 2) F2B_FUSED_LAUNCH(2) else F2B_FUSED_LAUNCH(1)
 #undef F2B_FUSED_LAUNCH
   return check_launch("f2b_render_fwd_fused");
 }

@@ -1,16 +1,16 @@
-// hash.cu — anchored multi-level hash-grid encode (forward gather, backward scatter) for sm_100a.
+// hash.cu — anchored multi-level hash-grid encode (forward gather, backward scatter) for sm_90a.
 //
 // Replaces Hash3DAnchoredForwardKernel / Hash3DAnchoredBackwardKernel
 // (src/Field/Hash3DAnchored.cu:11-155) and the per-call dtype passes of
 // Hash3DAnchoredFunction::forward/backward (:160-233) and Hash3DAnchored::AnchoredQuery's
 // (pts+1)/2 (src/Field/Hash3DAnchored.cpp:91).
 //
-// B200 design: one thread owns one sample for all 16 levels (the reference launches 16 grid.y
+// Design: one thread owns one sample for all 16 levels (the reference launches 16 grid.y
 // passes that each re-read the point), lanes of a warp hold 32 consecutive samples of (mostly)
 // one ray so the coarse levels' corners coalesce into the same 32 B sectors in L1; the 8 corner
 // loads of a level are issued back to back (8-16 independent 4 B half2 gathers in flight per
 // thread), the 32 encoded halfs leave as four 128-bit stores.  The fp16 table (17 MB live at
-// log2 19) is L2 resident on B200, so the bound is L2->SM sector throughput, not HBM.
+// log2 19) is L2 resident in H100's 50 MB L2, so the bound is L2->SM sector throughput, not HBM.
 // The blend reproduces the reference build's exact fp32 sequence (read off its PTX):
 //   acc = w001*f001; acc = fma(w000,f000,acc); then fma in order 010,011,100,101,110,111.
 #include "common.cuh"
@@ -73,7 +73,7 @@ constexpr int kDirectHeads = 24;
 
 // The grid is PERSISTENT and bounded (ctas_per_sm x SM count CTAs striding over the (32 samples, level) tasks): a few resident
 // warps per SM already saturate the reduction pipe, and a bounded grid lets the scatter of one ray chunk run on a side stream
-// next to the tcgen05 kernels of the next chunk without crowding their CTAs out (an unbounded grid of 260 k small blocks did).
+// next to the tensor-core kernels of the next chunk without crowding their CTAs out (an unbounded grid of 260 k small blocks did).
 template <bool GRAD_F16>
 __device__ __forceinline__ void hash_bwd_task(int64_t group, int l, int lane, const int* __restrict__ prim_pool,
                                               const float* __restrict__ bias_pool, int n_volumes, int local_size,
@@ -227,7 +227,7 @@ extern "C" int f2b_hash_bwd_levels(const int* prim_pool, const float* bias_pool,
   const int64_t n_tasks = int64_t(div_up(n_pts, 32)) * n_levels;           // one warp-task per (32 samples, level)
   static int ctas_per_sm = -1;                                             // resident 256-thread CTAs per SM (F2B_SCATTER_CTAS, default 8 = all)
   if (ctas_per_sm < 0) { const char* e = getenv("F2B_SCATTER_CTAS"); ctas_per_sm = e ? atoi(e) : 8; if (ctas_per_sm < 1) ctas_per_sm = 1; }
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int64_t want = div_up(n_tasks * 32, int64_t(256));
   int blocks = int(want < int64_t(sms) * ctas_per_sm ? want : int64_t(sms) * ctas_per_sm);

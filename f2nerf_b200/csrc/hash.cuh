@@ -1,5 +1,5 @@
 // hash.cuh — device functions of the anchored hash-grid encode shared by hash.cu (stand-alone encode)
-// and field.cu (encode fused in front of the tcgen05 MLP).  See hash.cu for the design notes.
+// and field.cu (encode fused in front of the wgmma MLP).  See hash.cu for the design notes.
 #pragma once
 #include "common.cuh"
 

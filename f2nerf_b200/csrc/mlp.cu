@@ -7,7 +7,7 @@
 //
 // This file is the CUDA-core implementation (impl 0): fp16 operands, fp32 accumulation, hidden
 // activations and outputs rounded to fp16 exactly where tiny-cuda-nn stores them.  It is the
-// validation twin of the tcgen05/TMEM kernels in mlp_tc.cu (impl 1) and shares their C ABI.
+// validation twin of the wgmma tensor-core kernels in mlp_tc.cu (impl 1) and shares their C ABI.
 // Parameter layout (fully_fused_mlp.cu:654-677): [W0 64x32 | Wh 64x64 (x n_hidden_matmuls) | Wout 16x64],
 // row-major [out][in], fp16.
 #include "common.cuh"
@@ -311,7 +311,7 @@ extern "C" int f2b_mlp_fwd_v0(const void* in_f16, const void* params_f16, int n_
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(in_f16 && params_f16 && out_f16, "f2b_mlp_fwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_fwd: n_hidden_matmuls must be 0 or 1");
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kTile);
   const int grid = n_tiles < sms * 8 ? n_tiles : sms * 8;
@@ -334,7 +334,7 @@ extern "C" int f2b_mlp_bwd2_v0(const void* dout_f16, const void* in_f16, const v
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(dout_f16 && in_f16 && hidden0_f16 && params_f16 && dparams_f32, "f2b_mlp_bwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || (n_hidden_matmuls == 1 && hidden1_f16), "f2b_mlp_bwd: n_hidden_matmuls must be 0 or 1 (with hidden1)");
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kTile);
   const int grid = n_tiles < sms * 2 ? n_tiles : sms * 2;

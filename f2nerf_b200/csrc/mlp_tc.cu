@@ -1,23 +1,25 @@
-// mlp_tc.cu — the fully-fused MLP on Blackwell's 5th-generation tensor cores (impl 1).
+// mlp_tc.cu — the fully-fused MLP on Hopper's warpgroup tensor-core instructions (impl 1).
 //
 // Replaces tiny-cuda-nn's wmma 16x16x16 fp16-accumulate kernels (kernel_mlp_fused /
 // kernel_mlp_fused_backward, External/tiny-cuda-nn/src/fully_fused_mlp.cu:150-259,499-557) with
-// tcgen05.mma (UMMA M128 x N{64,16} x K16, fp16 operands, fp32 accumulators in TMEM):
-//   * one CTA (4 warps) owns a 128-sample tile; thread i == sample i == TMEM lane i;
+// wgmma.mma_async (two m64 x N{64,16} x k16 per K step, fp16 operands from shared memory, fp32 accumulators
+// in registers):
+//   * one CTA (4 warps = one warpgroup) owns a 128-sample tile;
 //   * the layer input is written to shared memory in the canonical K-major swizzled layout
 //     (64 B rows / SWIZZLE_64B for K=32, 128 B rows / SWIZZLE_128B for K=64), the weights sit
 //     resident in shared memory in the same layouts for the CTA's lifetime (persistent tiles);
-//   * one elected thread issues K/16 MMAs per layer and commits to an mbarrier; all 128 threads then
-//     pull their accumulator row out of TMEM with tcgen05.ld (32x32b), apply ReLU, round to fp16 and
-//     write the next layer's operand row straight back to shared memory — activations never visit HBM
-//     except for the optional hidden_save the backward pass needs;
+//   * the warpgroup issues 2*K/16 wgmmas per layer, waits for them, applies ReLU to its accumulator
+//     fragments, rounds to fp16 and writes them straight back to shared memory as the next layer's operand
+//     tile — activations never visit HBM except for the optional hidden_save the backward pass needs;
+//   * the 16 outputs of a sample are gathered into one thread (thread i == sample i) through an fp32 row
+//     buffer in shared memory, so the epilogues below work on whole rows;
 //   * global traffic is decoupled from the per-thread row ownership: the next tile's input is fetched with
 //     cp.async (16 B per thread, linear sweep of the contiguous 8 KB tile) into the second half of a double
 //     buffer while the current tile computes, and each finished activation tile is copied out to hidden_save
 //     by all threads as whole 128 B lines WHILE the tensor core is consuming the same tile for the next layer
 //     (r01 profile: per-row 16 B stores at 128 B stride + exposed load latency were ~50 % of the stall samples);
-//   * TMEM: 64 columns per CTA (the 16-column output accumulator reuses the hidden one); 3 (NH=1) or 5 (NH=0)
-//     CTAs share an SM (shared-memory bound) and overlap each other's MMA round trips.
+//   * several CTAs share an SM (as many as registers and shared memory allow) and overlap each other's MMA
+//     round trips.
 #include "common.cuh"
 #include "tc.cuh"
 #include "shader.cuh"
@@ -26,7 +28,6 @@ namespace f2b {
 using namespace tc;
 
 constexpr int kTcTile = 128;
-constexpr int kTmemCols = 64;
 
 template <int NH>
 struct TcSmem {                         // offsets from a 1024-byte aligned base
@@ -36,8 +37,7 @@ struct TcSmem {                         // offsets from a 1024-byte aligned base
   static constexpr int W0 = NH ? 49152 : 32768;   // [64 x 32]  f16, SW64   (4 KB)
   static constexpr int WH = W0 + 4096;            // [64 x 64]  f16, SW128  (8 KB, NH only)
   static constexpr int WO = WH + (NH ? 8192 : 0); // [16 x 64]  f16, SW128  (2 KB)
-  static constexpr int BAR = WO + 2048;           // mbarrier (8 B) + tmem base (4 B)
-  static constexpr int BYTES = BAR + 64 + 1024;   // + alignment slack
+  static constexpr int BYTES = WO + 2048 + 1024;  // + alignment slack
 };
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
@@ -88,27 +88,6 @@ __device__ __forceinline__ void copy_out_hidden(const unsigned char* h_tile, __h
   }
 }
 
-// accumulator row (64 fp32 in TMEM) -> ReLU -> fp16 -> my row of the next operand tile
-__device__ __forceinline__ void relu_epilogue(uint32_t tmem_row, unsigned char* h_tile, int row) {
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    uint32_t r[16];
-    tmem_ld16(tmem_row + 16 * q, r);
-    tmem_ld_wait();
-    uint4 v0, v1;
-    v0.x = pack_half2(fmaxf(__uint_as_float(r[0]), 0.f), fmaxf(__uint_as_float(r[1]), 0.f));
-    v0.y = pack_half2(fmaxf(__uint_as_float(r[2]), 0.f), fmaxf(__uint_as_float(r[3]), 0.f));
-    v0.z = pack_half2(fmaxf(__uint_as_float(r[4]), 0.f), fmaxf(__uint_as_float(r[5]), 0.f));
-    v0.w = pack_half2(fmaxf(__uint_as_float(r[6]), 0.f), fmaxf(__uint_as_float(r[7]), 0.f));
-    v1.x = pack_half2(fmaxf(__uint_as_float(r[8]), 0.f), fmaxf(__uint_as_float(r[9]), 0.f));
-    v1.y = pack_half2(fmaxf(__uint_as_float(r[10]), 0.f), fmaxf(__uint_as_float(r[11]), 0.f));
-    v1.z = pack_half2(fmaxf(__uint_as_float(r[12]), 0.f), fmaxf(__uint_as_float(r[13]), 0.f));
-    v1.w = pack_half2(fmaxf(__uint_as_float(r[14]), 0.f), fmaxf(__uint_as_float(r[15]), 0.f));
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q)) = v0;
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q + 1)) = v1;
-  }
-}
-
 // Work that follows (or precedes) the MLP in Renderer::Render, done in its output epilogue while the row is in registers:
 //   EPI_SHADE (field MLP, NH = 0): the shading-feature assembly of Renderer.cpp:179-187 + SHShader.cpp:23-26 — the thread
 //     turns its 16 outputs into the shader MLP's fp16 input row ([1, feat 1..15] + appearance embedding | SH4(dir)) and
@@ -131,30 +110,23 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
   using S = TcSmem<NH>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(sm + S::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + S::BAR + 8);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  float* s_rows = reinterpret_cast<float*>(sm + S::H0);             // output rows [128][20] fp32 (H0 is dead by then)
+  const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kTcTile - 1) / kTcTile;
   const uint32_t a0 = smem_u32(sm + S::A0);
 
   int tile = blockIdx.x;
-  if (tile < n_tiles) prefetch_input(in, tile, n_pts, a0);       // overlaps the weight staging / TMEM allocation
+  if (tile < n_tiles) prefetch_input(in, tile, n_pts, a0);       // overlaps the weight staging
   cp_async_commit();
   stage_weights<32>(params, 64, sm + S::W0);
   if (NH) stage_weights<64>(params + 64 * 32, 64, sm + S::WH);
   stage_weights<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
-  if (tid == 0) mbar_init(mbar, 1);
-  if (warp == 0) tmem_alloc(tmem_slot, kTmemCols);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_row = tmem + (uint32_t(warp * 32) << 16);   // this warp's 32 TMEM lanes
 
   const uint32_t h0 = smem_u32(sm + S::H0), h1 = smem_u32(sm + S::H1);
   const uint32_t w0 = smem_u32(sm + S::W0), wh = smem_u32(sm + S::WH), wo = smem_u32(sm + S::WO);
-  constexpr uint32_t idesc64 = idesc_f16_f32(128, 64), idesc16 = idesc_f16_f32(128, 16);
-  uint32_t phase = 0, buf = 0;
+  uint32_t buf = 0;
+  Acc<64> acc;
+  Acc<16> acc_out;
 
   for (; tile < n_tiles; tile += gridDim.x, buf ^= 1) {
     const int p = tile * kTcTile + tid;
@@ -165,56 +137,38 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
     cp_async_commit();
     cp_async_wait<1>();                                          // everything but the newest group has landed
     fence_async_smem();
-    fence_before_sync();                                         // (the previous tile's TMEM reads are done)
-    __syncthreads();
+    __syncthreads();                                             // (also: the previous tile's output rows have been read)
     // ---- layer 0: D[128x64] = A0[128x32] . W0^T ------------------------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-      const uint32_t a = a0 + buf * 8192;
-#pragma unroll
-      for (int k = 0; k < 2; k++)
-        mma_f16(tmem, kmajor_desc(a + 32 * k, 64), kmajor_desc(w0 + 32 * k, 64), idesc64, k);
-      mma_commit(mbar);
-    }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-    relu_epilogue(tmem_row, sm + S::H0, tid);
-    fence_before_sync();
+    wg_fence();
+    mma_m128<64, 0, 2>(acc, a0 + buf * 8192, 64, w0, 64, false);
+    wg_commit();
+    wg_wait();
+    acc_relu_to_tile(acc, sm + S::H0, tid);
     fence_async_smem();
     __syncthreads();
     if (NH) {
       // ---- hidden layer: D[128x64] = H0[128x64] . Wh^T ---------------------------------------------
-      if (tid == 0) {
-        fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-          mma_f16(tmem, kmajor_desc(h0 + 32 * k, 128), kmajor_desc(wh + 32 * k, 128), idesc64, k);
-        mma_commit(mbar);
-      }
+      wg_fence();
+      mma_m128<64, 0, 4>(acc, h0, 128, wh, 128, false);
+      wg_commit();
       if (hidden_save) copy_out_hidden(sm + S::H0, hidden_save, tile, n_pts);        // while the MMA runs
-      mbar_wait(mbar, phase); phase ^= 1;
-      fence_after_sync();
-      relu_epilogue(tmem_row, sm + S::H1, tid);
-      fence_before_sync();
+      wg_wait();
+      acc_relu_to_tile(acc, sm + S::H1, tid);
       fence_async_smem();
       __syncthreads();
     }
     // ---- output layer: D[128x16] = H_last[128x64] . Wout^T (linear) ----------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-      const uint32_t hl = NH ? h1 : h0;
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-        mma_f16(tmem, kmajor_desc(hl + 32 * k, 128), kmajor_desc(wo + 32 * k, 128), idesc16, k);
-      mma_commit(mbar);
-    }
+    wg_fence();
+    mma_m128<16, 0, 4>(acc_out, NH ? h1 : h0, 128, wo, 128, false);
+    wg_commit();
     if (hidden_save) copy_out_hidden(sm + (NH ? S::H1 : S::H0), hidden_save + size_t(NH) * n_pts * 64, tile, n_pts);
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
+    wg_wait();
+    __syncthreads();                                             // every warp is done with H0 (operand / copy-out)
+    acc_to_rows(acc_out, s_rows, kRowLd16, tid);
+    __syncthreads();
     {
       uint32_t r[16];
-      tmem_ld16(tmem_row, r);
-      tmem_ld_wait();
+      row_ld16(s_rows, kRowLd16, tid, r);
       if (valid) {
         uint4 v0, v1;
         v0.x = pack_half2(__uint_as_float(r[0]), __uint_as_float(r[1]));   v0.y = pack_half2(__uint_as_float(r[2]), __uint_as_float(r[3]));
@@ -278,12 +232,8 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
         __syncthreads();                                         // the stage is the next-but-one tile's prefetch target
       }
     }
-    // the next iteration's barrier orders these TMEM reads before the next tile's first MMA
   }
   cp_async_wait<0>();
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, kTmemCols);
 }
 
 }  // namespace f2b
@@ -293,12 +243,12 @@ using namespace f2b;
 template <int NH, int EPI>
 static void launch_fwd(const void* in_f16, const void* params_f16, int n_pts, void* out_f16, float* out_f32,
                        void* hidden_save_f16, const EpiArgs& epi, void* stream) {
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
-  const int per_sm = NH ? 3 : 5;                                  // shared-memory bound (63 KB / 39 KB per CTA)
+  cudaFuncSetAttribute(mlp_fwd_tc_kernel<NH, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<NH>::BYTES);
+  const int per_sm = resident_per_sm(mlp_fwd_tc_kernel<NH, EPI>, kTcTile, TcSmem<NH>::BYTES);
   const int n_tiles = div_up(n_pts, kTcTile);
   const int grid = n_tiles < sms * per_sm ? n_tiles : sms * per_sm;
-  cudaFuncSetAttribute(mlp_fwd_tc_kernel<NH, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<NH>::BYTES);
   mlp_fwd_tc_kernel<NH, EPI><<<grid, kTcTile, TcSmem<NH>::BYTES, as_stream(stream)>>>(
       (const __half*)in_f16, (const __half*)params_f16, n_pts, (__half*)out_f16, out_f32, (__half*)hidden_save_f16, epi);
 }
@@ -311,7 +261,7 @@ extern "C" int f2b_mlp_fwd_tc(const void* in_f16, const void* params_f16, int n_
   const EpiArgs none = {};
   if (n_hidden_matmuls == 0) launch_fwd<0, EPI_NONE>(in_f16, params_f16, n_pts, out_f16, nullptr, hidden_save_f16, none, stream);
   else launch_fwd<1, EPI_NONE>(in_f16, params_f16, n_pts, out_f16, nullptr, hidden_save_f16, none, stream);
-  return check_launch("f2b_mlp_fwd(tcgen05)");
+  return check_launch("f2b_mlp_fwd(wgmma)");
 }
 
 // Same network, output widened to fp32 in the epilogue (what TCNNWP::Query hands back, TCNNWP.cpp:112):
@@ -324,14 +274,14 @@ extern "C" int f2b_mlp_fwd_tc_f32(const void* in_f16, const void* params_f16, in
   const EpiArgs none = {};
   if (n_hidden_matmuls == 0) launch_fwd<0, EPI_NONE>(in_f16, params_f16, n_pts, out_f16, out_f32, hidden_save_f16, none, stream);
   else launch_fwd<1, EPI_NONE>(in_f16, params_f16, n_pts, out_f16, out_f32, hidden_save_f16, none, stream);
-  return check_launch("f2b_mlp_fwd_f32(tcgen05)");
+  return check_launch("f2b_mlp_fwd_f32(wgmma)");
 }
 
 // Field MLP (32 -> 64 -> 16) on encoded features + the shading-feature assembly in its epilogue:
 // logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])).
 extern "C" int f2b_get_mlp_impl(void);
 #define F2B_REQUIRE_TC(name)                                                                                   \
-  if (f2b_get_mlp_impl() != 1) { set_error(name ": needs the tcgen05 MLP implementation (F2B_MLP_IMPL=1)"); return F2B_EUNSUPPORTED; }
+  if (f2b_get_mlp_impl() != 1) { set_error(name ": needs the tensor-core MLP implementation (F2B_MLP_IMPL=1)"); return F2B_EUNSUPPORTED; }
 
 extern "C" int f2b_field_shade_fwd(const void* feat_f16, const void* field_params_f16, const float* dirs, const float* app_emb,
                                    const int* pt_emb_idx, int n_pts, float* logit, void* mlp_in_f16, void* hidden_save_f16,

@@ -1,16 +1,15 @@
-// mlp_tc_bwd.cu — MLP backward on tcgen05 tensor cores (impl 1).
+// mlp_tc_bwd.cu — MLP backward on Hopper wgmma tensor cores (impl 1).
 //
 // Replaces kernel_mlp_fused_backward (External/tiny-cuda-nn/src/fully_fused_mlp.cu:150-259), the CUTLASS
 // dL/dinput GEMM (:832-835) and the three split-K weight-gradient GEMMs on side streams (:785,819,828)
-// with ONE persistent kernel per call.  Per 128-sample tile (thread i == sample i == TMEM lane i):
-//   activation gradients  dH = dOut.Wout, dH0 = dH1.Wh, dIn = dH0.W0   — UMMA M128, A = K-major tile of the
+// with ONE persistent kernel per call (one warpgroup per CTA).  Per 128-sample tile:
+//   activation gradients  dH = dOut.Wout, dH0 = dH1.Wh, dIn = dH0.W0   — two m64 wgmmas, A = K-major tile of the
 //       gradient rows, B = the weight matrix used as MN-major operand straight from its row-major layout
 //       (no transposed weight copies);
-//   weight gradients      dW = dAct^T . Act  — batch-reduction UMMAs with K = the 128 samples of the tile:
+//   weight gradients      dW = dAct^T . Act  — batch-reduction wgmmas with K = the 128 samples of the tile:
 //       both operands MN-major views of the very same shared-memory tiles, M = 64 output rows, fp32
-//       accumulators that stay resident in TMEM across all tiles of the CTA and are flushed once with
+//       accumulators that stay resident in registers across all tiles of the CTA and are flushed once with
 //       atomicAdd at the end (no split-K workspace, no fp16 accumulation, no reduction kernels).
-// TMEM columns: [0,64) activation-gradient accumulator, then dW0 (32), dWout^T (16), dWh (64 when NH).
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -33,21 +32,12 @@ struct BwdSmem {
   static constexpr int H0 = 12288;                          //                 [128 x 64] SW128 16 KB (becomes dH0)
   static constexpr int H1 = 28672;                          //                 [128 x 64] SW128 16 KB (becomes dH1; NH only)
   static constexpr int STAGE_BYTES = NH ? 45056 : 28672;
-  static constexpr int BAR = STAGE0 + 2 * STAGE_BYTES;
-  static constexpr int BYTES = BAR + 64 + 1024;
-  static constexpr int TMEM_COLS = NH ? 256 : 128;
-  static constexpr int C_ACT = 0, C_GW0 = 64, C_GWO = 96, C_GWH = 128;
+  static constexpr int BYTES = STAGE0 + 2 * STAGE_BYTES + 1024;
 };
 
 __device__ __forceinline__ uint32_t pk(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
-}
-
-// MN-major operand: tile of [k rows][row_bytes] with matching swizzle; k-step = 16 rows
-__device__ __forceinline__ uint64_t mnmajor_desc(uint32_t tile, int row_bytes, int k_step) {
-  const uint64_t layout = row_bytes == 128 ? kLayoutSW128 : (row_bytes == 64 ? kLayoutSW64 : kLayoutSW32);
-  return make_desc(tile + k_step * 16 * row_bytes, 16, 8 * row_bytes, layout);
 }
 
 template <int K>
@@ -97,26 +87,49 @@ __device__ __forceinline__ void prefetch_tile(const __half* __restrict__ dout, c
   }
 }
 
-// masked epilogue: acc (64 fp32 from TMEM) * [h > 0] -> fp16 row of the dH tile (SW128)
-__device__ __forceinline__ void relu_bwd_epilogue(uint32_t tmem_row, const unsigned char* h_tile, unsigned char* dh_tile, int row) {
+// masked epilogue: acc * [h > 0] -> fp16 dH tile (SW128); h_tile may be dh_tile (each element is read, then written, by one thread)
+__device__ __forceinline__ void relu_bwd_epilogue(const Acc<64>& acc, const unsigned char* h_tile, unsigned char* dh_tile, int t) {
 #pragma unroll
-  for (int q = 0; q < 4; q++) {
-    uint32_t r[16];
-    tmem_ld16(tmem_row + 16 * q, r);
-    tmem_ld_wait();
-    uint4 hv[2], o[2];
-    hv[0] = *reinterpret_cast<const uint4*>(h_tile + sw128_off(row, 2 * q));
-    hv[1] = *reinterpret_cast<const uint4*>(h_tile + sw128_off(row, 2 * q + 1));
-    const __half2* hh = reinterpret_cast<const __half2*>(hv);
-    uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+  for (int h = 0; h < 2; h++)
 #pragma unroll
-    for (int e = 0; e < 8; e++) {
-      const float2 hf = __half22float2(hh[e]);
-      ow[e] = pk(hf.x > 0.f ? __uint_as_float(r[2 * e]) : 0.f, hf.y > 0.f ? __uint_as_float(r[2 * e + 1]) : 0.f);
+    for (int i = 0; i < 32; i += 2) {
+      const uint32_t off = sw128_col(acc_row(t, h, i), acc_col(t, i));
+      const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(h_tile + off));
+      *reinterpret_cast<uint32_t*>(dh_tile + off) = pk(hf.x > 0.f ? acc.d[h][i] : 0.f, hf.y > 0.f ? acc.d[h][i + 1] : 0.f);
     }
-    *reinterpret_cast<uint4*>(dh_tile + sw128_off(row, 2 * q)) = o[0];
-    *reinterpret_cast<uint4*>(dh_tile + sw128_off(row, 2 * q + 1)) = o[1];
-  }
+}
+
+// dIn rows of the tile -> global fp16 [P,32]
+__device__ __forceinline__ void store_din(const Acc<32>& acc, __half* __restrict__ din, int tile, int n_pts, int t) {
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int i = 0; i < 16; i += 2) {
+      const int p = tile * kBT + acc_row(t, h, i);
+      if (p < n_pts) *reinterpret_cast<uint32_t*>(din + size_t(p) * 32 + acc_col(t, i)) = pk(acc.d[h][i], acc.d[h][i + 1]);
+    }
+}
+
+// weight-gradient accumulators (rows = output features) -> dparams with atomicAdd; dWout is held transposed
+template <int NH>
+__device__ __forceinline__ void flush_weight_grads(const Acc64<32>& gw0, const Acc64<16>& gwo, const Acc64<64>& gwh,
+                                                   float* __restrict__ dparams, int t) {
+  float* g0 = dparams;
+  float* gh = dparams + 64 * 32;
+  float* go = gh + NH * 64 * 64;
+#pragma unroll
+  for (int i = 0; i < 16; i++) atomicAdd(g0 + acc_row(t, 0, i) * 32 + acc_col(t, i), gw0.d[i]);
+#pragma unroll
+  for (int i = 0; i < 8; i++) atomicAdd(go + acc_col(t, i) * 64 + acc_row(t, 0, i), gwo.d[i]);
+  if (NH)
+#pragma unroll
+    for (int i = 0; i < 32; i++) atomicAdd(gh + acc_row(t, 0, i) * 64 + acc_col(t, i), gwh.d[i]);
+}
+
+template <int N>
+__device__ __forceinline__ void zero(Acc64<N>& a) {
+#pragma unroll
+  for (int i = 0; i < N / 2; i++) a.d[i] = 0.f;
 }
 
 template <int NH>
@@ -127,9 +140,7 @@ mlp_bwd_tc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
   using S = BwdSmem<NH>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(sm + S::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + S::BAR + 8);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kBT - 1) / kBT;
   const uint32_t stage0 = smem_u32(sm + S::STAGE0);
 
@@ -139,160 +150,76 @@ mlp_bwd_tc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
   stage_w<32>(params, 64, sm + S::W0);
   if (NH) stage_w<64>(params + 64 * 32, 64, sm + S::WH);
   stage_w<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
-  if (tid == 0) mbar_init(mbar, 1);
-  if (warp == 0) tmem_alloc(tmem_slot, S::TMEM_COLS);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_row = tmem + (uint32_t(warp * 32) << 16);
   const uint32_t s_w0 = smem_u32(sm + S::W0), s_wh = smem_u32(sm + S::WH), s_wo = smem_u32(sm + S::WO);
-  // instruction descriptors
-  constexpr uint32_t id_act64 = idesc_f16_f32(128, 64, 0, 1);     // A K-major, B MN-major
-  constexpr uint32_t id_act32 = idesc_f16_f32(128, 32, 0, 1);
-  constexpr uint32_t id_gw16 = idesc_f16_f32(64, 16, 1, 1);       // both MN-major
-  constexpr uint32_t id_gw32 = idesc_f16_f32(64, 32, 1, 1);
-  constexpr uint32_t id_gw64 = idesc_f16_f32(64, 64, 1, 1);
-  uint32_t phase = 0, first = 1, buf = 0;
+  Acc<64> act;
+  Acc<32> act_in;
+  Acc64<32> gw0;
+  Acc64<16> gwo;
+  Acc64<64> gwh;
+  zero(gw0); zero(gwo); zero(gwh);
+  const bool any = tile < n_tiles;
+  uint32_t buf = 0;
 
   for (; tile < n_tiles; tile += gridDim.x, buf ^= 1) {
-    const int p = tile * kBT + tid;
-    const bool valid = p < n_pts;
+    __syncthreads();                                             // every warp's MMAs are done with the stage refilled below
     const int next = tile + gridDim.x;
     if (next < n_tiles) prefetch_tile<NH>(dout, in, hidden, hid_last, next, n_pts, stage0 + (buf ^ 1) * S::STAGE_BYTES);
     asm volatile("cp.async.commit_group;" ::: "memory");
     asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
     fence_async_smem();
-    fence_before_sync();
     __syncthreads();
     unsigned char* const st = sm + S::STAGE0 + buf * S::STAGE_BYTES;
     const uint32_t sb = stage0 + buf * S::STAGE_BYTES;
     const uint32_t s_do = sb + S::DO, s_x = sb + S::X, s_h0 = sb + S::H0, s_h1 = sb + S::H1;
     const uint32_t s_hl = NH ? s_h1 : s_h0;
-    const uint32_t acc = (first ^ 1);
     // ---- A: dH_last = dOut . Wout  (K = 16) ; dWout^T += H_last^T . dOut (needs H_last before it is overwritten)
-    if (tid == 0) {
-      fence_after_sync();
-      mma_f16(tmem + S::C_ACT, kmajor_desc(s_do, 32), mnmajor_desc(s_wo, 128, 0), id_act64, 0);
-#pragma unroll
-      for (int k = 0; k < 8; k++)
-        mma_f16(tmem + S::C_GWO, mnmajor_desc(s_hl, 128, k), mnmajor_desc(s_do, 32, k), id_gw16, (k > 0) | acc);
-      mma_commit(mbar);
-    }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-    relu_bwd_epilogue(tmem_row + S::C_ACT, st + (NH ? S::H1 : S::H0), st + (NH ? S::H1 : S::H0), tid);   // in place
-    fence_before_sync();
+    wg_fence();
+    mma_m128<64, 1, 1>(act, s_do, 32, s_wo, 128, false);
+    mma_batch128<16>(gwo, s_hl, 128, s_do, 32);
+    wg_commit();
+    wg_wait();
+    __syncthreads();                                             // every warp's MMAs are done reading H_last
+    relu_bwd_epilogue(act, st + (NH ? S::H1 : S::H0), st + (NH ? S::H1 : S::H0), tid);   // in place
     fence_async_smem();
     __syncthreads();
     if (NH) {
       // ---- B: dH0 = dH1 . Wh ; dWh += dH1^T . H0 (H0 still the forward activation) ---------------------
-      if (tid == 0) {
-        fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-          mma_f16(tmem + S::C_ACT, kmajor_desc(s_h1 + 32 * k, 128), mnmajor_desc(s_wh, 128, k), id_act64, k);
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          mma_f16(tmem + S::C_GWH, mnmajor_desc(s_h1, 128, k), mnmajor_desc(s_h0, 128, k), id_gw64, (k > 0) | acc);
-        mma_commit(mbar);
-      }
-      mbar_wait(mbar, phase); phase ^= 1;
-      fence_after_sync();
-      relu_bwd_epilogue(tmem_row + S::C_ACT, st + S::H0, st + S::H0, tid);                                  // in place
-      fence_before_sync();
+      wg_fence();
+      mma_m128<64, 1, 4>(act, s_h1, 128, s_wh, 128, false);
+      mma_batch128<64>(gwh, s_h1, 128, s_h0, 128);
+      wg_commit();
+      wg_wait();
+      __syncthreads();
+      relu_bwd_epilogue(act, st + S::H0, st + S::H0, tid);                                                  // in place
       fence_async_smem();
       __syncthreads();
     }
     // ---- C: dIn = dH0 . W0 ; dW0 += dH0^T . X -----------------------------------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-        mma_f16(tmem + S::C_ACT, kmajor_desc(s_h0 + 32 * k, 128), mnmajor_desc(s_w0, 64, k), id_act32, k);
-#pragma unroll
-      for (int k = 0; k < 8; k++)
-        mma_f16(tmem + S::C_GW0, mnmajor_desc(s_h0, 128, k), mnmajor_desc(s_x, 64, k), id_gw32, (k > 0) | acc);
-      mma_commit(mbar);
-    }
-    first = 0;
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-    {
-#pragma unroll
-      for (int q = 0; q < 2; q++) {
-        uint32_t r[16];
-        tmem_ld16(tmem_row + S::C_ACT + 16 * q, r);
-        tmem_ld_wait();
-        if (din && valid) {
-          uint4 o[2];
-          uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-#pragma unroll
-          for (int e = 0; e < 8; e++) ow[e] = pk(__uint_as_float(r[2 * e]), __uint_as_float(r[2 * e + 1]));
-          uint4* dst = reinterpret_cast<uint4*>(din + size_t(p) * 32) + 2 * q;
-          dst[0] = o[0]; dst[1] = o[1];
-        }
-      }
-    }
-    // the next iteration's barrier orders these TMEM reads before the next tile's first MMA
+    wg_fence();
+    mma_m128<32, 1, 4>(act_in, s_h0, 128, s_w0, 64, false);
+    mma_batch128<32>(gw0, s_h0, 128, s_x, 64);
+    wg_commit();
+    wg_wait();
+    if (din) store_din(act_in, din, tile, n_pts, tid);
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
-  fence_before_sync();
-  __syncthreads();
-  // ---- flush the weight-gradient accumulators (M = 64 layout: warp w, lanes 0..15 hold rows 16w..16w+15) ----
-  if (!first) {
-    fence_after_sync();
-    const int row = warp * 16 + lane;
-    float* g0 = dparams;
-    float* gh = dparams + 64 * 32;
-    float* go = gh + NH * 64 * 64;
-#pragma unroll
-    for (int q = 0; q < 2; q++) {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + S::C_GW0 + 16 * q, r);
-      tmem_ld_wait();
-      if (lane < 16)
-#pragma unroll
-        for (int e = 0; e < 16; e++) atomicAdd(g0 + row * 32 + 16 * q + e, __uint_as_float(r[e]));
-    }
-    {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + S::C_GWO, r);
-      tmem_ld_wait();
-      if (lane < 16)
-#pragma unroll
-        for (int e = 0; e < 16; e++) atomicAdd(go + e * 64 + row, __uint_as_float(r[e]));      // transposed back
-    }
-    if (NH) {
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        uint32_t r[16];
-        tmem_ld16(tmem_row + S::C_GWH + 16 * q, r);
-        tmem_ld_wait();
-        if (lane < 16)
-#pragma unroll
-          for (int e = 0; e < 16; e++) atomicAdd(gh + row * 64 + 16 * q + e, __uint_as_float(r[e]));
-      }
-    }
-    fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, S::TMEM_COLS);
+  if (any) flush_weight_grads<NH>(gw0, gwo, gwh, dparams, tid);
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Recompute variant (hidden0 == NULL in f2b_mlp_bwd2): the forward pass saves NO hidden activations — 128 B (field) /
 // 256 B (shader) per sample it no longer writes and this kernel no longer reads.  The tile's activations are rebuilt on
-// the tensor pipe from the 64 B input row (same UMMAs, same operands, same fp16 rounding as mlp_fwd_tc_kernel => the
-// very same bits the forward would have saved), then the backward proceeds as above.  r01 profile: these kernels were
-// HBM-bound at 0.6-0.87 of peak with the tensor pipe 6-19 % busy — the recompute rides on idle MMA issue slots.
+// the tensor pipe from the 64 B input row (same MMAs, same operands, same fp16 rounding as mlp_fwd_tc_kernel => the
+// very same bits the forward would have saved), then the backward proceeds as above: the saved-activation kernels are
+// bound by HBM traffic with the tensor pipe mostly idle, so the recompute rides on idle MMA issue slots.
 // Per sample: 32 (dOut) + 64 (x) B read, 64 B written  (was 224 / 352 B read).
 //   NH = 0:  F0  H0 = relu(X.W0^T)                                  -> H0 tile
 //            A   dH0 = (dOut.Wout) * [H0 > 0] ; dWout^T += H0^T.dOut -> dH0 over H0
 //            C   dX = dH0.W0 ; dW0 += dH0^T.X
-//   NH = 1:  F0  H0 = relu(X.W0^T)  and, into a second accumulator,  G = dOut.Wout   (independent of F0: one round trip)
-//            F1  H1 = relu(H0.Wh^T) -> H1 tile ;  dH1 = G * [H1 > 0]  -> D1 tile   (same epilogue, both rows in registers)
+//   NH = 1:  F0  H0 = relu(X.W0^T)
+//            F1  H1 = relu(H0.Wh^T) -> H1 tile
+//            G   dH1 = (dOut.Wout) * [H1 > 0]  -> D1 tile   (the mask tests the fp16 H1 tile the forward would have saved)
 //            B   dWout^T += H1^T.dOut ; dH0 = (dH1.Wh) * [H0 > 0] ; dWh += dH1^T.H0 -> dH0 over H0
 //            C   dX = dH0.W0 ; dW0 += dH0^T.X
 template <int NH>
@@ -307,10 +234,7 @@ struct RcSmem {
   static constexpr int DO = 0;                              // stage-relative: [128 x 16] SW32 4 KB
   static constexpr int X = 4096;                            //                 [128 x 32] SW64 8 KB
   static constexpr int STAGE_BYTES = 12288;
-  static constexpr int BAR = STAGE0 + 2 * STAGE_BYTES;
-  static constexpr int BYTES = BAR + 64 + 1024;
-  static constexpr int TMEM_COLS = NH ? 256 : 128;
-  static constexpr int C_ACT = 0, C_GW0 = 64, C_GWO = 96, C_GWH = 128, C_ACT2 = 192;
+  static constexpr int BYTES = STAGE0 + 2 * STAGE_BYTES + 1024;
 };
 
 template <int NH>
@@ -335,48 +259,6 @@ __device__ __forceinline__ void prefetch_tile_rc(const __half* __restrict__ dout
   }
 }
 
-// forward epilogue: acc (64 fp32) -> ReLU -> fp16 -> my row of the H tile
-__device__ __forceinline__ void relu_fwd_epilogue(uint32_t tmem_row, unsigned char* h_tile, int row) {
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    uint32_t r[16];
-    tmem_ld16(tmem_row + 16 * q, r);
-    tmem_ld_wait();
-    uint4 o[2];
-    uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; e++) ow[e] = pk(fmaxf(__uint_as_float(r[2 * e]), 0.f), fmaxf(__uint_as_float(r[2 * e + 1]), 0.f));
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q)) = o[0];
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q + 1)) = o[1];
-  }
-}
-
-// forward + masked-gradient epilogue: h = fp16(relu(acc)) -> H tile ; g * [h > 0] -> fp16 -> D tile (the mask tests the ROUNDED
-// activation, like relu_bwd_epilogue reading the saved fp16 tile)
-__device__ __forceinline__ void relu_fwd_mask_epilogue(uint32_t tmem_h, uint32_t tmem_g, unsigned char* h_tile, unsigned char* d_tile, int row) {
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    uint32_t r[16], g[16];
-    tmem_ld16(tmem_h + 16 * q, r);
-    tmem_ld16(tmem_g + 16 * q, g);
-    tmem_ld_wait();
-    uint4 o[2], d[2];
-    uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-    uint32_t* dw = reinterpret_cast<uint32_t*>(d);
-#pragma unroll
-    for (int e = 0; e < 8; e++) {
-      const __half2 h = __floats2half2_rn(fmaxf(__uint_as_float(r[2 * e]), 0.f), fmaxf(__uint_as_float(r[2 * e + 1]), 0.f));
-      ow[e] = *reinterpret_cast<const uint32_t*>(&h);
-      const float2 hf = __half22float2(h);
-      dw[e] = pk(hf.x > 0.f ? __uint_as_float(g[2 * e]) : 0.f, hf.y > 0.f ? __uint_as_float(g[2 * e + 1]) : 0.f);
-    }
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q)) = o[0];
-    *reinterpret_cast<uint4*>(h_tile + sw128_off(row, 2 * q + 1)) = o[1];
-    *reinterpret_cast<uint4*>(d_tile + sw128_off(row, 2 * q)) = d[0];
-    *reinterpret_cast<uint4*>(d_tile + sw128_off(row, 2 * q + 1)) = d[1];
-  }
-}
-
 template <int NH>
 __global__ void __launch_bounds__(kBT)
 mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in, const __half* __restrict__ params, int n_pts,
@@ -384,9 +266,7 @@ mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
   using S = RcSmem<NH>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(sm + S::BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + S::BAR + 8);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kBT - 1) / kBT;
   const uint32_t stage0 = smem_u32(sm + S::STAGE0);
 
@@ -396,167 +276,80 @@ mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
   stage_w<32>(params, 64, sm + S::W0);
   if (NH) stage_w<64>(params + 64 * 32, 64, sm + S::WH);
   stage_w<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
-  if (tid == 0) mbar_init(mbar, 1);
-  if (warp == 0) tmem_alloc(tmem_slot, S::TMEM_COLS);
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_row = tmem + (uint32_t(warp * 32) << 16);
   const uint32_t s_w0 = smem_u32(sm + S::W0), s_wh = smem_u32(sm + S::WH), s_wo = smem_u32(sm + S::WO);
   const uint32_t s_h0 = smem_u32(sm + S::H0), s_h1 = smem_u32(sm + S::H1), s_d1 = smem_u32(sm + S::D1);
-  constexpr uint32_t id_fwd64 = idesc_f16_f32(128, 64);           // forward layers: both operands K-major
-  constexpr uint32_t id_act64 = idesc_f16_f32(128, 64, 0, 1);     // A K-major, B MN-major
-  constexpr uint32_t id_act32 = idesc_f16_f32(128, 32, 0, 1);
-  constexpr uint32_t id_gw16 = idesc_f16_f32(64, 16, 1, 1);       // both MN-major
-  constexpr uint32_t id_gw32 = idesc_f16_f32(64, 32, 1, 1);
-  constexpr uint32_t id_gw64 = idesc_f16_f32(64, 64, 1, 1);
-  uint32_t phase = 0, first = 1, buf = 0;
+  Acc<64> act;
+  Acc<32> act_in;
+  Acc64<32> gw0;
+  Acc64<16> gwo;
+  Acc64<64> gwh;
+  zero(gw0); zero(gwo); zero(gwh);
+  const bool any = tile < n_tiles;
+  uint32_t buf = 0;
 
   for (; tile < n_tiles; tile += gridDim.x, buf ^= 1) {
-    const int p = tile * kBT + tid;
-    const bool valid = p < n_pts;
+    __syncthreads();                                             // every warp's MMAs are done with the stage refilled below
     const int next = tile + gridDim.x;
     if (next < n_tiles) prefetch_tile_rc<NH>(dout, in, next, n_pts, stage0 + (buf ^ 1) * S::STAGE_BYTES);
     asm volatile("cp.async.commit_group;" ::: "memory");
     asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
     fence_async_smem();
-    fence_before_sync();
-    __syncthreads();
+    __syncthreads();                                             // (also: the previous tile's MMAs are done with H0 / H1 / D1)
     const uint32_t sb = stage0 + buf * S::STAGE_BYTES;
     const uint32_t s_do = sb + S::DO, s_x = sb + S::X;
-    const uint32_t acc = (first ^ 1);
-    // ---- F0: H0 = relu(X . W0^T)   (NH: and G = dOut . Wout into the second accumulator) ----------------
-    if (tid == 0) {
-      fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < 2; k++) mma_f16(tmem + S::C_ACT, kmajor_desc(s_x + 32 * k, 64), kmajor_desc(s_w0 + 32 * k, 64), id_fwd64, k);
-      if (NH) mma_f16(tmem + S::C_ACT2, kmajor_desc(s_do, 32), mnmajor_desc(s_wo, 128, 0), id_act64, 0);
-      mma_commit(mbar);
-    }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-    relu_fwd_epilogue(tmem_row + S::C_ACT, sm + S::H0, tid);
-    fence_before_sync();
+    // ---- F0: H0 = relu(X . W0^T) ---------------------------------------------------------------------------
+    wg_fence();
+    mma_m128<64, 0, 2>(act, s_x, 64, s_w0, 64, false);
+    wg_commit();
+    wg_wait();
+    acc_relu_to_tile(act, sm + S::H0, tid);
     fence_async_smem();
     __syncthreads();
     if (NH) {
-      // ---- F1: H1 = relu(H0 . Wh^T) ; dH1 = G * [H1 > 0] ------------------------------------------------
-      if (tid == 0) {
-        fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 4; k++) mma_f16(tmem + S::C_ACT, kmajor_desc(s_h0 + 32 * k, 128), kmajor_desc(s_wh + 32 * k, 128), id_fwd64, k);
-        mma_commit(mbar);
-      }
-      mbar_wait(mbar, phase); phase ^= 1;
-      fence_after_sync();
-      relu_fwd_mask_epilogue(tmem_row + S::C_ACT, tmem_row + S::C_ACT2, sm + S::H1, sm + S::D1, tid);
-      fence_before_sync();
+      // ---- F1: H1 = relu(H0 . Wh^T) ------------------------------------------------------------------------
+      wg_fence();
+      mma_m128<64, 0, 4>(act, s_h0, 128, s_wh, 128, false);
+      wg_commit();
+      wg_wait();
+      acc_relu_to_tile(act, sm + S::H1, tid);
+      fence_async_smem();
+      __syncthreads();
+      // ---- G: dH1 = (dOut . Wout) * [H1 > 0] -----------------------------------------------------------------
+      wg_fence();
+      mma_m128<64, 1, 1>(act, s_do, 32, s_wo, 128, false);
+      wg_commit();
+      wg_wait();
+      relu_bwd_epilogue(act, sm + S::H1, sm + S::D1, tid);
       fence_async_smem();
       __syncthreads();
       // ---- B: dWout^T += H1^T . dOut ; dH0 = dH1 . Wh ; dWh += dH1^T . H0 (H0 still the forward activation) ----
-      if (tid == 0) {
-        fence_after_sync();
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          mma_f16(tmem + S::C_GWO, mnmajor_desc(s_h1, 128, k), mnmajor_desc(s_do, 32, k), id_gw16, (k > 0) | acc);
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-          mma_f16(tmem + S::C_ACT, kmajor_desc(s_d1 + 32 * k, 128), mnmajor_desc(s_wh, 128, k), id_act64, k);
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          mma_f16(tmem + S::C_GWH, mnmajor_desc(s_d1, 128, k), mnmajor_desc(s_h0, 128, k), id_gw64, (k > 0) | acc);
-        mma_commit(mbar);
-      }
+      wg_fence();
+      mma_batch128<16>(gwo, s_h1, 128, s_do, 32);
+      mma_m128<64, 1, 4>(act, s_d1, 128, s_wh, 128, false);
+      mma_batch128<64>(gwh, s_d1, 128, s_h0, 128);
+      wg_commit();
     } else {
       // ---- A: dH0 = dOut . Wout ; dWout^T += H0^T . dOut -------------------------------------------------
-      if (tid == 0) {
-        fence_after_sync();
-        mma_f16(tmem + S::C_ACT, kmajor_desc(s_do, 32), mnmajor_desc(s_wo, 128, 0), id_act64, 0);
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          mma_f16(tmem + S::C_GWO, mnmajor_desc(s_h0, 128, k), mnmajor_desc(s_do, 32, k), id_gw16, (k > 0) | acc);
-        mma_commit(mbar);
-      }
+      wg_fence();
+      mma_m128<64, 1, 1>(act, s_do, 32, s_wo, 128, false);
+      mma_batch128<16>(gwo, s_h0, 128, s_do, 32);
+      wg_commit();
     }
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-    relu_bwd_epilogue(tmem_row + S::C_ACT, sm + S::H0, sm + S::H0, tid);                                    // dH0 over H0, in place
-    fence_before_sync();
+    wg_wait();
+    __syncthreads();                                             // every warp's MMAs are done reading H0
+    relu_bwd_epilogue(act, sm + S::H0, sm + S::H0, tid);                                                    // dH0 over H0, in place
     fence_async_smem();
     __syncthreads();
     // ---- C: dIn = dH0 . W0 ; dW0 += dH0^T . X -----------------------------------------------------------
-    if (tid == 0) {
-      fence_after_sync();
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-        mma_f16(tmem + S::C_ACT, kmajor_desc(s_h0 + 32 * k, 128), mnmajor_desc(s_w0, 64, k), id_act32, k);
-#pragma unroll
-      for (int k = 0; k < 8; k++)
-        mma_f16(tmem + S::C_GW0, mnmajor_desc(s_h0, 128, k), mnmajor_desc(s_x, 64, k), id_gw32, (k > 0) | acc);
-      mma_commit(mbar);
-    }
-    first = 0;
-    mbar_wait(mbar, phase); phase ^= 1;
-    fence_after_sync();
-#pragma unroll
-    for (int q = 0; q < 2; q++) {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + S::C_ACT + 16 * q, r);
-      tmem_ld_wait();
-      if (din && valid) {
-        uint4 o[2];
-        uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-#pragma unroll
-        for (int e = 0; e < 8; e++) ow[e] = pk(__uint_as_float(r[2 * e]), __uint_as_float(r[2 * e + 1]));
-        uint4* dst = reinterpret_cast<uint4*>(din + size_t(p) * 32) + 2 * q;
-        dst[0] = o[0]; dst[1] = o[1];
-      }
-    }
-    // the next iteration's barrier orders these TMEM reads before the next tile's first MMA
+    wg_fence();
+    mma_m128<32, 1, 4>(act_in, s_h0, 128, s_w0, 64, false);
+    mma_batch128<32>(gw0, s_h0, 128, s_x, 64);
+    wg_commit();
+    wg_wait();
+    if (din) store_din(act_in, din, tile, n_pts, tid);
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
-  fence_before_sync();
-  __syncthreads();
-  // ---- flush the weight-gradient accumulators (M = 64 layout: warp w, lanes 0..15 hold rows 16w..16w+15) ----
-  if (!first) {
-    fence_after_sync();
-    const int row = warp * 16 + lane;
-    float* g0 = dparams;
-    float* gh = dparams + 64 * 32;
-    float* go = gh + NH * 64 * 64;
-#pragma unroll
-    for (int q = 0; q < 2; q++) {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + S::C_GW0 + 16 * q, r);
-      tmem_ld_wait();
-      if (lane < 16)
-#pragma unroll
-        for (int e = 0; e < 16; e++) atomicAdd(g0 + row * 32 + 16 * q + e, __uint_as_float(r[e]));
-    }
-    {
-      uint32_t r[16];
-      tmem_ld16(tmem_row + S::C_GWO, r);
-      tmem_ld_wait();
-      if (lane < 16)
-#pragma unroll
-        for (int e = 0; e < 16; e++) atomicAdd(go + e * 64 + row, __uint_as_float(r[e]));      // transposed back
-    }
-    if (NH) {
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        uint32_t r[16];
-        tmem_ld16(tmem_row + S::C_GWH + 16 * q, r);
-        tmem_ld_wait();
-        if (lane < 16)
-#pragma unroll
-          for (int e = 0; e < 16; e++) atomicAdd(gh + row * 64 + 16 * q + e, __uint_as_float(r[e]));
-      }
-    }
-    fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, S::TMEM_COLS);
+  if (any) flush_weight_grads<NH>(gw0, gwo, gwh, dparams, tid);
 }
 
 }  // namespace f2b
@@ -569,38 +362,36 @@ extern "C" int f2b_mlp_bwd2_tc(const void* dout_f16, const void* in_f16, const v
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(dout_f16 && in_f16 && params_f16 && dparams_f32, "f2b_mlp_bwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_bwd: n_hidden_matmuls must be 0 or 1");
-  int sms = 148;
+  int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kBT);
+  // persistent grid: as many CTAs as are resident at once (each flushes its weight gradients once)
+#define F2B_BWD_LAUNCH(KERNEL, BYTES, ...)                                                          \
+  {                                                                                                 \
+    cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);               \
+    const int cap = sms * resident_per_sm(KERNEL, kBT, BYTES);                                      \
+    KERNEL<<<n_tiles < cap ? n_tiles : cap, kBT, BYTES, as_stream(stream)>>>(__VA_ARGS__);          \
+  }
   if (!hidden0_f16) {                                             // no saved activations: rebuild them on the tensor pipe
-    if (n_hidden_matmuls == 0) {
-      const int grid = n_tiles < sms * 4 ? n_tiles : sms * 4;     // 48 KB shared memory, 128 TMEM columns per CTA
-      cudaFuncSetAttribute(mlp_bwd_rc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, RcSmem<0>::BYTES);
-      mlp_bwd_rc_kernel<0><<<grid, kBT, RcSmem<0>::BYTES, as_stream(stream)>>>((const __half*)dout_f16, (const __half*)in_f16,
-                                                                              (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32);
-    } else {
-      const int grid = n_tiles < sms * 2 ? n_tiles : sms * 2;     // 256 TMEM columns per CTA
-      cudaFuncSetAttribute(mlp_bwd_rc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, RcSmem<1>::BYTES);
-      mlp_bwd_rc_kernel<1><<<grid, kBT, RcSmem<1>::BYTES, as_stream(stream)>>>((const __half*)dout_f16, (const __half*)in_f16,
-                                                                              (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32);
-    }
-    return check_launch("f2b_mlp_bwd(tcgen05, recompute)");
+    if (n_hidden_matmuls == 0)
+      F2B_BWD_LAUNCH(mlp_bwd_rc_kernel<0>, RcSmem<0>::BYTES, (const __half*)dout_f16, (const __half*)in_f16,
+                     (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32)
+    else
+      F2B_BWD_LAUNCH(mlp_bwd_rc_kernel<1>, RcSmem<1>::BYTES, (const __half*)dout_f16, (const __half*)in_f16,
+                     (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32)
+    return check_launch("f2b_mlp_bwd(wgmma, recompute)");
   }
   F2B_REQUIRE(n_hidden_matmuls == 0 || hidden1_f16, "f2b_mlp_bwd: hidden1 missing (n_hidden_matmuls == 1 with saved activations)");
-  if (n_hidden_matmuls == 0) {
-    const int grid = n_tiles < sms * 3 ? n_tiles : sms * 3;
-    cudaFuncSetAttribute(mlp_bwd_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<0>::BYTES);
-    mlp_bwd_tc_kernel<0><<<grid, kBT, BwdSmem<0>::BYTES, as_stream(stream)>>>(
-        (const __half*)dout_f16, (const __half*)in_f16, (const __half*)hidden0_f16, (const __half*)hidden0_f16,
-        (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32);
-  } else {
-    const int grid = n_tiles < sms * 2 ? n_tiles : sms * 2;
-    cudaFuncSetAttribute(mlp_bwd_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<1>::BYTES);
-    mlp_bwd_tc_kernel<1><<<grid, kBT, BwdSmem<1>::BYTES, as_stream(stream)>>>(
-        (const __half*)dout_f16, (const __half*)in_f16, (const __half*)hidden0_f16, (const __half*)hidden1_f16,
-        (const __half*)params_f16, n_pts, (__half*)din_f16, dparams_f32);
-  }
-  return check_launch("f2b_mlp_bwd(tcgen05)");
+  if (n_hidden_matmuls == 0)
+    F2B_BWD_LAUNCH(mlp_bwd_tc_kernel<0>, BwdSmem<0>::BYTES, (const __half*)dout_f16, (const __half*)in_f16,
+                   (const __half*)hidden0_f16, (const __half*)hidden0_f16, (const __half*)params_f16, n_pts, (__half*)din_f16,
+                   dparams_f32)
+  else
+    F2B_BWD_LAUNCH(mlp_bwd_tc_kernel<1>, BwdSmem<1>::BYTES, (const __half*)dout_f16, (const __half*)in_f16,
+                   (const __half*)hidden0_f16, (const __half*)hidden1_f16, (const __half*)params_f16, n_pts, (__half*)din_f16,
+                   dparams_f32)
+#undef F2B_BWD_LAUNCH
+  return check_launch("f2b_mlp_bwd(wgmma)");
 }
 
 extern "C" int f2b_mlp_bwd_tc(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,

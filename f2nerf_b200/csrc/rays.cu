@@ -3,7 +3,7 @@
 // Replaces Dataset::Img2WorldRayFlex + Img2WorldRayKernel (src/Dataset/Dataset.cu:100-152, with the 100-iteration
 // Newton undistortion of :30-74 taken from instant-ngp) and the CPU-side ground-truth gather + host->device copy of
 // Dataset::RandRaysData (src/Dataset/Dataset.cpp:290): with the images resident in HBM one small kernel each.
-// The fp32 operation order of the undistortion was read off the reference build's SASS (nvcc 12.9, sm_100a; ptxas
+// The fp32 operation order of the undistortion was read off the reference build's SASS (nvcc 12.9; ptxas
 // fuses further mul+sub pairs that the PTX still shows separately) and is spelled out with explicit roundings, so rays are bit-identical to the reference's (tests/test_ref_parity.py).
 #include "common.cuh"
 

@@ -1,7 +1,7 @@
 // render.cu — the per-batch launch sequences of the fused Renderer::Render pipeline behind single C-ABI calls
 // (f2b_render_phase1 / _phase2_fwd / _bwd / _grad_finalize, include/f2nerf_b200.h).
 //
-// Why: measured on B200 (profiles/r02_timeline.md) the step spent ~0.8 ms with the GPU idle behind the one host sync of
+// Why: the step would otherwise keep the GPU idle behind the one host sync of
 // Renderer::Render — a Python host needs ~130 foreign calls / allocator calls to enqueue the second half of the step, and
 // the short kernels right after the sync finish faster than it can launch them.  The sequences are fixed, so they live here:
 // one foreign call per phase, the kernels back to back.  No new arithmetic: every launch goes through the entry points
@@ -97,7 +97,7 @@ extern "C" int f2b_render_phase2_fwd(const f2b_render* r) {
 
 extern "C" int f2b_render_bwd(const f2b_render* r) {
   F2B_REQUIRE(r, "f2b_render_bwd: null argument block");
-  // f_hidden / s_hidden NULL: the forward saved no hidden activations, f2b_mlp_bwd2 rebuilds them (recompute, tcgen05 only)
+  // f_hidden / s_hidden NULL: the forward saved no hidden activations, f2b_mlp_bwd2 rebuilds them (recompute, tensor-core only)
   const int64_t nk = r->n_kept, ne = 2 * int64_t(r->n_edge_pairs), nq = nk + ne;
   cudaStream_t st = as_stream(r->stream), side = as_stream(r->side_stream);
   const bool emb = r->app_emb && r->ray_emb_idx;
@@ -155,7 +155,7 @@ extern "C" int f2b_render_grad_finalize(const f2b_render* r) {
                                                                            r->d_fparams, r->n_field_params, 1.f / r->field_loss_scale,
                                                                            emb ? r->d_app : nullptr, n_app, r->nonfinite);
   if (r->d_table && r->table_live >= 4) {
-    int sms = 148;
+    int sms = 132;
     f2b_device_info(&sms, nullptr);
     finalize_table_kernel<<<sms * 4, 256, 0, as_stream(r->stream)>>>(reinterpret_cast<const float4*>(r->d_table), r->table_live / 4,
                                                                      r->nonfinite);

@@ -1,4 +1,4 @@
-// sampler.cu — fused octree traversal + perspective-warp ray march for sm_100a.
+// sampler.cu — fused octree traversal + perspective-warp ray march for sm_90a.
 //
 // Replaces, behind f2b_sampler_count / f2b_sampler_fill, the reference's
 //   FindRayOctreeIntersectionKernel<false/true>  (src/PtsSampler/PersSampler.cu:53-152)
@@ -7,7 +7,7 @@
 // and GetEdgeSamplesKernel (:436-452), MarkVistNodeKernel (:475-526), MarkInvalidNodes (:528-534)
 // plus the ATen vote/stat update of UpdateOctNodes (:579-592).
 //
-// B200 design (not a translation):
+// Design (not a translation):
 //  * traversal and march are ONE kernel: the DFS is a coroutine that yields the next leaf hit
 //    when the march walks off the current leaf, so the (node, near, far) hit list is never
 //    written to HBM and the reference's first host sync (.item() at :353) disappears;

@@ -1,5 +1,5 @@
 // shader.cuh — device functions shared by shader.cu (stand-alone operators) and mlp_tc.cu (the same work fused into
-// the tcgen05 MLP epilogues).  Explicit roundings: both users produce bit-identical rows.
+// the tensor-core MLP epilogues).  Explicit roundings: both users produce bit-identical rows.
 #pragma once
 #include "common.cuh"
 #include <cuda_fp16.h>

@@ -209,7 +209,7 @@ class Hash3DAnchored:
 
 def field_forward(field, table16, params16, points, anchors, anchor_stride, save, logit_only=False, save_feat=None):
     """hash encode -> MLP.  Returns (out, feat16, hidden); out is fp32 [n,16], or [n] (channel 0) when
-    ``logit_only``; feat16 when ``save`` or ``save_feat``, hidden only when ``save``.  With the tcgen05 MLP
+    ``logit_only``; feat16 when ``save`` or ``save_feat``, hidden only when ``save``.  With the tensor-core MLP
     selected (default) this is ONE fused kernel (f2b_field_fwd); with the CUDA-core twin it is encode + MLP + cast."""
     from . import _lib
     save_feat = save if save_feat is None else save_feat

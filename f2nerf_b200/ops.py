@@ -116,7 +116,7 @@ def hash_bwd(prim_pool, bias_pool, n_volumes, local_size, pts, vol, vol_stride, 
 
 def field_fwd(table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, pts, vol, vol_stride=1, logit_only=False,
               save=False, save_feat=None):
-    """Fused hash encode + tcgen05 field MLP.  -> (out [n] or [n,16] fp32, feat16 | None, hidden | None).
+    """Fused hash encode + tensor-core field MLP.  -> (out [n] or [n,16] fp32, feat16 | None, hidden | None).
     ``save`` keeps features + hidden activations (gradient pass); ``save_feat`` keeps only the features."""
     n = pts.shape[0]
     save_feat = save if save_feat is None else save_feat

@@ -20,7 +20,7 @@ from .rng import burn_mlp_output, burn_rand
 from .sampler import TRAIN, VALIDATE, LazySampleResult, SampleResultFlex
 
 N_EDGE_PTS = 8192
-# The tcgen05 MLP backward rebuilds the hidden activations from the 64 B input row instead of reading 128 / 256 B per sample the
+# The tensor-core MLP backward rebuilds the hidden activations from the 64 B input row instead of reading 128 / 256 B per sample the
 # forward saved (f2b_mlp_bwd2 with hidden0 == NULL): bit-identical dL/dinput, no hidden_save traffic.  F2B_MLP_RECOMPUTE=0 saves.
 MLP_RECOMPUTE = os.environ.get("F2B_MLP_RECOMPUTE", "1") == "1"
 
@@ -616,7 +616,7 @@ class _RenderFunction(torch.autograd.Function):
         n_q = feat16.shape[0]
         emb = app_emb if pt_emb_idx is not None else None
         if _lib.lib.f2b_get_mlp_impl() == 1 and field.mlp_.n_hidden_matmuls == 0 and shader.mlp_.n_hidden_matmuls == 1:
-            # fused epilogues (tcgen05 kernels): field MLP -> [logit | shader-MLP input row], shader MLP -> [raw | rgb];
+            # fused epilogues (tensor-core kernels): field MLP -> [logit | shader-MLP input row], shader MLP -> [raw | rgb];
             # the fp32 scene_feat of the ray samples is never materialised (edge points still need all 16 channels)
             save = grad_on and not MLP_RECOMPUTE
             f_hidden = torch.empty((1, n_q, 64), dtype=torch.float16, device=dev) if save else None
@@ -676,9 +676,8 @@ class _RenderFunction(torch.autograd.Function):
             burn_rand(n_kept, dev)
         # ---- backward, optionally in ray chunks (bwd_chunks_ / F2B_BWD_CHUNKS): the dense chain (composite -> sigmoid ->
         # shader MLP -> input assembly -> field MLP; HBM streaming) of chunk k+1 on the main stream, the hash scatter of
-        # chunk k (L2 reductions) on a side stream.  Measured on B200 (r01): co-running them is SLOWER (6.05 ms at 1
-        # chunk, 6.5 / 6.8 / 7.7 ms at 2 / 4 / 8: the scatter's 260 k small blocks crowd out the persistent tcgen05 CTAs),
-        # so the default is one chunk; the scatter still runs on the side stream behind an event.
+        # chunk k (L2 reductions) on a side stream.  Co-running them is slower (the scatter's many small blocks crowd out
+        # the persistent tensor-core CTAs), so the default is one chunk; the scatter still runs on the side stream behind an event.
         s_scale, f_scale = shader.mlp_.loss_scale_, field.mlp_.loss_scale_
         nh_s, nh_f = shader.mlp_.n_hidden_matmuls, field.mlp_.n_hidden_matmuls
         f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)

@@ -195,8 +195,8 @@ class PersSampler:
         ev.record(main)                                            # the ray upload / noise draw queued so far precede the march (the
         stream.wait_event(ev)                                      # scratch it writes is the OTHER set: no reader to wait for)
         with torch.cuda.stream(stream):
-            # F2B_MARCH_BG=1 selects the <= 64-register build: measured SLOWER overall on B200 (4.56 vs 4.40 ms per step: more
-            # of it co-resides with the dense backward and takes its issue slots), so the default stays the 96-register kernel
+            # F2B_MARCH_BG=1 selects the <= 64-register build: more of it co-resides with the dense backward and takes its issue
+            # slots, so the default stays the 96-register kernel
             self.march_rays(slots, 0, n_rays, background=os.environ.get("F2B_MARCH_BG", "0") == "1")
             ring = self.__dict__.setdefault("_pinned_totals", [torch.empty((2,), dtype=torch.int32).pin_memory() for _ in range(4)])
             self._pinned_turn = (getattr(self, "_pinned_turn", -1) + 1) % len(ring)

@@ -1,5 +1,5 @@
 // RenderReferenceThunk.cpp — compiled with -DRender=RenderReference, like the reference's own Renderer.cpp in the
-// B200 build (oracle/Makefile.ref, INTEGRATION.md section 3): under that macro the class declaration in
+// drop-in build (oracle/Makefile.ref, INTEGRATION.md section 3): under that macro the class declaration in
 // Renderer/Renderer.h names the reference's body `RenderReference`, and this one-line wrapper makes it callable from
 // B200Renderer.cpp (which sees the header without the macro) — used when F2B_RENDER=reference selects the reference path.
 #include "Renderer/Renderer.h"

@@ -1,4 +1,4 @@
-/* f2nerf_b200.h — C ABI of the B200-native (sm_100a) F2-NeRF per-ray rendering hot path.
+/* f2nerf_b200.h — C ABI of the H100-native (sm_90a) F2-NeRF per-ray rendering hot path.
  *
  * Every entry point takes plain device pointers + sizes + a cudaStream_t (as void*), never
  * allocates, never retains a pointer past the call, never throws.  Return value: 0 on success,
@@ -149,7 +149,7 @@ int f2b_hash_bwd_levels(const int* prim_pool, const float* bias_pool, int n_volu
 int f2b_mlp_fwd(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
                 void* out_f16, void* hidden_save_f16, void* stream);
 /* Same network with the output widened to fp32 in the epilogue — what TCNNWP::Query returns
- * (`feat...to(torch::kFloat32)`, TCNNWP.cpp:112).  out_f32 [P,16] and/or out_f16 [P,16]; with the tcgen05
+ * (`feat...to(torch::kFloat32)`, TCNNWP.cpp:112).  out_f32 [P,16] and/or out_f16 [P,16]; with the tensor-core
  * implementation either may be NULL (not both), the CUDA-core twin needs out_f16. */
 int f2b_mlp_fwd_f32(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
                     float* out_f32, void* out_f16, void* hidden_save_f16, void* stream);
@@ -162,7 +162,7 @@ int f2b_mlp_bwd(const void* dout_f16, const void* in_f16, const void* hidden_sav
 int f2b_cast_f32_to_f16(const float* src, void* dst, int64_t n, float scale, void* stream);
 int f2b_cast_f16_to_f32(const void* src, float* dst, int64_t n, float scale, void* stream);
 
-/* Fused Hash3DAnchored::AnchoredQuery (Hash3DAnchored.cpp:84-99): hash encode + tcgen05 MLP(32->64->16) in one
+/* Fused Hash3DAnchored::AnchoredQuery (Hash3DAnchored.cpp:84-99): hash encode + tensor-core MLP(32->64->16) in one
  * kernel; the encoded features reach HBM only through feat_save (backward needs them).
  * logit_only != 0: the no-grad early-stop pass — out is [P] fp32 (channel 0 only); feat_save optional, no hidden_save.
  * otherwise out is [P,16] fp32 (fp16-rounded values, as TCNNWP::Query returns); feat_save [P,32] fp16 and
@@ -184,24 +184,24 @@ int f2b_field_fwd_slots(const void* table_f16, const int* prim_pool, const float
 /* Field MLP on already-encoded features with the shading-feature assembly fused into its epilogue (the fp32 [P,16]
  * scene_feat tensor, `ones_like`/`cat`/ScatterAdd of Renderer.cpp:179-187 and the SH encode + cast of SHShader.cpp:23-26
  * never materialise): logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])).
- * tcgen05 implementation only (F2B_EUNSUPPORTED with the CUDA-core twin selected). */
+ * tensor-core implementation only (F2B_EUNSUPPORTED with the CUDA-core twin selected). */
 int f2b_field_shade_fwd(const void* feat_f16 /* [P,32] */, const void* field_params_f16, const float* dirs /* [P,3] */,
                         const float* app_emb /* [n_emb,16] or NULL */, const int* pt_emb_idx /* [P] or NULL */, int n_pts,
                         float* logit /* [P] */, void* mlp_in_f16 /* [P,32] */, void* hidden_save_f16 /* [P,64] or NULL */,
                         void* stream);
 /* Shader MLP with the colour activation of SHShader.cpp:27-28 in its epilogue: raw [P,16] fp16 and
- * rgb [P,3] = (1 + 2e-3) * sigmoid(raw[:, :3]) - 1e-3.  tcgen05 implementation only. */
+ * rgb [P,3] = (1 + 2e-3) * sigmoid(raw[:, :3]) - 1e-3.  tensor-core implementation only. */
 int f2b_shader_mlp_rgb_fwd(const void* mlp_in_f16, const void* shader_params_f16, int n_pts, void* raw_f16, float* rgb,
                            void* hidden_save_f16 /* [2,P,64] or NULL */, void* stream);
 /* f2b_mlp_bwd on a row range of a larger saved batch: the two activation layers are passed as separate pointers
  * (hidden1 NULL when n_hidden_matmuls == 0).  dparams is accumulated into, like f2b_mlp_bwd.
- * hidden0 == NULL (tcgen05 implementation only): the forward saved nothing — the kernel rebuilds the tile's hidden
+ * hidden0 == NULL (tensor-core implementation only): the forward saved nothing — the kernel rebuilds the tile's hidden
  * activations from in_f16 on the tensor pipe (bit-identical to what the forward would have saved) before the backward;
  * 96 B read + 64 B written per sample instead of 224 / 352 + 64 (and the forward does not write 128 / 256 B). */
 int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void* hidden0_f16, const void* hidden1_f16,
                  const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16, float* dparams_f32, void* stream);
 
-/* Implementation selection for f2b_mlp_fwd / f2b_mlp_bwd: 1 = tcgen05/TMEM kernels (default when
+/* Implementation selection for f2b_mlp_fwd / f2b_mlp_bwd: 1 = wgmma tensor-core kernels (default when
  * built), 0 = CUDA-core twin (validation).  Env F2B_MLP_IMPL overrides the default. */
 int f2b_set_mlp_impl(int impl);
 int f2b_get_mlp_impl(void);
@@ -420,7 +420,7 @@ int f2b_render_grad_finalize(const f2b_render* r);
  * > 0: normal; <= 0: the reference's empty-batch result, depth = 512, Renderer.cpp:83-97).  ticket: [1] device int scratch.
  * Outputs: colors [R,3], disparity [R], depth [R], kept_counts [R] (survivors per ray), and — nullable — weights_slots
  * [R*slot]: the kept samples' weights at their slots (f2b_gather_kept_weights packs them into RenderResult.weights order).
- * Values are bit-identical to f2b_render_phase1 + f2b_render_phase2_fwd on the same batch.  tcgen05 implementation only. */
+ * Values are bit-identical to f2b_render_phase1 + f2b_render_phase2_fwd on the same batch.  tensor-core implementation only. */
 int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
                          const void* field_params_f16, const void* shader_params_f16, const float* slot_pts, const float* slot_dt,
                          const float* slot_t, const int* slot_anchors, const int* ray_counts, const float* rays_d, const float* bg,

@@ -95,7 +95,7 @@ int main(int argc, char** argv) {
 #ifdef F2B_WITH_SHIM
   // ---- ref_driver_b200 only.  Default (F2B_SHIM unset or "fused"): the body of Renderer::Render is the fused B200 host
   // (f2nerf_b200/shim/B200Renderer.cpp) working on the reference's own operator objects.  F2B_SHIM=ops: the operator-level
-  // drop-in — the reference's OWN Renderer::Render / autograd / loss drive the B200 subclasses (INTEGRATION.md): same octree
+  // drop-in — the reference's OWN Renderer::Render / autograd / loss drive this library's subclasses (INTEGRATION.md): same octree
   // object, same parameters.  Either way every dump below is directly comparable with the pure-reference run of
   // oracle/_ref/ref_driver.  Never built into ref_driver (the reference arm stays unmodified).
   const char* shim_env = std::getenv("F2B_SHIM");

@@ -42,7 +42,8 @@ def cos(a, b):
 
 
 def main():
-    g = dict(np.load(os.path.join(ROOT, "tests", "golden", "ref_ngp_fox.npz")))
+    from workloads import load_golden
+    g = load_golden()
     sc = g["scalars"]
     V, pool, R = int(sc[4]), int(sc[5]), int(sc[7])
     gen = torch.Generator().manual_seed(1234)

@@ -1,7 +1,7 @@
 // microbench_gather.cu — rate of random 4-byte gathers from an L2-resident table on this GPU: the roofline that governs the
 // hash encode (f2b_field_fwd / f2b_hash_fwd: 128 half2 gathers per sample from the 17 MB live prefix of the fp16 table).
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/gather scripts/microbench_gather.cu && /tmp/gather > gpurun_out/gather_rate.json
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/gather scripts/microbench_gather.cu && /tmp/gather > gather_rate.json
 //
 // Patterns: `spread` — every lane its own random entry (the fine levels: every sample in its own cell);
 //           `warp_same` — all 32 lanes of a warp read the same 8 random entries (the coarse levels: a warp's samples share a cell);

@@ -1,9 +1,9 @@
 // microbench_red.cu — issue rate of global-memory reductions on this GPU, the roofline that governs f2b_hash_bwd.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/red scripts/microbench_red.cu && /tmp/red > gpurun_out/red_rate.json
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/red scripts/microbench_red.cu && /tmp/red > red_rate.json
 //
 // Every lane issues `red.global.add` to pseudo-random addresses inside a buffer of the hash table's live size (34 MB of
-// fp32 pairs: L2-resident on B200, like the real gradient table), for three flavours:
+// fp32 pairs: L2-resident, like the real gradient table), for three flavours:
 //   v2f32   red.global.add.v2.f32   (8 B: what hash_bwd issues, one per (sample, level, corner))
 //   f32     red.global.add.f32      (4 B)
 //   f16x2   red.global.add.noftz.f16x2 (4 B: both channels of one table entry in fp16 — the reference's own format)

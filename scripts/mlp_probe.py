@@ -1,4 +1,4 @@
-"""Probe: how much of the tcgen05 MLP kernels' time is HBM traffic for the saved activations?  Times f2b_mlp_fwd with and
+"""Probe: how much of the tensor-core MLP kernels' time is HBM traffic for the saved activations?  Times f2b_mlp_fwd with and
 without hidden_save, f2b_field_shade_fwd / f2b_shader_mlp_rgb_fwd, and f2b_mlp_bwd2, on N samples (default 3.1 M = the headline's
 kept samples).  If the no-save forward is several times faster, recomputing the hidden layers in the backward (instead of
 saving 384 B/sample) pays.  Output: one JSON line."""

@@ -40,8 +40,8 @@ if has configs; then
   done
 fi
 if has probes; then
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/red scripts/microbench_red.cu && timeout 120 /tmp/red > $O/${TAG}_red_rate.json
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/gather scripts/microbench_gather.cu && timeout 120 /tmp/gather > $O/${TAG}_gather_rate.json
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/red scripts/microbench_red.cu && timeout 120 /tmp/red > $O/${TAG}_red_rate.json
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/gather scripts/microbench_gather.cu && timeout 120 /tmp/gather > $O/${TAG}_gather_rate.json
   timeout 300 python scripts/level_probe.py > $O/${TAG}_level_probe.json 2> $O/${TAG}_level_probe.err
   timeout 300 python scripts/mlp_probe.py > $O/${TAG}_mlp_probe.json 2> $O/${TAG}_mlp_probe.err
   timeout 300 python scripts/timeline.py --steps 6 > $O/${TAG}_timeline.json 2> $O/${TAG}_timeline.err

@@ -1,5 +1,5 @@
 #!/bin/bash
-# the final build's C++ host through the unmodified trainer, full 20 000-iteration schedule (B200 arm only; the reference arm's
+# the final build's C++ host through the unmodified trainer, full 20 000-iteration schedule (drop-in arm only; the reference arm's
 # 20 k run of this round is profiles/r02e_train_psnr_20k.json)
 cd "$(dirname "$0")/.."
 O=gpurun_out; mkdir -p $O; TAG=${TAG:-r02o}

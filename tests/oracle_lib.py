@@ -3,6 +3,7 @@ cpu_baseline leg.  Test infrastructure: never imported by the f2nerf_b200 packag
 import ctypes
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -11,11 +12,15 @@ SO = os.path.join(ROOT, "oracle", "libf2oracle.so")
 
 
 def build():
+    """The oracle library build() made; (re)compiled when missing or older than its source — into a temporary directory
+    when the tree is read-only."""
     src = os.path.join(ROOT, "oracle", "f2_oracle.c")
-    if not os.path.exists(SO) or os.path.getmtime(SO) < os.path.getmtime(src):
-        subprocess.check_call(["gcc", "-O2", "-march=x86-64-v3", "-fopenmp", "-ffp-contract=off", "-fno-fast-math",
-                               "-shared", "-fPIC", src, "-o", SO, "-lm"])
-    return SO
+    if os.path.exists(SO) and os.path.getmtime(SO) >= os.path.getmtime(src):
+        return SO
+    out = SO if os.access(os.path.dirname(SO), os.W_OK) else os.path.join(tempfile.mkdtemp(prefix="f2b_oracle_"), "libf2oracle.so")
+    subprocess.check_call(["gcc", "-O2", "-march=x86-64-v3", "-fopenmp", "-ffp-contract=off", "-fno-fast-math",
+                           "-shared", "-fPIC", src, "-o", out, "-lm"])
+    return out
 
 
 _lib = None

@@ -1,6 +1,5 @@
-"""Host-side logic of bench.py that must not break on the GPU box (no GPU needed): the `config` object both arms print, the governing
-rooflines computed from the committed captures / microbenchmarks, the clock sampler on ranks that do not sample."""
-import glob
+"""Host-side logic of bench.py that must not break on the GPU box (no GPU needed): the `config` object both arms print, the clock
+sampler on ranks that do not sample, the keys of the committed bench lines."""
 import json
 import os
 import sys
@@ -24,23 +23,6 @@ def test_config_object_is_a_pure_function_of_the_flags():
     assert weak["rays_per_gpu"] == 4096 and weak["global_rays"] == 8 * 4096
 
 
-def test_governing_rooflines_from_committed_profiles():
-    """profiles/*_traffic.json (ncu sector counts) + the two microbenchmark files must give sane fractions for the two table
-    kernels at their measured times, and nothing for kernels / workloads they do not describe."""
-    assert glob.glob(os.path.join(ROOT, "profiles", "*_traffic.json"))
-    bench.GOVERNING_OK = True
-    g = bench.governing_roofline("f2b_field_fwd_slots", 0.90)
-    assert g["bound"] == "l1_l2_gather_sectors" and 0.9 < g["frac"] <= 1.01 and g["units_per_launch"] > 2e8
-    r = bench.governing_roofline("f2b_hash_bwd", 0.87)
-    assert r["bound"] == "l2_reduction_issue" and 0.6 < r["frac"] < 0.95 and r["units_per_launch"] > 1e8
-    assert bench.governing_roofline("f2b_composite_fwd", 0.1) is None
-    bench.GOVERNING_OK = False                                                                # any other workload than the captured one
-    assert bench.governing_roofline("f2b_hash_bwd", 0.87) is None
-    bench.GOVERNING_OK = True
-    t = bench.ncu_traffic("f2b_hash_bwd")
-    assert t is not None and t["dram_bytes_per_launch"] > 1e8
-
-
 def test_clock_sampler_is_inert_on_non_sampling_ranks():
     c = bench.ClockSampler(-1)
     c.poll()
@@ -50,15 +32,13 @@ def test_clock_sampler_is_inert_on_non_sampling_ranks():
 
 
 def test_committed_bench_lines_carry_the_contract_keys():
-    """The driver-format lines kept under profiles/ (the numbers DESIGN.md / BASELINE.md quote) have every key of the bench contract."""
-    line = json.loads(open(os.path.join(ROOT, "profiles", "r02q_bench.json")).read().strip().splitlines()[-1])
+    """The bench lines kept under profiles/ (the numbers BASELINE.md quotes) have every key of the bench contract."""
+    line = json.loads(open(os.path.join(ROOT, "profiles", "h100_bench.json")).read().strip().splitlines()[-1])
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
               "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
         assert k in line, k
     assert line["vs_baseline"] is None and line["roofline"]["bound"] in ("hbm", "tensor") and line["gpu_launches"] > 0
     assert {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} <= set(line["e2e"])
     assert {"value", "unit", "cores", "kind", "sample"} <= set(line["cpu_baseline"])
-    ref = json.loads(open(os.path.join(ROOT, "profiles", "r02h_bench_ref.json")).read().strip().splitlines()[-1])
+    ref = json.loads(open(os.path.join(ROOT, "profiles", "h100_bench_ref.json")).read().strip().splitlines()[-1])
     assert ref["impl"] == "reference" and ref["config"] == line["config"] and ref["metric"] == line["metric"]
-    gov = {r["kernel"]: r["governing"] for r in line["rooflines"]}
-    assert 0.9 < gov["f2b_field_fwd_slots"]["frac"] <= 1.01 and 0.6 < gov["f2b_hash_bwd"]["frac"] < 0.95

@@ -224,7 +224,7 @@ def test_mlp_fwd_bwd(oracle, nh, impl):
 
 @pytest.mark.parametrize("nh", [0, 1])
 def test_mlp_tc_tiles_and_f32_output(oracle, nh):
-    """Persistent-tile path of the tcgen05 forward: sizes below / across / far beyond one tile per CTA (double-buffered
+    """Persistent-tile path of the tensor-core forward: sizes below / across / far beyond one tile per CTA (double-buffered
     cp.async input, coalesced hidden copy-out), tc == CUDA-core twin within fp16 noise, fp32 output == widened fp16."""
     from f2nerf_b200 import ops
     rng = np.random.default_rng(77 + nh)
@@ -244,7 +244,7 @@ def test_mlp_tc_tiles_and_f32_output(oracle, nh):
         assert none16 is None
         np.testing.assert_array_equal(N(out32b), N(out32))
         # backward over the same tiles (double-buffered operand prefetch, in-place activation gradients,
-        # weight gradients resident in TMEM across the CTA's tiles) against the CUDA-core twin
+        # weight gradients resident in registers across the CTA's tiles) against the CUDA-core twin
         dout = T((rng.standard_normal((n, 16)) * 0.1).astype(np.float16))
         din, dp = ops.mlp_bwd(dout, x, hid0, params, nh, need_din=True, impl="tc")
         din0, dp0 = ops.mlp_bwd(dout, x, hid0, params, nh, need_din=True, impl="v0")
@@ -255,7 +255,7 @@ def test_mlp_tc_tiles_and_f32_output(oracle, nh):
 @pytest.mark.parametrize("nh", [0, 1])
 def test_mlp_bwd_recompute_equals_saved(oracle, nh):
     """f2b_mlp_bwd2 with hidden0 == NULL rebuilds the hidden activations on the tensor pipe from the input rows (no 128 / 256 B
-    per sample saved by the forward): dL/dinput must equal the saved-activation kernel's BIT FOR BIT (same UMMAs on the same
+    per sample saved by the forward): dL/dinput must equal the saved-activation kernel's BIT FOR BIT (same MMAs on the same
     operands), the weight gradients up to the order of the fp32 atomics that flush them."""
     from f2nerf_b200 import ops
     from f2nerf_b200._lib import call, stream
@@ -308,7 +308,7 @@ def test_fused_epilogues_match_operator_sequence(oracle):
 
 
 def test_fused_field_matches_unfused(scene, oracle, hash_params):
-    """f2b_field_fwd (encode fused into the tcgen05 MLP) == f2b_hash_fwd -> f2b_mlp_fwd_tc, bit for bit."""
+    """f2b_field_fwd (encode fused into the tensor-core MLP) == f2b_hash_fwd -> f2b_mlp_fwd_tc, bit for bit."""
     from f2nerf_b200 import ops
     s = sample_points(scene, oracle, 100)
     hp = hash_params

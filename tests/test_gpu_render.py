@@ -75,7 +75,7 @@ def test_render_train_step_matches_oracle(scene, oracle, n_rays, gs_progress):
     assert_close(N(res.depth), ref["depth"], rtol=2e-3, atol_frac=2e-3, name="depth")
     assert abs(float(loss) - ref["loss"]) <= 2e-5 * abs(ref["loss"])
     # gradients.  Globally (relative L2 against the oracle's fp32-accumulate chain with the same fp16 rounding points) they
-    # agree to ~1e-5 (measured on B200, cf. tests/test_gpu_headline.py); element-wise a single flipped fp16 rounding shows,
+    # agree to ~1e-5 (cf. tests/test_gpu_headline.py); element-wise a single flipped fp16 rounding shows,
     # hence the looser per-element bars below
     rel = lambda a, b: float(np.linalg.norm(np.asarray(a, np.float64) - b) / (np.linalg.norm(b) + 1e-300))
     for name, mine in (("grad_field_mlp", field.mlp_.params_.grad), ("grad_shader_mlp", shader.mlp_.params_.grad),

@@ -1,13 +1,14 @@
 """CUDA path against the REAL reference (unmodified Totoro97/f2-nerf + tiny-cuda-nn, compiled into
 oracle/_ref/ref_driver) on the reference's own ngp_fox octree / cameras, from two sources:
 
-  * ``golden`` — the committed dump of a reference run, tests/golden/ref_ngp_fox.npz (oracle/make_golden.py): needs no
+  * ``golden`` — the committed dump of a reference run, tests/golden/ref_ngp_fox_{run,rays}.npz (oracle/make_golden.py): needs no
     binary, so these cases run wherever a GPU is;
-  * ``live``   — the binary run on this GPU at 512 rays (oracle/_ref/ref_driver, built by build() from /root/reference).
+  * ``live``   — the reference on a 512-ray batch: the binary run on this GPU (oracle/_ref/ref_driver, built by build() when the
+    reference's sources are present), else its stored run, tests/golden/ref_ngp_fox_512_*.npz (every per-ray tensor, and the
+    per-sample tensors of the rays in ``sample_rays``, which the per-sample comparisons are restricted to).
 
 Integer outputs (sample bounds, anchors, compacted bounds, octree statistics and pruned nodes) must be
 bit-exact; fp32 stages within 1e-4; fp16 stages (hash features -> tcnn MLP) within fp16 noise of tcnn.
-The ``live`` cases are skipped only when the driver binary is absent (build() makes it whenever /root/reference exists).
 """
 import json
 import os
@@ -18,24 +19,23 @@ import pytest
 import torch
 
 from test_gpu_parity import N, T, assert_close, half_ulps
+from workloads import diag_path, load_golden
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DRV = os.path.join(ROOT, "oracle", "_ref", "ref_driver")
 N_RAYS_LIVE = 512
-GOLD = os.path.join(ROOT, "tests", "golden", "ref_ngp_fox.npz")
 BOTH = ["golden", "live"]
 
 
 def _live():
     if not os.path.exists(DRV):
-        pytest.skip("oracle/_ref/ref_driver not built")
-    out = "/tmp/f2b_ref_dump"                                   # large (full 64 MB table gradient): not under gpurun_out
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
+        return load_golden("ref_ngp_fox_512")
+    out = "/tmp/f2b_ref_dump"                                   # large (full 64 MB table gradient)
     r = subprocess.run([DRV, os.path.join(ROOT, "oracle", "ref_config_ngp_fox.yaml"), out, str(N_RAYS_LIVE), "0", "1"], cwd=ROOT,
                        capture_output=True, text=True, timeout=900)
-    open(os.path.join(ROOT, "gpurun_out", "ref_driver.log"), "w").write(r.stdout[-20000:] + "\n--- stderr ---\n" + r.stderr[-20000:])
+    open(diag_path("ref_driver.log"), "w").write(r.stdout[-20000:] + "\n--- stderr ---\n" + r.stderr[-20000:])
     assert r.returncode == 0, r.stderr[-3000:]
     return {f[:-4]: np.load(os.path.join(out, f)) for f in os.listdir(out) if f.endswith(".npy")}
 
@@ -48,11 +48,8 @@ def ref(request):
     """The reference's dumps, keyed like ref_driver.cpp names them.  fp16-stored fixture entries are widened to fp32."""
     kind = request.param
     if kind not in _cache:
-        if kind == "live":
-            _cache[kind] = _live()
-        else:
-            d = dict(np.load(GOLD))
-            _cache[kind] = {k: (v.astype(np.float32) if v.dtype == np.float16 else v) for k, v in d.items()}
+        d = _live() if kind == "live" else load_golden()
+        _cache[kind] = {k: (v.astype(np.float32) if v.dtype == np.float16 else v) for k, v in d.items()}
     d = _cache[kind]
     d["_kind"] = kind
     return d
@@ -60,6 +57,14 @@ def ref(request):
 
 def n_rays_of(ref):
     return int(ref["scalars"][7])
+
+
+def stored_rows(ref, a, bounds_key):
+    """Our per-sample tensor ``a`` restricted to the rays whose samples ``ref`` holds: all rays, unless it stores the
+    segments of ``sample_rays`` only ([begin, end) row ranges per ray in ``ref[bounds_key]``, concatenated in ray order)."""
+    if "sample_rays" not in ref:
+        return a
+    return np.concatenate([a[b:e] for b, e in ref[bounds_key][ref["sample_rays"]]])
 
 
 def build_from_ref(ref):
@@ -96,9 +101,10 @@ def test_sampler_validate_bit_exact(ref):
     gdp.mode_ = VALIDATE
     s = sampler.GetSamples(T(ref["rays_o"]), T(ref["rays_d"]), None)
     np.testing.assert_array_equal(N(s.pts_idx_bounds), ref["val_bounds"])
-    np.testing.assert_array_equal(N(s.anchors)[:, :2], ref["val_anchors"])
-    for k, v in (("val_first_oct_dis", s.first_oct_dis), ("val_t", s.t), ("val_dt", s.dt), ("val_dirs", s.dirs), ("val_pts", s.pts)):
-        np.testing.assert_array_equal(N(v).view(np.uint32), ref[k].view(np.uint32), err_msg=k)
+    np.testing.assert_array_equal(stored_rows(ref, N(s.anchors)[:, :2], "val_bounds"), ref["val_anchors"])
+    np.testing.assert_array_equal(N(s.first_oct_dis).view(np.uint32), ref["val_first_oct_dis"].view(np.uint32))
+    for k, v in (("val_t", s.t), ("val_dt", s.dt), ("val_dirs", s.dirs), ("val_pts", s.pts)):
+        np.testing.assert_array_equal(stored_rows(ref, N(v), "val_bounds").view(np.uint32), ref[k].view(np.uint32), err_msg=k)
 
 
 def test_field_and_shader_vs_tcnn(ref):
@@ -128,14 +134,14 @@ def test_render_validate_vs_reference(ref):
     cnt_m, cnt_t = mine[:, 1] - mine[:, 0], theirs[:, 1] - theirs[:, 0]
     frac_rays_same = (cnt_m == cnt_t).mean()
     json.dump(dict(frac_rays_same_count=float(frac_rays_same), max_count_diff=int(np.abs(cnt_m - cnt_t).max()),
-                   kept_mine=int(cnt_m.sum()), kept_ref=int(cnt_t.sum())), open(os.path.join(ROOT, "gpurun_out", "ref_validate_mask.json"), "w"))
+                   kept_mine=int(cnt_m.sum()), kept_ref=int(cnt_t.sum())), open(diag_path("ref_validate_mask.json"), "w"))
     # the T > 1e-4 crossing sits downstream of the fp16 MLP: tcnn's fp16-accumulate noise shifts it by a few samples
     assert frac_rays_same >= 0.9 and abs(int(cnt_m.sum()) - int(cnt_t.sum())) <= 2e-3 * cnt_t.sum(), (frac_rays_same, cnt_m.sum(), cnt_t.sum())
     assert np.abs(N(r.colors) - ref["val_colors"]).max() <= 0.03
     assert np.median(np.abs(N(r.colors) - ref["val_colors"])) <= 3e-3
     assert np.median(np.abs(N(r.depth) - ref["val_depth"]) / (np.abs(ref["val_depth"]) + 1e-3)) <= 1e-2
     if same_mask:
-        assert np.median(np.abs(N(r.weights) - ref["val_weights"])) <= 1e-3
+        assert np.median(np.abs(stored_rows(ref, N(r.weights), "val_idx_start_end") - ref["val_weights"])) <= 1e-3
 
 
 def test_edge_samples_vs_reference(ref):
@@ -146,7 +152,7 @@ def test_edge_samples_vs_reference(ref):
     np.testing.assert_array_equal(N(idx), ref["edge_anchors"])
     diff = np.abs(N(pts).astype(np.float64) - ref["edge_pts"].astype(np.float64))
     json.dump(dict(max_abs=float(diff.max()), frac_bit_exact=float((N(pts).view(np.uint32) == ref["edge_pts"].view(np.uint32)).mean())),
-              open(os.path.join(ROOT, "gpurun_out", "ref_edge_samples.json"), "w"))
+              open(diag_path("ref_edge_samples.json"), "w"))
     np.testing.assert_array_equal(N(pts).view(np.uint32), ref["edge_pts"].view(np.uint32))       # bit-exact
     torch.manual_seed(4242)                                       # same Philox stream => identical draws through our mirror
     e_pts, e_idx = sampler.GetEdgeSamples(8192)
@@ -168,9 +174,9 @@ def test_render_train_vs_reference(ref):
     r = renderer.Render(rays_o, rays_d, None, emb_idx)
     sr = renderer.sample_result_
     np.testing.assert_array_equal(N(sr.pts_idx_bounds), ref["train_bounds"])
-    np.testing.assert_array_equal(N(sr.anchors)[:, :2], ref["train_anchors"])
+    np.testing.assert_array_equal(stored_rows(ref, N(sr.anchors)[:, :2], "train_bounds"), ref["train_anchors"])
     for k, v in (("train_t", sr.t), ("train_dt", sr.dt), ("train_pts", sr.pts)):
-        np.testing.assert_array_equal(N(v).view(np.uint32), ref[k].view(np.uint32), err_msg=k)
+        np.testing.assert_array_equal(stored_rows(ref, N(v), "train_bounds").view(np.uint32), ref[k].view(np.uint32), err_msg=k)
     # octree occupancy state after UpdateOctNodes: votes depend on the (fp16-noisy) early weights through
     # thresholds, so allow a tiny number of flipped votes but require byte equality of everything else
     for mine, theirs in ((sampler.tree_weight_stats_, "train_weight_stats_after"), (sampler.tree_alpha_stats_, "train_alpha_stats_after"),
@@ -204,13 +210,13 @@ def test_render_train_vs_reference(ref):
                                      frac_rows_close=float(row_close.mean()), frac_rows_close_a=float(row_close[:, 0].mean()),
                                      frac_rows_close_b=float(row_close[:, 1].mean()),
                                      per_channel_cos=[cs(ef_m[..., k], ef_t[..., k]) for k in range(16)])
-        json.dump(summary, open(os.path.join(ROOT, "gpurun_out", "ref_edge_feats.json"), "w"), indent=1)
+        json.dump(summary, open(diag_path("ref_edge_feats.json"), "w"), indent=1)
         # identical edge points (RNG-stream parity incl. the reference's torch::rand output buffers): fp16 MLP noise only
         assert summary["edge_feats"]["cos_ours_ref"] >= 0.999 and summary["edge_feats"]["frac_rows_close"] >= 0.97, summary["edge_feats"]
     if "grad_feat_pool" in ref:
         table_pair = (field.feat_pool_.grad.reshape(-1), ref["grad_feat_pool"])
     else:                                             # committed fixture: a seeded 2^18-element subsample of the live prefix
-        sub = torch.from_numpy(ref["grad_feat_pool_sub_idx"]).cuda()
+        sub = torch.from_numpy(ref["grad_feat_pool_sub_idx"]).long().cuda()
         table_pair = (field.feat_pool_.grad.reshape(-1)[sub], ref["grad_feat_pool_sub_val"])
     for name, mine, theirs in (("field_mlp", field.mlp_.params_.grad, ref["grad_field_mlp"]),
                                ("shader_mlp", shader.mlp_.params_.grad, ref["grad_shader_mlp"]),
@@ -225,7 +231,7 @@ def test_render_train_vs_reference(ref):
         mine_flat = field.feat_pool_.grad.reshape(-1).double()
         norms = np.array([float(torch.linalg.norm(mine_flat[l * S:(l + 1) * S])) for l in range(17)])
         summary["slab_norm_ratio"] = (norms / np.maximum(ref["grad_feat_pool_slab_norm"].astype(np.float64), 1e-30)).tolist()
-        json.dump(summary, open(os.path.join(ROOT, "gpurun_out", "golden_grad_parity.json"), "w"), indent=1)
+        json.dump(summary, open(diag_path("golden_grad_parity.json"), "w"), indent=1)
         for name in ("field_mlp", "shader_mlp", "app_emb"):
             assert summary[name]["cos"] >= 0.98 and summary[name]["rel_l2"] <= 0.2, (name, summary[name])
         assert summary["feat_pool"]["cos"] >= 0.97, summary
@@ -265,36 +271,42 @@ def test_render_train_vs_reference(ref):
                           norm_ref=float(np.linalg.norm(gref[sl])), norm_ours=float(np.linalg.norm(mine_flat[sl])),
                           nnz_ref=int((gref[sl] != 0).sum()), nnz_ours=int((mine_flat[sl] != 0).sum())))
     summary["feat_pool_slabs"] = slabs
-    json.dump(summary, open(os.path.join(ROOT, "gpurun_out", "ref_grad_parity.json"), "w"), indent=1)
+    json.dump(summary, open(diag_path("ref_grad_parity.json"), "w"), indent=1)
     for name in ("field_mlp", "shader_mlp", "app_emb"):
         assert summary[name]["cos"] >= 0.98 and summary[name]["rel_l2"] <= 0.2, (name, summary[name])
     assert summary["feat_pool_ours_vs_oracle_exact"] >= 0.995, summary
     # Ours equals the exact sum (oracle, double accumulation) to 1e-9; what is left against the reference is its own
     # fp16 noise (fp16 products + nondeterministic fp16 atomics + tcnn's fp16-accumulated dL/dinput), recorded per
-    # level-slab in gpurun_out/ref_grad_parity.json.  (Before the RNG-stream fix in f2nerf_b200/rng.py this cosine
+    # level-slab in ref_grad_parity.json (workloads.diag_path).  (Before the RNG-stream fix in f2nerf_b200/rng.py this cosine
     # was 0.78: the TV-loss edge points were different draws.)
     assert summary["feat_pool"]["cos"] >= 0.97, summary
 
 
-@pytest.mark.parametrize("ref", ["live"], indirect=True)
 def test_fused_adam_vs_reference_optimizer(ref):
     """SURVEY 8f N1: f2b_adam_step against the reference's own torch::optim::Adam (C++ frontend, ExpRunner.cpp:54,136)
-    stepping its own parameters with its own gradients twice — bit-identical parameters, table and MLP group."""
-    if "feat_pool_after_adam" not in ref:
-        pytest.skip("ref_driver without the optimizer dump")
+    stepping its own parameters with its own gradients twice — bit-identical parameters, table and MLP group.  A stored
+    run keeps the MLP vector whole and a sample of the table (its live prefix first, then a few dead elements)."""
     from f2nerf_b200._lib import call, stream
-    lr = float(ref["adam_lr"][0])
-    pool = ref["feat_pool_before_adam"].shape[0]
-    local = ((pool // 2 // 16) >> 4) << 4
-    for name, wd, n_live in (("feat_pool", 0.0, 17 * local), ("field_mlp", 1e-6, None)):
-        p, g = T(ref[name + "_before_adam"]).clone(), T(ref["grad_" + name].reshape(-1))
+    if "adam_feat_pool_idx" in ref:                  # a stored run: the sampled optimizer step
+        lr = float(ref["adam_lr"][0])
+        cases = [(name, ref[f"adam_{name}_before"], ref[f"adam_{name}_grad"], ref[f"adam_{name}_after"], wd, n_live)
+                 for name, wd, n_live in (("feat_pool", 0.0, int(ref["adam_feat_pool_n_live"][0])), ("field_mlp", 1e-6, None))]
+    else:
+        if "feat_pool_after_adam" not in ref:
+            pytest.skip("ref_driver without the optimizer dump")
+        lr = float(ref["adam_lr"][0])
+        pool = ref["feat_pool_before_adam"].shape[0]
+        local = ((pool // 2 // 16) >> 4) << 4
+        cases = [(name, ref[name + "_before_adam"], ref["grad_" + name].reshape(-1), ref[name + "_after_adam"], wd, n_live)
+                 for name, wd, n_live in (("feat_pool", 0.0, 17 * local), ("field_mlp", 1e-6, None))]
+    for name, before, grad, want, wd, n_live in cases:
+        p, g = T(before).clone(), T(np.ascontiguousarray(grad))
         m, v = torch.zeros_like(p), torch.zeros_like(p)
         n = p.numel()
         for step in (1, 2):
             call("f2b_adam_step", p, g, m, v, n, n if n_live is None else n_live, lr, 0.9, 0.99, 1e-15, wd, step, None, stream())
-        want = ref[name + "_after_adam"]
         got = N(p)
-        assert (got != ref[name + "_before_adam"]).any()
+        assert (got != before).any()
         np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32), err_msg=name)
 
 
@@ -317,7 +329,7 @@ def test_ray_generation_vs_reference(ref):
                    sample=[dict(row=int(r), ours=N(rays_d)[r].tolist(), ref=ref["rays_d"][r].tolist(), cam=int(ref["emb_idx"][r]),
                                 ij=ref["ray_ij"][r].tolist()) for r in np.nonzero(bad.any(1))[0][:3]],
                    dist_params=ref["ds_dist_params"][:3].tolist(), intri0=ref["ds_intri"][0].tolist(), pose0=ref["ds_poses"][0].tolist()),
-              open(os.path.join(ROOT, "gpurun_out", "ref_rays.json"), "w"))
+              open(diag_path("ref_rays.json"), "w"))
     np.testing.assert_array_equal(N(cam), ref["emb_idx"])
     np.testing.assert_array_equal(N(rays_o).view(np.uint32), ref["rays_o"].view(np.uint32))
     np.testing.assert_array_equal(N(rays_d).view(np.uint32), ref["rays_d"].view(np.uint32))
@@ -326,7 +338,7 @@ def test_ray_generation_vs_reference(ref):
     o2, d2 = gen.Img2WorldRayFlex(T(ref["emb_idx"].astype(np.int32)), T(ref["ray_ij"]))
     np.testing.assert_array_equal(N(d2).view(np.uint32), ref["rays_d"].view(np.uint32))
     json.dump(dict(dist_params_abs_max=float(np.abs(ref["ds_dist_params"]).max()), n_rays=int(N_RAYS)),
-              open(os.path.join(ROOT, "gpurun_out", "ref_rays.json"), "w"))
+              open(diag_path("ref_rays.json"), "w"))
 
 
 def _node_fields(blob):
@@ -355,7 +367,7 @@ def test_octree_maintenance_vs_reference(ref, oracle):
     theirs = ref["oct_nodes_invis"].view(np.int32).reshape(-1, 16)[:, 14]
     flips = int(((mine < 0) != (theirs < 0)).sum())
     json.dump(dict(nodes=int(m), invisible_ref=int((theirs < 0).sum()), invisible_ours=int((mine < 0).sum()), flips=flips),
-              open(os.path.join(ROOT, "gpurun_out", "ref_octree.json"), "w"))
+              open(diag_path("ref_octree.json"), "w"))
     assert flips <= max(1, m // 2000), flips                                     # fp32 visibility tests: borderline nodes only
     sampler.tree_nodes_gpu_ = T(ref["oct_nodes_invis"])                          # continue from the reference's own marks
     m = sampler.ProcOctree(True, False, False)
@@ -368,7 +380,8 @@ def test_sh_encode_bit_exact_vs_reference(ref):
     """f2b_sh_encode (and with it the fused shader-input epilogue, which shares the device function) == SHKenerl bit for bit."""
     from f2nerf_b200 import ops
     got = ops.sh_encode(T(ref["val_dirs"]))
-    np.testing.assert_array_equal(N(got).view(np.uint32), ref["val_sh"].view(np.uint32))
+    stride = int(ref["val_sh_stride"][0]) if "val_sh_stride" in ref else 1    # the fixture keeps every stride-th sample's SH
+    np.testing.assert_array_equal(N(got)[::stride].view(np.uint32), ref["val_sh"].view(np.uint32))
 
 
 def test_mark_invisible_vs_reference(ref, oracle):

@@ -19,6 +19,7 @@ import pytest
 import torch
 
 from test_gpu_parity import N, T
+from workloads import diag_path
 
 pytestmark = pytest.mark.gpu
 
@@ -42,8 +43,7 @@ def _run(kind):
         env["F2B_SHIM"] = "ops"
     r = subprocess.run([binary, os.path.join(ROOT, "oracle", "ref_config_ngp_fox.yaml"), out, str(N_RAYS), "0", "1"],
                        cwd=ROOT, capture_output=True, text=True, timeout=900, env=env)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    open(os.path.join(ROOT, "gpurun_out", f"shim_{kind}.log"), "w").write(r.stdout[-8000:] + "\n--- stderr ---\n" + r.stderr[-8000:])
+    open(diag_path(f"shim_{kind}.log"), "w").write(r.stdout[-8000:] + "\n--- stderr ---\n" + r.stderr[-8000:])
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
     if kind == "ops":
         assert "replaced by the B200 subclasses" in r.stdout

@@ -12,18 +12,25 @@ BASELINE.json `configs` -> the reference YAMLs they name (sampler / renderer / f
   synthetic  (round 1)   wanjinyou sampler on the synthetic 24-camera octree of tests/synth_scene.py
 
 Scene: the only dataset the reference ships is data/example/ngp_fox; its octree / warp / edge blobs, cameras and hash
-primes / biases as the UNMODIFIED reference built them are committed in tests/golden/ref_ngp_fox.npz (oracle/make_golden.py),
+primes / biases as the UNMODIFIED reference built them are committed in tests/golden/ref_ngp_fox.npz (oracle/make_golden.py; kept
+fixed so the benchmark's inputs do not move), while the reference-parity tests use a later run of the reference: the scene it built
+(tests/golden/ref_ngp_fox_run.npz: the same octree, warp weights equal to ~1e-7, its own random biases) and the dumps of a small
+seeded ray batch through it (tests/golden/ref_ngp_fox_rays.npz) and of its optimizer step (tests/golden/ref_ngp_fox_adam.npz),
 so every config runs on the reference's own ngp_fox geometry with that config's settings.  Rays are drawn like
 Dataset::RandRaysData (Dataset.cpp:287-289: camera / row / column from the CPU generator) so the compiled reference
 (oracle/_ref/ref_driver, seed 2023) marches the very same batch.  Parameters are initialised like oracle/ref_driver.cpp:76-83
 (table U(-1,1) from CPU generator 1234, field MLP x4, appearance embedding from the same generator).
 """
 import os
+import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_ngp_fox.npz")
+GOLD_RUN = os.path.join(ROOT, "tests", "golden", "ref_ngp_fox_run.npz")
+GOLD_RAYS = os.path.join(ROOT, "tests", "golden", "ref_ngp_fox_rays.npz")
+GOLD_ADAM = os.path.join(ROOT, "tests", "golden", "ref_ngp_fox_adam.npz")
 
 _W = dict(near=0.01, scale_by_dis=True, use_app_emb=True, sample_l=1.0 / 256)
 _F = dict(near=0.05, scale_by_dis=False, use_app_emb=False, sample_l=1.0 / 256)
@@ -48,6 +55,23 @@ def load_ngp_fox():
     bias_pool, ds_poses [n,12], ds_intri [n,9], ds_dist_params, ds_bounds, ds_hw, ds_train_set, scalars, level_scales."""
     g = dict(np.load(GOLD))
     return g
+
+
+def diag_path(name):
+    """Where a test writes its diagnostics (JSON summaries, subprocess logs): a directory under the system's temporary
+    directory, so that the suite also runs on a read-only tree."""
+    d = os.path.join(tempfile.gettempdir(), "f2b_test_diag")
+    os.makedirs(d, exist_ok=True)
+    return os.path.join(d, name)
+
+
+def load_golden(batch="ref_ngp_fox"):
+    """A reference-parity fixture (oracle/make_golden.py): the scene of the reference run, its dumps of the seeded ray batch and
+    a sample of its optimizer step, in one dict.  ``batch``: "ref_ngp_fox" (8 rays, every per-sample tensor) or
+    "ref_ngp_fox_512" (512 rays, per-sample tensors of the rays listed in ``sample_rays``)."""
+    d = os.path.join(ROOT, "tests", "golden")
+    return dict(np.load(os.path.join(d, batch + "_run.npz")), **np.load(os.path.join(d, batch + "_rays.npz")),
+                **np.load(os.path.join(d, batch + "_adam.npz")))
 
 
 def scene_blobs(cfg_name):

@@ -7,13 +7,12 @@ NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xptxas -v
 CSRC    := f2nerf_b200/csrc
 SRCS    := $(wildcard $(CSRC)/*.cu)
 OBJS    := $(patsubst $(CSRC)/%.cu,build/%.o,$(SRCS))
-DEFS    := $(if $(wildcard $(CSRC)/mlp_tc.cu),-DF2B_HAVE_TC,)
 
 all: f2nerf_b200/libf2nerf_b200.so oracle/libf2oracle.so
 
 build/%.o: $(CSRC)/%.cu $(wildcard $(CSRC)/*.cuh) include/f2nerf_b200.h
 	@mkdir -p build
-	$(NVCC) $(NVFLAGS) $(DEFS) -c $< -o $@ 2> build/$*.ptxas.log || (cat build/$*.ptxas.log; false)
+	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> build/$*.ptxas.log || (cat build/$*.ptxas.log; false)
 
 f2nerf_b200/libf2nerf_b200.so: $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS)

@@ -40,8 +40,6 @@ SIGNATURES = {
     "f2b_sampler_fill": [_P, c_int, _P, c_int, _P, _P, _P, c_int, c_float, c_float, c_float, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_sampler_march": [_P, c_int, _P, c_int, _P, _P, _P, c_int, c_float, c_float, c_float, c_int, c_int, c_int, _P, _P, _P, _P,
                           _P, _P, _P, _P, _P],
-    "f2b_sampler_march_bg": [_P, c_int, _P, c_int, _P, _P, _P, c_int, c_float, c_float, c_float, c_int, c_int, c_int, _P, _P, _P, _P,
-                             _P, _P, _P, _P, _P],
     "f2b_sampler_gather": [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_edge_samples": [_P, _P, _P, _P, c_int, _P, _P, _P],
     "f2b_oct_mark_visit": [_P, c_int, _P, c_int, _P, _P, _P, _P, _P, _P, _P],
@@ -60,11 +58,8 @@ SIGNATURES = {
     "f2b_mlp_bwd2": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_mlp_fwd_v0": [_P, _P, c_int, c_int, _P, _P, _P],
     "f2b_mlp_bwd_v0": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
-    "f2b_mlp_fwd_tc": [_P, _P, c_int, c_int, _P, _P, _P],
-    "f2b_mlp_bwd_tc": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_field_fwd": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P],
     "f2b_field_fwd_slots": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P],
-    "f2b_set_mlp_impl": [c_int],
     "f2b_get_mlp_impl": [],
     "f2b_cast_f32_to_f16": [_P, _P, c_i64, c_float, _P],
     "f2b_cast_f16_to_f32": [_P, _P, c_i64, c_float, _P],
@@ -121,7 +116,7 @@ class RenderArgs(ctypes.Structure):
         ("pts", _P), ("dirs", _P), ("dt", _P), ("t", _P), ("anchors", _P), ("feat_q", _P),
         ("edge_idx", _P), ("edge_coord", _P), ("e_pts", _P), ("e_anc", _P),
         ("pt_emb_idx", _P),
-        ("logit", _P), ("mlp_in", _P), ("f_hidden", _P), ("edge32", _P), ("raw", _P), ("rgb", _P), ("s_hidden", _P),
+        ("logit", _P), ("mlp_in", _P), ("edge32", _P), ("raw", _P), ("rgb", _P),
         ("colors", _P), ("disparity", _P), ("depth", _P), ("weights", _P),
         ("d_colors", _P), ("d_disparity", _P), ("d_depth", _P), ("d_weights", _P), ("d_edge", _P),
         ("gs_progress", _F), ("shader_loss_scale", _F), ("field_loss_scale", _F), ("table_grad_mul", _F),
@@ -175,8 +170,8 @@ def stream():
 
 # kernels launched per entry point (for bench.py's gpu_launches claim; memsets are not counted)
 KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_phase2_fwd": 10, "f2b_render_bwd": 8, "f2b_render_grad_finalize": 2,
-                    "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_sampler_march_bg": 2, "f2b_early_stop": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
-                    "f2b_abi_version": 0, "f2b_set_mlp_impl": 0, "f2b_get_mlp_impl": 0}
+                    "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_early_stop": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
+                    "f2b_abi_version": 0, "f2b_get_mlp_impl": 0}
 LAUNCHES = 0      # running count of product kernels launched through this binding
 TRACE = None      # set to a list to record (name, start_event, end_event, int_args) per call (bench.py)
 

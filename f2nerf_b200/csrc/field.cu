@@ -15,13 +15,12 @@
 #include "common.cuh"
 #include "hash.cuh"
 #include "tc.cuh"
-#include <stdlib.h>
 
 namespace f2b {
 using namespace tc;
 
 constexpr int kFT = 128;
-constexpr int kFieldDefaultMinB = 4;   // see DESIGN.md: 4 = max loads in flight per thread, 6 = max resident warps
+constexpr int kFieldDefaultMinB = 4;   // resident CTAs per SM the kernel is compiled for; see DESIGN.md
 
 struct FieldSmem {
   static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB
@@ -176,10 +175,9 @@ static int field_fwd_launch(const void* table_f16, const int* prim_pool, const f
   int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kFT);
-  static int minb = -1;                                           // resident CTAs per SM the kernel is compiled for
-  if (minb < 0) { const char* e = getenv("F2B_FIELD_MINB"); minb = e ? atoi(e) : kFieldDefaultMinB; }
-#define F2B_FIELD_LAUNCH(LO, MB)                                                                                      \
+#define F2B_FIELD_LAUNCH(LO)                                                                                          \
   {                                                                                                                   \
+    constexpr int MB = kFieldDefaultMinB;                                                                             \
     const int grid = n_tiles < sms * MB ? n_tiles : sms * MB;                                                         \
     cudaFuncSetAttribute(field_fwd_kernel<LO, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, FieldSmem::BYTES);    \
     field_fwd_kernel<LO, MB><<<grid, kFT, FieldSmem::BYTES, as_stream(stream)>>>(                                     \
@@ -187,11 +185,7 @@ static int field_fwd_launch(const void* table_f16, const int* prim_pool, const f
         vol_stride, n_pts, slot_counts, slot_size, out_f32, (__half*)feat_save_f16,                                  \
         LO ? nullptr : (__half*)hidden_save_f16);                                                                     \
   }
-  if (logit_only) {
-    if (minb >= 6) F2B_FIELD_LAUNCH(true, 6) else if (minb == 5) F2B_FIELD_LAUNCH(true, 5) else F2B_FIELD_LAUNCH(true, 4)
-  } else {
-    if (minb >= 6) F2B_FIELD_LAUNCH(false, 6) else if (minb == 5) F2B_FIELD_LAUNCH(false, 5) else F2B_FIELD_LAUNCH(false, 4)
-  }
+  if (logit_only) F2B_FIELD_LAUNCH(true) else F2B_FIELD_LAUNCH(false)
 #undef F2B_FIELD_LAUNCH
   return check_launch("f2b_field_fwd");
 }

@@ -8,7 +8,7 @@
 // slots + its 128 table gathers (SURVEY.md §8d "fused forward pipeline": 512 B/pt of gathers is the whole traffic).
 //
 // Shape: a "walker" (128 threads = one warpgroup, thread i == sample i) walks ONE RAY front to back, a 128-sample tile at a
-// time, and carries the ray's optical depth across tiles; a CTA holds one walker (optionally two independent ones sharing the weights).  Because the reference's early-stop mask `T_i > 1e-4`
+// time, and carries the ray's optical depth across tiles; a CTA is one walker.  Because the reference's early-stop mask `T_i > 1e-4`
 // (Renderer.cpp:125) is a prefix of the ray (tau >= 0 => T non-increasing), the walk simply ENDS at the first tile whose
 // leading sample is already opaque: the samples behind it are never encoded (the unfused path encodes every marched sample,
 // then drops them).  No occupancy votes are taken in VALIDATE mode, so nothing downstream needs those samples.
@@ -22,25 +22,23 @@
 #include "hash.cuh"
 #include "shader.cuh"
 #include "tc.cuh"
-#include <stdlib.h>
 
 namespace f2b {
 using namespace tc;
 
 constexpr int kRT = 128;
 
-// Shared memory of a CTA with NW independent ray walkers (128 threads each) that share the two MLPs' weights:
-//   [0, 20 KB) weights | per walker: A0 8 KB + H0 16 KB | barriers.  The composite's scratch (tau, optical depth, the five addend
-//   rows) lives inside the walker's H0 tile, which is dead whenever the scratch is live (between an MLP's last MMA and the next
-//   MLP's first epilogue).
-template <int NW>
+// Shared memory of a CTA (one ray walker, 128 threads):
+//   [0, 20 KB) the two MLPs' weights | A0 8 KB + H0 16 KB | ray ticket + level scales.  The composite's scratch (tau, optical
+//   depth, the five addend rows) lives inside the walker's H0 tile, which is dead whenever the scratch is live (between an MLP's
+//   last MMA and the next MLP's first epilogue).
 struct FusedSmem {
   static constexpr int SWH = 0;           // shader Wh   [64 x 64] SW128  8 KB
   static constexpr int FWO = 8192;        // field  Wout [16 x 64] SW128  2 KB
   static constexpr int SWO = 10240;       // shader Wout [16 x 64] SW128  2 KB
   static constexpr int FW0 = 12288;       // field  W0   [64 x 32] SW64   4 KB
   static constexpr int SW0 = 16384;       // shader W0   [64 x 32] SW64   4 KB
-  static constexpr int WALK0 = 20480;     // walker w: A0 at WALK0 + w * WALK, H0 behind it
+  static constexpr int WALK0 = 20480;     // the walker's A0, H0 behind it
   static constexpr int WALK = 8192 + 16384;
   static constexpr int A0 = 0;            // [128 x 32] f16 SW64   8 KB   encoded features, then the shader MLP's input rows
   static constexpr int H0 = 8192;         // [128 x 64] f16 SW128 16 KB   hidden activations (both MLPs, rewritten in place)
@@ -48,8 +46,8 @@ struct FusedSmem {
   static constexpr int ACC = H0 + 512;    // float acc[129]
   static constexpr int ADD = H0 + 2048;   // float add[5][128]
   static constexpr int ROWS = H0 + 4608;  // float rows[128][20]     (inside H0) an MLP's 16 outputs per sample
-  static constexpr int BAR = WALK0 + NW * WALK;   // per walker 16 B: ray ticket (4); then 16 B | 16 level scales
-  static constexpr int BYTES = BAR + 16 * NW + 16 + 64 + 1024;   // + alignment slack (the tiles need 1024-byte alignment)
+  static constexpr int BAR = WALK0 + WALK;        // 16 B: ray ticket (4); then 16 B | 16 level scales
+  static constexpr int BYTES = BAR + 16 + 16 + 64 + 1024;   // + alignment slack (the tiles need 1024-byte alignment)
 };
 
 template <int K>
@@ -63,25 +61,16 @@ __device__ __forceinline__ void stage_w_fused(const __half* __restrict__ w, int 
 
 __device__ __forceinline__ float h16(uint32_t acc_bits) { return __half2float(__float2half_rn(__uint_as_float(acc_bits))); }
 
-// barrier over the 128 threads of one walker (named barrier 1 + walker; barrier 0 stays the CTA-wide one)
-__device__ __forceinline__ void walker_sync(int w) {
-  if (w == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-  else asm volatile("bar.sync 2, 128;" ::: "memory");
-}
-__device__ __forceinline__ int walker_sync_count(int w, bool pred) {
+// barrier over the walker's 128 threads (named barrier 1; barrier 0 stays the CTA-wide one)
+__device__ __forceinline__ void walker_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ int walker_sync_count(bool pred) {
   int n;
-  if (w == 0)
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\tbar.red.popc.u32 %0, 1, 128, p;\n\t}\n" : "=r"(n) : "r"((int)pred) : "memory");
-  else
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\tbar.red.popc.u32 %0, 2, 128, p;\n\t}\n" : "=r"(n) : "r"((int)pred) : "memory");
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\tbar.red.popc.u32 %0, 1, 128, p;\n\t}\n" : "=r"(n) : "r"((int)pred) : "memory");
   return n;
 }
 
-// NW = 1 (default): the CTA is one walker (3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers); NW = 2: two
-// walkers share the 20 KB of weights (two CTAs, <= 128 registers, with spills) — more walkers to keep the gather pipe busy during each
-// other's MLP / composite phases, but fewer gathers in flight per thread.
-template <int NW>
-__global__ void __launch_bounds__(kRT * NW, NW == 2 ? 2 : 3)
+// 3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers.
+__global__ void __launch_bounds__(kRT, 3)
 render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool,
                         int n_volumes, int local_size, const __half* __restrict__ fparams, const __half* __restrict__ sparams,
                         const float* __restrict__ s_pts, const float* __restrict__ s_dt, const float* __restrict__ s_t,
@@ -89,14 +78,13 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
                         const float* __restrict__ bg, int n_rays, int slot, const int* __restrict__ total_all,
                         int* __restrict__ ticket, float* __restrict__ colors, float* __restrict__ disparity,
                         float* __restrict__ depth, int* __restrict__ kept_counts, float* __restrict__ weights_slots) {
-  using S = FusedSmem<NW>;
+  using S = FusedSmem;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int wk = threadIdx.x >> 7;                               // my walker
-  const int tid = threadIdx.x & 127;                             // thread within the walker == sample
-  unsigned char* wsm = sm + S::WALK0 + wk * S::WALK;
-  int* s_ray = reinterpret_cast<int*>(sm + S::BAR + 16 * wk);
-  float* s_scale = reinterpret_cast<float*>(sm + S::BAR + 16 * NW + 16);
+  const int tid = threadIdx.x;                                   // thread == sample
+  unsigned char* wsm = sm + S::WALK0;
+  int* s_ray = reinterpret_cast<int*>(sm + S::BAR);
+  float* s_scale = reinterpret_cast<float*>(sm + S::BAR + 16 + 16);
   float* s_tau = reinterpret_cast<float*>(wsm + S::TAU);
   float* s_acc = reinterpret_cast<float*>(wsm + S::ACC);         // exclusive optical depth per sample, [128] = inclusive end
   float* s_add = reinterpret_cast<float*>(wsm + S::ADD);         // [5][128] addends of the five per-ray sums
@@ -117,7 +105,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   Acc<16> acc_out;
   const bool empty_batch = total_all && (__ldg(total_all) <= 0);   // Renderer.cpp:83-97: no sample in the WHOLE batch
 
-  // one MMA group issued by the walker's warpgroup, which waits for it
+  // one MMA group issued by the CTA's warpgroup, which waits for it
 #define F2B_MMA_STAGE(...) \
   do {                     \
     wg_fence();            \
@@ -128,15 +116,15 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   // the walker's 16 outputs per sample -> my row (the rows sit in H0, the operand of the MMA just completed)
 #define F2B_OUT_ROW(r)                               \
   do {                                               \
-    walker_sync(wk);                                 \
+    walker_sync();                                   \
     acc_to_rows(acc_out, s_rows, kRowLd16, tid);     \
-    walker_sync(wk);                                 \
+    walker_sync();                                   \
     row_ld16(s_rows, kRowLd16, tid, r);              \
   } while (0)
 
   for (;;) {
     if (tid == 0) *s_ray = atomicAdd(ticket, 1);
-    walker_sync(wk);
+    walker_sync();
     const int ray = *s_ray;
     if (ray >= n_rays) break;
     const int cnt = __ldg(counts + ray);
@@ -165,12 +153,12 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       for (int c = 0; c < 4; c++)
         *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = make_uint4(enc[4 * c], enc[4 * c + 1], enc[4 * c + 2], enc[4 * c + 3]);
       fence_async_smem();
-      walker_sync(wk);                                           // (also: the previous tile's sums have been read out of H0)
+      walker_sync();                                             // (also: the previous tile's sums have been read out of H0)
       // ---- field MLP: 32 -> 64 (ReLU) -> 16 -------------------------------------------------------------------------
       F2B_MMA_STAGE(mma_m128<64, 0, 2>(acc, a0, 64, fw0, 64, false));
       acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
-      walker_sync(wk);
+      walker_sync();
       F2B_MMA_STAGE(mma_m128<16, 0, 4>(acc_out, h0, 128, fwo, 128, false));
       float feat[16];
       {
@@ -188,7 +176,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
         alpha = fsub(1.f, expf(-tau));
       }
       s_tau[tid] = tau;
-      walker_sync(wk);
+      walker_sync();
       if (tid == 0) {                                            // fixed trip count (lanes past nv hold tau = +0: x + 0 == x), so the
         float a = run;                                           // loads pipeline ahead of the 128-long dependent add chain
 #pragma unroll 16
@@ -196,10 +184,10 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
         s_acc[kRT] = a;
         run = a;
       }
-      walker_sync(wk);
+      walker_sync();
       const float trans = expf(-s_acc[tid < nv ? tid : 0]);
       const bool keep = valid && (trans > 1e-4f);
-      const int nk = walker_sync_count(wk, keep);                // kept samples are a prefix of the ray: the first nk of the tile
+      const int nk = walker_sync_count(keep);                    // kept samples are a prefix of the ray: the first nk of the tile
       if (tid == 0) run_end = s_acc[nk];
       if (nk == 0) break;                                        // the ray is opaque in front of this tile: done (walker-uniform)
       // ---- shader MLP input: [1, feat 1..15 | SH4(dir)] -> 64 -> 64 -> 16, colour activation --------------------------
@@ -210,16 +198,16 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
         for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = row[c];
       }
       fence_async_smem();
-      walker_sync(wk);                                           // (thread 0 has read acc[nk]: H0 may be overwritten again)
+      walker_sync();                                             // (thread 0 has read acc[nk]: H0 may be overwritten again)
       F2B_MMA_STAGE(mma_m128<64, 0, 2>(acc, a0, 64, sw0, 64, false));
       acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
-      walker_sync(wk);
+      walker_sync();
       F2B_MMA_STAGE(mma_m128<64, 0, 4>(acc, h0, 128, swh, 128, false));
-      walker_sync(wk);                                           // in place: every warp's part of the hidden layer's MMA has completed
+      walker_sync();                                             // in place: every warp's part of the hidden layer's MMA has completed
       acc_relu_to_tile(acc, wsm + S::H0, tid);
       fence_async_smem();
-      walker_sync(wk);
+      walker_sync();
       F2B_MMA_STAGE(mma_m128<16, 0, 4>(acc_out, h0, 128, swo, 128, false));
       {                                                          // (H0 is dead again: the five addend rows live in it)
         uint32_t r[16];
@@ -234,7 +222,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
         s_add[0 * 128 + tid] = fmul(w, cr); s_add[1 * 128 + tid] = fmul(w, cg); s_add[2 * 128 + tid] = fmul(w, cb);
         s_add[3 * 128 + tid] = fdiv(w, ts); s_add[4 * 128 + tid] = fmul(w, ts);
       }
-      walker_sync(wk);
+      walker_sync();
       if (tid < 5) {                                             // FlexOps::Sum order: serial, left to right; samples that are not
         const float* mine = s_add + tid * 128;                   // kept add +0 (w = 0), which leaves the running sum bit-identical
 #pragma unroll 16
@@ -244,9 +232,9 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       if (nk < nv) break;                                        // terminated inside this tile
     }
     // ---- per-ray results (Renderer.cpp:196-208; empty batch :83-97) -------------------------------------------------
-    walker_sync(wk);                                             // the sums above have been read out of the addend rows
+    walker_sync();                                               // the sums above have been read out of the addend rows
     if (tid < 5) s_add[tid] = acc5;
-    walker_sync(wk);
+    walker_sync();
     if (tid == 0) {
       const float lt = expf(-run_end);                           // last_trans = exp(-Sum(sec_density)) over the kept samples
       colors[ray * 3 + 0] = fadd(s_add[0], fmul(lt, bg[ray * 3 + 0]));
@@ -292,22 +280,13 @@ extern "C" int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool,
   int sms = 132;
   f2b_device_info(&sms, nullptr);
   if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("f2b_render_fwd_fused: memset failed"); return F2B_ECUDA; }
-  // ray walkers per CTA (F2B_FUSED_WALKERS): the default is one.
-  static int walkers = -1;
-  if (walkers < 0) { const char* e = getenv("F2B_FUSED_WALKERS"); walkers = (e && atoi(e) == 2) ? 2 : 1; }
-#define F2B_FUSED_LAUNCH(NW)                                                                                                      \
-  {                                                                                                                               \
-    cudaFuncSetAttribute(render_fwd_fused_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem<NW>::BYTES);        \
-    const int per_sm = resident_per_sm(render_fwd_fused_kernel<NW>, kRT * NW, FusedSmem<NW>::BYTES);                              \
-    const int want = div_up(n_rays, NW);                                                                                          \
-    const int grid = want < sms * per_sm ? want : sms * per_sm;                                                                   \
-    render_fwd_fused_kernel<NW><<<grid, kRT * NW, FusedSmem<NW>::BYTES, as_stream(stream)>>>(                                     \
-        (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,                  \
-        (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,    \
-        total_all, ticket, colors, disparity, depth, kept_counts, weights_slots);                                                 \
-  }
-  if (walkers == 2) F2B_FUSED_LAUNCH(2) else F2B_FUSED_LAUNCH(1)
-#undef F2B_FUSED_LAUNCH
+  cudaFuncSetAttribute(render_fwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem::BYTES);
+  const int per_sm = resident_per_sm(render_fwd_fused_kernel, kRT, FusedSmem::BYTES);
+  const int grid = n_rays < sms * per_sm ? n_rays : sms * per_sm;
+  render_fwd_fused_kernel<<<grid, kRT, FusedSmem::BYTES, as_stream(stream)>>>(
+      (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,
+      (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,
+      total_all, ticket, colors, disparity, depth, kept_counts, weights_slots);
   return check_launch("f2b_render_fwd_fused");
 }
 

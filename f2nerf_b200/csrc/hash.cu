@@ -15,7 +15,6 @@
 //   acc = w001*f001; acc = fma(w000,f000,acc); then fma in order 010,011,100,101,110,111.
 #include "common.cuh"
 #include "hash.cuh"
-#include <stdlib.h>
 
 namespace f2b {
 
@@ -225,8 +224,7 @@ extern "C" int f2b_hash_bwd_levels(const int* prim_pool, const float* bias_pool,
   int log2_levels = 0;
   while ((1 << log2_levels) < n_levels) log2_levels++;
   const int64_t n_tasks = int64_t(div_up(n_pts, 32)) * n_levels;           // one warp-task per (32 samples, level)
-  static int ctas_per_sm = -1;                                             // resident 256-thread CTAs per SM (F2B_SCATTER_CTAS, default 8 = all)
-  if (ctas_per_sm < 0) { const char* e = getenv("F2B_SCATTER_CTAS"); ctas_per_sm = e ? atoi(e) : 8; if (ctas_per_sm < 1) ctas_per_sm = 1; }
+  constexpr int ctas_per_sm = 8;                                           // resident 256-thread CTAs per SM: all of them
   int sms = 132;
   f2b_device_info(&sms, nullptr);
   const int64_t want = div_up(n_tasks * 32, int64_t(256));

@@ -253,8 +253,8 @@ static void launch_fwd(const void* in_f16, const void* params_f16, int n_pts, vo
       (const __half*)in_f16, (const __half*)params_f16, n_pts, (__half*)out_f16, out_f32, (__half*)hidden_save_f16, epi);
 }
 
-extern "C" int f2b_mlp_fwd_tc(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
-                              void* out_f16, void* hidden_save_f16, void* stream) {
+extern "C" int f2b_mlp_fwd(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
+                           void* out_f16, void* hidden_save_f16, void* stream) {
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(in_f16 && params_f16 && out_f16, "f2b_mlp_fwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_fwd: n_hidden_matmuls must be 0 or 1");
@@ -266,8 +266,8 @@ extern "C" int f2b_mlp_fwd_tc(const void* in_f16, const void* params_f16, int n_
 
 // Same network, output widened to fp32 in the epilogue (what TCNNWP::Query hands back, TCNNWP.cpp:112):
 // out_f32 [P,16] and/or out_f16 [P,16] (either may be NULL, not both).
-extern "C" int f2b_mlp_fwd_tc_f32(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
-                                  float* out_f32, void* out_f16, void* hidden_save_f16, void* stream) {
+extern "C" int f2b_mlp_fwd_f32(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
+                               float* out_f32, void* out_f16, void* hidden_save_f16, void* stream) {
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(in_f16 && params_f16 && (out_f32 || out_f16), "f2b_mlp_fwd_f32: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_fwd_f32: n_hidden_matmuls must be 0 or 1");
@@ -277,17 +277,16 @@ extern "C" int f2b_mlp_fwd_tc_f32(const void* in_f16, const void* params_f16, in
   return check_launch("f2b_mlp_fwd_f32(wgmma)");
 }
 
+// The public MLP entry points always run the wgmma kernels (1); the CUDA-core kernels are reached only as f2b_mlp_*_v0.
+extern "C" int f2b_get_mlp_impl(void) { return 1; }
+
 // Field MLP (32 -> 64 -> 16) on encoded features + the shading-feature assembly in its epilogue:
 // logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])).
-extern "C" int f2b_get_mlp_impl(void);
-#define F2B_REQUIRE_TC(name)                                                                                   \
-  if (f2b_get_mlp_impl() != 1) { set_error(name ": needs the tensor-core MLP implementation (F2B_MLP_IMPL=1)"); return F2B_EUNSUPPORTED; }
 
 extern "C" int f2b_field_shade_fwd(const void* feat_f16, const void* field_params_f16, const float* dirs, const float* app_emb,
                                    const int* pt_emb_idx, int n_pts, float* logit, void* mlp_in_f16, void* hidden_save_f16,
                                    void* stream) {
   if (n_pts <= 0) return F2B_OK;
-  F2B_REQUIRE_TC("f2b_field_shade_fwd")
   F2B_REQUIRE(feat_f16 && field_params_f16 && dirs && logit && mlp_in_f16, "f2b_field_shade_fwd: null pointer");
   F2B_REQUIRE(!app_emb || pt_emb_idx, "f2b_field_shade_fwd: app_emb without pt_emb_idx");
   EpiArgs e = {};
@@ -301,7 +300,6 @@ extern "C" int f2b_field_shade_fwd(const void* feat_f16, const void* field_param
 extern "C" int f2b_shader_mlp_rgb_fwd(const void* mlp_in_f16, const void* shader_params_f16, int n_pts, void* raw_f16,
                                       float* rgb, void* hidden_save_f16, void* stream) {
   if (n_pts <= 0) return F2B_OK;
-  F2B_REQUIRE_TC("f2b_shader_mlp_rgb_fwd")
   F2B_REQUIRE(mlp_in_f16 && shader_params_f16 && raw_f16 && rgb, "f2b_shader_mlp_rgb_fwd: null pointer");
   EpiArgs e = {};
   e.rgb = rgb;

@@ -356,9 +356,9 @@ mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
 
 using namespace f2b;
 
-extern "C" int f2b_mlp_bwd2_tc(const void* dout_f16, const void* in_f16, const void* hidden0_f16, const void* hidden1_f16,
-                               const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16,
-                               float* dparams_f32, void* stream) {
+extern "C" int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void* hidden0_f16, const void* hidden1_f16,
+                            const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16,
+                            float* dparams_f32, void* stream) {
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(dout_f16 && in_f16 && params_f16 && dparams_f32, "f2b_mlp_bwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_bwd: n_hidden_matmuls must be 0 or 1");
@@ -394,12 +394,12 @@ extern "C" int f2b_mlp_bwd2_tc(const void* dout_f16, const void* in_f16, const v
   return check_launch("f2b_mlp_bwd(wgmma)");
 }
 
-extern "C" int f2b_mlp_bwd_tc(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,
-                              const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16,
-                              float* dparams_f32, void* stream) {
+extern "C" int f2b_mlp_bwd(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,
+                           const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16,
+                           float* dparams_f32, void* stream) {
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(hidden_save_f16, "f2b_mlp_bwd: null pointer");
   const __half* h = (const __half*)hidden_save_f16;
-  return f2b_mlp_bwd2_tc(dout_f16, in_f16, h, h + size_t(n_hidden_matmuls ? 1 : 0) * n_pts * 64, params_f16, n_hidden_matmuls, n_pts,
-                         din_f16, dparams_f32, stream);
+  return f2b_mlp_bwd2(dout_f16, in_f16, h, h + size_t(n_hidden_matmuls ? 1 : 0) * n_pts * 64, params_f16, n_hidden_matmuls, n_pts,
+                      din_f16, dparams_f32, stream);
 }

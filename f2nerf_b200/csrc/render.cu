@@ -86,18 +86,17 @@ extern "C" int f2b_render_phase2_fwd(const f2b_render* r) {
   F2B_TRY(f2b_cast_f32_to_f16(r->field_params, r->fparams16, r->n_field_params, 1.f, r->stream));
   F2B_TRY(f2b_cast_f32_to_f16(r->shader_params, r->sparams16, r->n_shader_params, 1.f, r->stream));
   F2B_TRY(f2b_field_shade_fwd(r->feat_q, r->fparams16, r->dirs, emb ? r->app_emb : nullptr, emb ? r->pt_emb_idx : nullptr, (int)nk,
-                              r->logit, r->mlp_in, r->f_hidden, r->stream));
+                              r->logit, r->mlp_in, nullptr, r->stream));
   if (ne > 0)
-    F2B_TRY(f2b_mlp_fwd_f32(off(r->feat_q, nk * 64), r->fparams16, 0, (int)ne, r->edge32, nullptr,
-                            r->f_hidden ? off(r->f_hidden, nk * 128) : nullptr, r->stream));
-  F2B_TRY(f2b_shader_mlp_rgb_fwd(r->mlp_in, r->sparams16, (int)nk, r->raw, r->rgb, r->s_hidden, r->stream));
+    F2B_TRY(f2b_mlp_fwd_f32(off(r->feat_q, nk * 64), r->fparams16, 0, (int)ne, r->edge32, nullptr, nullptr, r->stream));
+  F2B_TRY(f2b_shader_mlp_rgb_fwd(r->mlp_in, r->sparams16, (int)nk, r->raw, r->rgb, nullptr, r->stream));
   return f2b_composite_fwd(r->logit, 1, r->rgb, r->dt, r->t, r->new_bounds, r->bg, r->n_rays, r->colors, r->disparity, r->depth,
                            r->weights, r->stream);
 }
 
 extern "C" int f2b_render_bwd(const f2b_render* r) {
   F2B_REQUIRE(r, "f2b_render_bwd: null argument block");
-  // f_hidden / s_hidden NULL: the forward saved no hidden activations, f2b_mlp_bwd2 rebuilds them (recompute, tensor-core only)
+  // the forward saved no hidden activations: f2b_mlp_bwd2 (hidden0 == NULL) rebuilds them from the input rows
   const int64_t nk = r->n_kept, ne = 2 * int64_t(r->n_edge_pairs), nq = nk + ne;
   cudaStream_t st = as_stream(r->stream), side = as_stream(r->side_stream);
   const bool emb = r->app_emb && r->ray_emb_idx;
@@ -114,14 +113,13 @@ extern "C" int f2b_render_bwd(const f2b_render* r) {
     F2B_TRY(f2b_composite_act_bwd(r->logit, 1, r->rgb, r->dt, r->t, r->new_bounds, r->bg, r->n_rays, r->d_colors, r->d_disparity,
                                   r->d_depth, r->d_weights, r->gs_progress, r->raw, r->shader_loss_scale, r->d_logit, 1, r->d_raw,
                                   r->stream));
-    F2B_TRY(f2b_mlp_bwd2(r->d_raw, r->mlp_in, r->s_hidden, r->s_hidden ? off(r->s_hidden, nk * 128) : nullptr, r->sparams16, 1, (int)nk, r->d_in16, r->d_sparams,
-                         r->stream));
+    F2B_TRY(f2b_mlp_bwd2(r->d_raw, r->mlp_in, nullptr, nullptr, r->sparams16, 1, (int)nk, r->d_in16, r->d_sparams, r->stream));
     F2B_TRY(f2b_shader_prep_bwd_f16(r->d_in16, r->d_logit, r->new_bounds, emb ? r->ray_emb_idx : nullptr, r->n_rays,
                                     1.f / r->shader_loss_scale, r->field_loss_scale, r->d_scene16, emb ? r->d_app : nullptr, r->stream));
-    F2B_TRY(f2b_mlp_bwd2(r->d_scene16, r->feat_q, r->f_hidden, nullptr, r->fparams16, 0, (int)nk, r->dfeat16, r->d_fparams, r->stream));
+    F2B_TRY(f2b_mlp_bwd2(r->d_scene16, r->feat_q, nullptr, nullptr, r->fparams16, 0, (int)nk, r->dfeat16, r->d_fparams, r->stream));
   }
   if (ne > 0)
-    F2B_TRY(f2b_mlp_bwd2(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), r->f_hidden ? off(r->f_hidden, nk * 128) : nullptr, nullptr, r->fparams16, 0, (int)ne,
+    F2B_TRY(f2b_mlp_bwd2(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), nullptr, nullptr, r->fparams16, 0, (int)ne,
                          off(r->dfeat16, nk * 64), r->d_fparams, r->stream));
   if (r->scatter_mode != 0) return F2B_OK;
   // the scatter (L2 reductions) on the side stream behind the dense chain, joined before returning

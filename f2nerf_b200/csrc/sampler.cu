@@ -11,23 +11,20 @@
 //  * traversal and march are ONE kernel: the DFS is a coroutine that yields the next leaf hit
 //    when the march walks off the current leaf, so the (node, near, far) hit list is never
 //    written to HBM and the reference's first host sync (.item() at :353) disappears;
-//  * 4 lanes cooperate on one ray: each lane owns 3 of the 12 perspective projections, the
-//    3x12 mixing sums are finished with two xor-shuffles.  This split is exactly the summation
-//    tree Eigen's unrolled redux produces in the reference build
+//  * 16 lanes (half a warp) cooperate on one ray, two rays per warp: 12 lanes each evaluate one of
+//    the 12 perspective projections, then each lane forms one of the 3x4 mixing sums serially in
+//    exactly the summation tree Eigen's unrolled redux produces in the reference build
 //    ((p0+(p1+p2)) + (p3+(p4+p5))) + ((p6+(p7+p8)) + (p9+(p10+p11))), so every fp32 rounding —
 //    and hence every sample count / index — is bit-identical to the reference kernel
 //    (sequence read off the reference's PTX; see DESIGN.md §march-rounding);
-//  * 4x more warps than thread-per-ray and a 3x shorter dependent chain per step;
+//  * 16x more warps than thread-per-ray and a much shorter dependent chain per step;
 //  * DFS stack lives in shared memory (packed node<<4|cursor, one private copy per lane so no
 //    intra-group ordering is assumed), not 192 B/thread of local memory.
 #include "common.cuh"
 #include "scan.cuh"
-#include <stdlib.h>
 
 namespace f2b {
 
-constexpr int kLanesPerRay = 4;
-constexpr int kRaysPerBlock = 8;            // one warp per block: 512 blocks for 4096 rays
 constexpr int kMaxDepth = 24;               // reference MAX_STACK_SIZE 48 = 24 (node, cursor) pairs
 constexpr int kStackPitch = kMaxDepth + 1;  // 25 is odd: conflict-free across the 32 lanes
 
@@ -117,188 +114,9 @@ __device__ __forceinline__ bool next_hit(Dfs& s, const TreeNode* __restrict__ no
   return false;
 }
 
-// Per-lane slice of one TransInfo: 3 projections + the matching 3 columns of the 3x12 weight.
-struct TransSlice {
-  float a[3][4], b[3][4];   // w2xz rows 0/1
-  float w[3][3];            // w[r][j] = weight[r][3*sub + j]
-  float c[3];
-  float dis;
-};
-
-__device__ __forceinline__ void load_slice(const TransInfo* __restrict__ T, int sub, TransSlice& s) {
-  const float4* p = reinterpret_cast<const float4*>(&T->w2xz[3 * sub][0]);
-#pragma unroll
-  for (int j = 0; j < 3; j++) {
-    const float4 ra = __ldg(p + 2 * j), rb = __ldg(p + 2 * j + 1);
-    s.a[j][0] = ra.x; s.a[j][1] = ra.y; s.a[j][2] = ra.z; s.a[j][3] = ra.w;
-    s.b[j][0] = rb.x; s.b[j][1] = rb.y; s.b[j][2] = rb.z; s.b[j][3] = rb.w;
-  }
-#pragma unroll
-  for (int r = 0; r < 3; r++)
-#pragma unroll
-    for (int j = 0; j < 3; j++) s.w[r][j] = __ldg(&T->weight[r][3 * sub + j]);
-  const float4 cd = __ldg(reinterpret_cast<const float4*>(&T->center[0]));
-  s.c[0] = cd.x; s.c[1] = cd.y; s.c[2] = cd.z; s.dis = cd.w;
-}
-
-// sum of the 4 lane partials in the reference's tree order: (g0+g1) + (g2+g3).  xor 1 / xor 2 stay inside
-// the ray's 4-lane group; the whole warp executes them together (constant full mask).
-__device__ __forceinline__ float group_sum(float g) {
-  g = fadd(g, __shfl_xor_sync(0xffffffffu, g, 1));
-  g = fadd(g, __shfl_xor_sync(0xffffffffu, g, 2));
-  return g;
-}
-
-template <int MODE>   // 0: count only, 1: fill at pts_idx_bounds, 2: one pass into per-ray scratch slots of 1024 samples
-__global__ void __launch_bounds__(kRaysPerBlock* kLanesPerRay)
-march_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__ trans,
-             const float* __restrict__ rays_o, const float* __restrict__ rays_d,
-             const float* __restrict__ rays_noise, int n_rays, float near0, float far0,
-             float sample_l, int scale_by_dis, int max_hits, int count_all_hits,
-             int* __restrict__ ray_counts,            // count pass out
-             int* __restrict__ total_hits,            // count pass out (atomic)
-             const int* __restrict__ bounds,          // fill pass in
-             float* __restrict__ o_pts, float* __restrict__ o_dirs, float* __restrict__ o_dt,
-             float* __restrict__ o_t, int* __restrict__ o_anchors,
-             float* __restrict__ first_oct_dis) {
-  __shared__ int s_stack[kRaysPerBlock * kLanesPerRay * kStackPitch];
-  const int lane = threadIdx.x;
-  const int sub = lane & (kLanesPerRay - 1);
-  const int ray_local = lane / kLanesPerRay;
-  int ray = blockIdx.x * kRaysPerBlock + ray_local;
-  const bool active = ray < n_rays;
-  if (!active) ray = n_rays - 1;                       // keep the warp converged for shuffles
-
-  const float o[3] = {__ldg(rays_o + ray * 3), __ldg(rays_o + ray * 3 + 1), __ldg(rays_o + ray * 3 + 2)};
-  const float d[3] = {__ldg(rays_d + ray * 3), __ldg(rays_d + ray * 3 + 1), __ldg(rays_d + ray * 3 + 2)};
-  const float* noise = rays_noise + ray;
-
-  Dfs dfs;
-  dfs.stack = s_stack + lane * kStackPitch;
-  dfs.sp = 0; dfs.n_hits = 0; dfs.max_hits = max_hits;
-  dfs.st = (int(d[0] > 0.f) << 2) | (int(d[1] > 0.f) << 1) | int(d[2] > 0.f);
-  dfs.stack[0] = 0;                                    // root, cursor -1
-
-  constexpr bool FILL = MODE != 0;
-  int cap = F2B_MAX_SAMPLE_PER_RAY;
-  size_t out_base = 0;
-  if (MODE == 1) {
-    out_base = bounds[ray * 2];
-    cap = bounds[ray * 2 + 1] - int(out_base);
-  } else if (MODE == 2) {
-    out_base = size_t(ray) * F2B_MAX_SAMPLE_PER_RAY;
-  }
-
-  Hit hit;
-  hit.node = 0; hit.trans_idx = 0; hit.near = 0.f; hit.far = 0.f;
-  bool have = next_hit(dfs, nodes, o, d, near0, far0, hit);
-  if (FILL && active && sub == 0) first_oct_dis[ray] = have ? hit.near : 1e9f;
-
-  int k = 0;
-  {
-    float t = hit.near, far = hit.far;
-    int cur_node = hit.node, cur_trans = hit.trans_idx, loaded_trans = -1;
-    bool first = true;
-    TransSlice ts = {};
-    float rclip = 1.f;
-    // Warp-uniform loop: every lane executes every step's arithmetic and its full-mask shuffles until the
-    // slowest ray of the warp is done (finished rays compute on stale values, all side effects are
-    // predicated on `running`).  Partial-mask shuffles inside a data-dependent loop cost a
-    // WARPSYNC.COLLECTIVE each (~30 per step); with a constant full mask they are plain SHFL.BFLY.
-    bool running = have && cap > 0;
-    while (__any_sync(0xffffffffu, running)) {
-      if (running && cur_trans != loaded_trans) {
-        load_slice(trans + cur_trans, sub, ts);
-        loaded_trans = cur_trans;
-        // cur_radius = |o - center| / dis_summary, clipped at 1   (PersSampler.cu:262-263)
-        const float ex = fsub(o[0], ts.c[0]), ey = fsub(o[1], ts.c[1]), ez = fsub(o[2], ts.c[2]);
-        const float nrm = fsqrt(ffma(ex, ex, ffma(ey, ey, fmul(ez, ez))));
-        rclip = fmaxf(fdiv(nrm, ts.dis), 1.f);
-      }
-      const float X = ffma(t, d[0], o[0]), Y = ffma(t, d[1], o[1]), Z = ffma(t, d[2], o[2]);
-      // my 3 projections: xz = A_i * [x;1], jac row = (1/z) A_i[0,:3] - (x/z^2) A_i[1,:3]
-      float T0[3], T1[3], T2[3], V[3];
-#pragma unroll
-      for (int j = 0; j < 3; j++) {
-        const float xz0 = fadd(ffma(X, ts.a[j][0], fmul(Y, ts.a[j][1])), ffma(Z, ts.a[j][2], ts.a[j][3]));
-        const float xz1 = fadd(ffma(X, ts.b[j][0], fmul(Y, ts.b[j][1])), ffma(Z, ts.b[j][2], ts.b[j][3]));
-        const float r = frcp(xz1);
-        const float q = fdiv(-xz0, fmul(xz1, xz1));
-        T0[j] = ffma(ts.a[j][0], r, fmul(ts.b[j][0], q));
-        T1[j] = ffma(r, ts.a[j][1], fmul(q, ts.b[j][1]));
-        T2[j] = ffma(r, ts.a[j][2], fmul(q, ts.b[j][2]));
-        if (FILL) V[j] = fdiv(xz0, xz1);
-      }
-      float proj[3];
-#pragma unroll
-      for (int r = 0; r < 3; r++) {
-        const float j0 = group_sum(ffma(ts.w[r][0], T0[0], ffma(ts.w[r][1], T0[1], fmul(ts.w[r][2], T0[2]))));
-        const float j1 = group_sum(ffma(ts.w[r][0], T1[0], ffma(ts.w[r][1], T1[1], fmul(ts.w[r][2], T1[2]))));
-        const float j2 = group_sum(ffma(ts.w[r][0], T2[0], ffma(ts.w[r][1], T2[1], fmul(ts.w[r][2], T2[2]))));
-        proj[r] = ffma(j0, d[0], ffma(j1, d[1], fmul(j2, d[2])));
-      }
-      float w[3] = {0.f, 0.f, 0.f};
-      if (FILL) {
-#pragma unroll
-        for (int r = 0; r < 3; r++)
-          w[r] = group_sum(ffma(ts.w[r][0], V[0], ffma(ts.w[r][1], V[1], fmul(ts.w[r][2], V[2]))));
-      }
-      const float den = fadd(fsqrt(ffma(proj[0], proj[0], ffma(proj[1], proj[1], fmul(proj[2], proj[2])))), 1e-6f);
-      float step = fdiv(fmul(sample_l, __ldg(noise + k)), den);
-      if (scale_by_dis) step = fmul(rclip, step);
-
-      if (running) {
-        if (!first) {
-          if (FILL && active) {
-            const size_t idx = out_base + k;
-            if (sub == 0) {
-              o_pts[idx * 3] = w[0]; o_pts[idx * 3 + 1] = w[1]; o_pts[idx * 3 + 2] = w[2];
-            } else if (sub == 1) {
-              if (MODE == 1) { o_dirs[idx * 3] = d[0]; o_dirs[idx * 3 + 1] = d[1]; o_dirs[idx * 3 + 2] = d[2]; }
-            } else if (sub == 2) {
-              o_dt[idx] = fmul(step, den);
-              o_t[idx] = t;
-            } else {
-              if (MODE == 1) { o_anchors[idx * 3] = cur_trans; o_anchors[idx * 3 + 1] = cur_node; o_anchors[idx * 3 + 2] = 0; }
-              else { o_anchors[idx * 2] = cur_trans; o_anchors[idx * 2 + 1] = cur_node; }
-            }
-          }
-          k++;
-        }
-        // advance; hop leaves with an integer multiple of the step (PersSampler.cu:291-303; the
-        // reference build contracts cur_t + step*float(n) into one fma)
-        float tn = fadd(t, step);
-        if (tn > far) {
-          for (;;) {
-            have = next_hit(dfs, nodes, o, d, near0, far0, hit);
-            if (!have) break;
-            far = hit.far; cur_node = hit.node; cur_trans = hit.trans_idx;
-            const float nf = ceilf(fmaxf(fdiv(fsub(hit.near, t), step), 1.f));
-            const int n = (int)nf;                       // cvt.rzi.s32.f32 (saturating)
-            tn = ffma(step, (float)n, t);
-            if (!(tn > far)) break;
-          }
-        }
-        t = tn;
-        first = false;
-        running = (k < cap) && have;
-      }
-    }
-  }
-  if (MODE != 1) {
-    if (count_all_hits) {                                      // exact n_all_oct_intersect (:353,378), informational EMA only
-      while (next_hit(dfs, nodes, o, d, near0, far0, hit)) {}
-    }
-    if (active && sub == 0) {
-      ray_counts[ray] = k;
-      if (dfs.n_hits) atomicAdd(total_hits, dfs.n_hits);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------
-// 16-lane variant: two rays per warp => 4x the warps of the 4-lane kernel (the march is latency bound: at
-// 4 lanes/ray 4096 rays are only 512 warps on 592 SM sub-partitions).  Each step has two phases:
+// The march: two rays per warp, 16 lanes each (the march is latency bound: at 4 lanes/ray 4096 rays would be
+// only 512 warps on 528 SM sub-partitions).  Each step has two phases:
 //   A  lane g < 12 evaluates perspective projection g: xz, 1/xz1, the Jacobian factors T0..T2 and the value V;
 //   B  the 4 x 12 block {T0,T1,T2,V} x projections is transposed through 192 B of shared memory and lane
 //      (r, c) = (g >> 2, g & 3) forms ONE of the 12 mixing sums S[r][c] = sum_i weight[r][i] * T_c[i] serially
@@ -311,12 +129,8 @@ march_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__ t
 constexpr int kL16 = 16;
 constexpr int kRaysPerBlock16 = 2;
 
-// LEAN: the same kernel compiled for <= 64 registers (13 words of spill) for the software-pipelined march of the NEXT batch, which
-// shares the SMs with this batch's backward: at 96 registers its 14 resident one-warp CTAs per SM hold 43 k of the 64 k registers
-// and halve the occupancy of everything that runs beside it (r02d timeline: compaction 0.15 -> 0.35 ms, composite backward 0.14 ->
-// 0.33 ms); identical arithmetic, identical results.
-template <int MODE, bool LEAN = false>
-__global__ void __launch_bounds__(32, LEAN ? 32 : 1)
+template <int MODE>   // 0: count only, 1: fill at pts_idx_bounds, 2: one pass into per-ray scratch slots of 1024 samples
+__global__ void __launch_bounds__(32, 1)
 march16_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__ trans,
                const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                const float* __restrict__ rays_noise, int n_rays, float near0, float far0,
@@ -611,21 +425,8 @@ __global__ void update_stats_kernel(int n_nodes, const int* __restrict__ vote_w,
 
 using namespace f2b;
 
-static int march_lanes() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("F2B_MARCH_LANES"); v = (e && atoi(e) == 4) ? 4 : 16; }
-  return v;
-}
-#define F2B_LAUNCH_MARCH(MODE, st, ...)                                                                   \
-  do {                                                                                                    \
-    if (march_lanes() == 4) march_kernel<MODE><<<div_up(n_rays, kRaysPerBlock), kRaysPerBlock * kLanesPerRay, 0, st>>>(__VA_ARGS__); \
-    else march16_kernel<MODE><<<div_up(n_rays, kRaysPerBlock16), 32, 0, st>>>(__VA_ARGS__);               \
-  } while (0)
-
-static int march_slots(bool lean, const void* tree_nodes, int n_nodes, const void* trans, int n_trans, const float* rays_o,
-                       const float* rays_d, const float* rays_noise, int n_rays, float near, float far, float sample_l,
-                       int scale_by_dis, int max_oct_intersect_per_ray, int count_all_hits, float* s_pts, float* s_dt, float* s_t,
-                       int* s_anchors, int* ray_counts, int* pts_idx_bounds, int* totals, float* first_oct_dis, void* stream);
+#define F2B_LAUNCH_MARCH(MODE, st, ...) \
+  march16_kernel<MODE><<<div_up(n_rays, kRaysPerBlock16), 32, 0, st>>>(__VA_ARGS__)
 
 extern "C" int f2b_sampler_count(const void* tree_nodes, int n_nodes, const void* trans, int n_trans,
                                  const float* rays_o, const float* rays_d, const float* rays_noise,
@@ -669,27 +470,6 @@ extern "C" int f2b_sampler_march(const void* tree_nodes, int n_nodes, const void
                                  int max_oct_intersect_per_ray, int count_all_hits, float* s_pts, float* s_dt,
                                  float* s_t, int* s_anchors, int* ray_counts, int* pts_idx_bounds, int* totals,
                                  float* first_oct_dis, void* stream) {
-  return march_slots(false, tree_nodes, n_nodes, trans, n_trans, rays_o, rays_d, rays_noise, n_rays, near, far, sample_l, scale_by_dis,
-                     max_oct_intersect_per_ray, count_all_hits, s_pts, s_dt, s_t, s_anchors, ray_counts, pts_idx_bounds, totals,
-                     first_oct_dis, stream);
-}
-
-// Same march, compiled to share the SMs (<= 64 registers): for a march that runs in the background of other kernels.
-extern "C" int f2b_sampler_march_bg(const void* tree_nodes, int n_nodes, const void* trans, int n_trans,
-                                    const float* rays_o, const float* rays_d, const float* rays_noise, int n_rays,
-                                    float near, float far, float sample_l, int scale_by_dis,
-                                    int max_oct_intersect_per_ray, int count_all_hits, float* s_pts, float* s_dt,
-                                    float* s_t, int* s_anchors, int* ray_counts, int* pts_idx_bounds, int* totals,
-                                    float* first_oct_dis, void* stream) {
-  return march_slots(true, tree_nodes, n_nodes, trans, n_trans, rays_o, rays_d, rays_noise, n_rays, near, far, sample_l, scale_by_dis,
-                     max_oct_intersect_per_ray, count_all_hits, s_pts, s_dt, s_t, s_anchors, ray_counts, pts_idx_bounds, totals,
-                     first_oct_dis, stream);
-}
-
-static int march_slots(bool lean, const void* tree_nodes, int n_nodes, const void* trans, int n_trans, const float* rays_o,
-                       const float* rays_d, const float* rays_noise, int n_rays, float near, float far, float sample_l,
-                       int scale_by_dis, int max_oct_intersect_per_ray, int count_all_hits, float* s_pts, float* s_dt, float* s_t,
-                       int* s_anchors, int* ray_counts, int* pts_idx_bounds, int* totals, float* first_oct_dis, void* stream) {
   F2B_REQUIRE(n_rays >= 0 && n_nodes > 0 && n_trans >= 0, "f2b_sampler_march: bad sizes");
   F2B_REQUIRE(totals, "f2b_sampler_march: null totals");
   cudaStream_t st = as_stream(stream);
@@ -697,16 +477,10 @@ static int march_slots(bool lean, const void* tree_nodes, int n_nodes, const voi
   if (n_rays == 0) return check_launch("f2b_sampler_march");
   F2B_REQUIRE(tree_nodes && trans && rays_o && rays_d && rays_noise && s_pts && s_dt && s_t && s_anchors && ray_counts &&
               pts_idx_bounds && first_oct_dis, "f2b_sampler_march: null pointer");
-  if (lean && march_lanes() == 16)
-    march16_kernel<2, true><<<div_up(n_rays, kRaysPerBlock16), 32, 0, st>>>(
-        (const TreeNode*)tree_nodes, (const TransInfo*)trans, rays_o, rays_d, rays_noise, n_rays, near, far, sample_l,
-        scale_by_dis, max_oct_intersect_per_ray, count_all_hits, ray_counts, totals + 1, nullptr, s_pts, nullptr, s_dt, s_t,
-        s_anchors, first_oct_dis);
-  else
-    F2B_LAUNCH_MARCH(2, st,
-        (const TreeNode*)tree_nodes, (const TransInfo*)trans, rays_o, rays_d, rays_noise, n_rays, near, far, sample_l,
-        scale_by_dis, max_oct_intersect_per_ray, count_all_hits, ray_counts, totals + 1, nullptr, s_pts, nullptr, s_dt, s_t,
-        s_anchors, first_oct_dis);
+  F2B_LAUNCH_MARCH(2, st,
+      (const TreeNode*)tree_nodes, (const TransInfo*)trans, rays_o, rays_d, rays_noise, n_rays, near, far, sample_l,
+      scale_by_dis, max_oct_intersect_per_ray, count_all_hits, ray_counts, totals + 1, nullptr, s_pts, nullptr, s_dt, s_t,
+      s_anchors, first_oct_dis);
   scan_counts_kernel<<<1, 1024, 0, st>>>(ray_counts, n_rays, pts_idx_bounds, totals);
   return check_launch("f2b_sampler_march");
 }

@@ -209,11 +209,10 @@ class Hash3DAnchored:
 
 def field_forward(field, table16, params16, points, anchors, anchor_stride, save, logit_only=False, save_feat=None):
     """hash encode -> MLP.  Returns (out, feat16, hidden); out is fp32 [n,16], or [n] (channel 0) when
-    ``logit_only``; feat16 when ``save`` or ``save_feat``, hidden only when ``save``.  With the tensor-core MLP
-    selected (default) this is ONE fused kernel (f2b_field_fwd); with the CUDA-core twin it is encode + MLP + cast."""
-    from . import _lib
+    ``logit_only``; feat16 when ``save`` or ``save_feat``, hidden only when ``save``.  For the default 32 -> 64 -> 16 field
+    MLP this is ONE fused kernel (f2b_field_fwd); other depths run encode + MLP + cast."""
     save_feat = save if save_feat is None else save_feat
-    if _lib.lib.f2b_get_mlp_impl() == 1 and field.mlp_.n_hidden_matmuls == 0:
+    if field.mlp_.n_hidden_matmuls == 0:
         return ops.field_fwd(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_, params16,
                              points, anchors, anchor_stride, logit_only=logit_only, save=save, save_feat=save_feat)
     feat16 = ops.hash_fwd(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_, points,

@@ -129,30 +129,31 @@ def field_fwd(table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16
 
 
 def mlp_fwd(x_f16, params_f16, n_hidden_matmuls, save_hidden=False, impl=None):
+    """impl="v0": the CUDA-core reference kernels; otherwise the tensor-core kernels."""
     n = x_f16.shape[0]
     out = dev_empty((n, 16), F16, x_f16)
     hidden = dev_empty((n_hidden_matmuls + 1, n, 64), F16, x_f16) if save_hidden else None
-    name = "f2b_mlp_fwd" if impl is None else f"f2b_mlp_fwd_{impl}"
+    name = "f2b_mlp_fwd_v0" if impl == "v0" else "f2b_mlp_fwd"
     call(name, x_f16, params_f16, int(n_hidden_matmuls), n, out, hidden, stream())
     return out, hidden
 
 
 def mlp_fwd_f32(x_f16, params_f16, n_hidden_matmuls, save_hidden=False, want_f16=False):
     """MLP forward returning fp32 [n,16] (fp16-rounded values) straight from the epilogue: -> (out32, out16|None, hidden)."""
-    from . import _lib
     n = x_f16.shape[0]
     out32 = dev_empty((n, 16), F32, x_f16)
-    out16 = dev_empty((n, 16), F16, x_f16) if (want_f16 or _lib.lib.f2b_get_mlp_impl() != 1) else None
+    out16 = dev_empty((n, 16), F16, x_f16) if want_f16 else None
     hidden = dev_empty((n_hidden_matmuls + 1, n, 64), F16, x_f16) if save_hidden else None
     call("f2b_mlp_fwd_f32", x_f16, params_f16, int(n_hidden_matmuls), n, out32, out16, hidden, stream())
     return out32, out16, hidden
 
 
 def mlp_bwd(dout_f16, x_f16, hidden, params_f16, n_hidden_matmuls, need_din=True, impl=None):
+    """impl="v0": the CUDA-core reference kernels; otherwise the tensor-core kernels."""
     n = x_f16.shape[0]
     din = dev_empty((n, 32), F16, x_f16) if need_din else None
     dparams = torch.zeros(params_f16.numel(), dtype=F32, device=x_f16.device)
-    name = "f2b_mlp_bwd" if impl is None else f"f2b_mlp_bwd_{impl}"
+    name = "f2b_mlp_bwd_v0" if impl == "v0" else "f2b_mlp_bwd"
     call(name, dout_f16, x_f16, hidden, params_f16, int(n_hidden_matmuls), n, din, dparams, stream())
     return din, dparams
 

@@ -20,9 +20,6 @@ from .rng import burn_mlp_output, burn_rand
 from .sampler import TRAIN, VALIDATE, LazySampleResult, SampleResultFlex
 
 N_EDGE_PTS = 8192
-# The tensor-core MLP backward rebuilds the hidden activations from the 64 B input row instead of reading 128 / 256 B per sample the
-# forward saved (f2b_mlp_bwd2 with hidden0 == NULL): bit-identical dL/dinput, no hidden_save traffic.  F2B_MLP_RECOMPUTE=0 saves.
-MLP_RECOMPUTE = os.environ.get("F2B_MLP_RECOMPUTE", "1") == "1"
 
 
 @dataclass
@@ -100,15 +97,20 @@ class Renderer:
 
     def Render(self, rays_o, rays_d, bounds, emb_idx=None):
         """Renderer::Render (Renderer.cpp:52-213)."""
+        n_rays = rays_o.shape[0]
+        if self.global_data_pool_.mode_ != TRAIN and self._fused_forward_ok(n_rays):
+            return self.render_forward(rays_o, rays_d)
+        if self._fused_launch_ok(n_rays):
+            return self._render_fused_launches(rays_o, rays_d, emb_idx)
+        return self._render_per_kernel(rays_o, rays_d, emb_idx)
+
+    def _render_per_kernel(self, rays_o, rays_d, emb_idx=None):
+        """Renderer::Render (Renderer.cpp:52-213) with one C-ABI call per kernel: the pipeline of ``_render_fused_launches`` for
+        per-kernel tracing (bench.py's breakdown) and for MLP depths the fused launch sequences do not cover."""
         gdp = self.global_data_pool_
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
         train = gdp.mode_ == TRAIN
-        if not train and self._fused_forward_ok(n_rays):
-            return self.render_forward(rays_o, rays_d)
-        if self._fused_launch_ok(n_rays):
-            return self._render_fused_launches(rays_o, rays_d, emb_idx)
-        # ---- the same pipeline, one C-ABI call per kernel (per-kernel tracing, the CUDA-core MLP twin, ray / backward chunking)
         # ---- phase 1: march -> early-stop field pass -> survivors, in the march's slot layout (no host sync) ----
         pf = sampler.take_prefetched(rays_o, rays_d) if n_rays > 0 else None
         if pf is not None:                                           # marched during the previous backward (prefetch_next)
@@ -136,33 +138,16 @@ class Renderer:
             keep = self._buf("keep", (n_rays * S,), torch.uint8, dev)
             kept_counts = self._buf("kept", (n_rays,), torch.int32, dev)
             main = torch.cuda.current_stream(dev)
-            chunks = self._ray_chunks(n_rays)
-            lanes = [main] + [self._side_stream(dev, i) for i in range(1, len(chunks))]
-            ready = torch.cuda.Event()
-            ready.record(main)                                       # inputs / table / noise are ready here
-            for (r0, r1), st in zip(chunks, lanes):                  # ray chunks on their own streams: chunk k's field
-                if st is not main:                                   # pass (memory latency) overlaps chunk k+1's march (issue)
-                    st.wait_event(ready)
-                with torch.cuda.stream(st):
-                    if pf is None:
-                        sampler.march_rays(slots, r0, r1)
-                    ops.field_fwd_slots(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_,
-                                        fparams16, slots.s_pts[r0 * S:r1 * S], slots.s_anchors[r0 * S:r1 * S],
-                                        slots.counts[r0:r1], r1 - r0, S, logit_s[r0 * S:r1 * S], feat_s[r0 * S:r1 * S])
-                    ops.early_stop_rays(logit_s, 1, slots.s_dt, slots.slot_bounds[r0:r1], weights0, alphas0, keep,
-                                        kept_counts[r0:r1])
-            for st in lanes[1:]:
-                main.wait_stream(st)
+            if pf is None:
+                sampler.march_rays(slots, 0, n_rays)
+            ops.field_fwd_slots(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_,
+                                fparams16, slots.s_pts[:n_rays * S], slots.s_anchors[:n_rays * S],
+                                slots.counts[:n_rays], n_rays, S, logit_s, feat_s)
+            ops.early_stop_rays(logit_s, 1, slots.s_dt, slots.slot_bounds[:n_rays], weights0, alphas0, keep, kept_counts)
             new_bounds, total = ops.count_scan(kept_counts, n_rays)
-            cut_rays = self._bwd_cut_rays(n_rays)                    # interior ray boundaries of the backward's chunks
-            head = [total] + ([new_bounds[cut_rays, 0]] if cut_rays is not None else [])
-            n_head = 1 + (0 if cut_rays is None else cut_rays.numel())
-            vals = torch.cat(head + [t.reshape(-1) for t in slots.totals]).tolist()      # THE host sync of the step
+            vals = torch.cat([total] + [t.reshape(-1) for t in slots.totals]).tolist()      # THE host sync of the step
             n_kept = int(vals[0])
-            n_all, n_all_oct = int(sum(vals[n_head::2])), int(sum(vals[n_head + 1::2]))
-            rcut = [0] + ([] if cut_rays is None else self._cut_list) + [n_rays]
-            scut = [0] + [int(v) for v in vals[1:n_head]] + [n_kept]
-            self._bwd_cuts_ = [(rcut[i], rcut[i + 1], scut[i], scut[i + 1]) for i in range(len(rcut) - 1)]
+            n_all, n_all_oct = int(sum(vals[1::2])), int(sum(vals[2::2]))
             sampler.note_totals(n_rays, n_all_oct)
             slots.noted = True
             self.n_sampled_pts_, self.n_kept_pts_ = n_all, n_kept     # host-side counts of this call (no extra sync)
@@ -220,16 +205,13 @@ class Renderer:
     # ------------------------------------------------------------------------------------------
     def _fused_launch_ok(self, n_rays):
         """One foreign call per phase (f2b_render_phase1 / _phase2_fwd / _bwd, csrc/render.cu) instead of one per kernel: the
-        default.  The per-kernel path stays for per-kernel tracing (bench.py's breakdown), the CUDA-core MLP twin and the
-        experimental ray / backward chunking."""
-        if n_rays <= 0 or _lib.TRACE is not None or os.environ.get("F2B_FUSED_LAUNCH", "1") != "1":
+        default.  Per-kernel tracing (bench.py's breakdown) and other MLP depths take ``_render_per_kernel``."""
+        if n_rays <= 0 or _lib.TRACE is not None:
             return False
-        if _lib.lib.f2b_get_mlp_impl() != 1 or self.scene_field_.mlp_.n_hidden_matmuls != 0 or self.shader_.mlp_.n_hidden_matmuls != 1:
-            return False
-        return len(self._ray_chunks(n_rays)) == 1 and self._bwd_cut_rays(n_rays) is None
+        return self.scene_field_.mlp_.n_hidden_matmuls == 0 and self.shader_.mlp_.n_hidden_matmuls == 1
 
     def _render_fused_launches(self, rays_o, rays_d, emb_idx):
-        """Renderer::Render (Renderer.cpp:52-213): identical kernels, order, streams and RNG draws as the per-kernel path below,
+        """Renderer::Render (Renderer.cpp:52-213): identical kernels, order, streams and RNG draws as ``_render_per_kernel``,
         issued through the three launch sequences of csrc/render.cu."""
         gdp = self.global_data_pool_
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
@@ -301,8 +283,6 @@ class Renderer:
                          feat_q=f16(rows + n_edge, 32), logit=f32(rows), mlp_in=f16(rows, 32), raw=f16(rows, 16),
                          rgb=f32(rows, 3), edge32=f32(n_edge, 16), colors=f32(n_rays, 3), disparity=f32(n_rays), depth=f32(n_rays),
                          weights=f32(rows))
-                if grad_on and not MLP_RECOMPUTE:
-                    T.update(f_hidden=f16(1, rows + n_edge, 64), s_hidden=f16(2, rows, 64))
                 if train:                                             # TV-loss edge points: the reference's draws
                     if sampler.n_edges <= 0:
                         raise RuntimeError("GetEdgeSamples: empty edge pool (needs >= 2 face-adjacent valid leaves)")
@@ -322,13 +302,12 @@ class Renderer:
                 pf["done"].synchronize()                  # the march (and the pinned copy behind it) finished during the last backward
                 pre_all = int(pf["host_totals"][0])
             T = None
-            if pre_all is not None and pre_all > 0 and os.environ.get("F2B_PRESYNC_HOST", "1") == "1":
+            if pre_all is not None and pre_all > 0:
                 burn_mlp_output(pre_all, dev)             # RNG parity: the reference's MLP output is a torch::rand (rng.py)
                 if train:
                     launch_votes()
                 T = phase2_buffers(pre_all)
             n_kept, n_all, n_all_oct = heads.tolist()                 # THE host sync of the step
-            self._bwd_cuts_ = None
             sampler.note_totals(n_rays, n_all_oct)
             slots.noted = True
             slots.totals = [heads[1:]]
@@ -373,11 +352,10 @@ class Renderer:
 
     def _fused_forward_ok(self, n_rays):
         """VALIDATE mode takes no gradient, no occupancy votes and no TV-loss edge points: march + ONE kernel
-        (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 (or per-kernel tracing / the CUDA-core MLP twin) keeps the operator pipeline."""
+        (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 (or per-kernel tracing / other MLP depths) keeps the operator pipeline."""
         if n_rays <= 0 or _lib.TRACE is not None or os.environ.get("F2B_FUSED_FORWARD", "1") != "1":
             return False
-        return (_lib.lib.f2b_get_mlp_impl() == 1 and self.scene_field_.mlp_.n_hidden_matmuls == 0
-                and self.shader_.mlp_.n_hidden_matmuls == 1)
+        return self.scene_field_.mlp_.n_hidden_matmuls == 0 and self.shader_.mlp_.n_hidden_matmuls == 1
 
     def render_forward(self, rays_o, rays_d, out=None, lane=0):
         """Renderer::Render (Renderer.cpp:52-213) for a batch that takes no gradient (VALIDATE mode): the march, then hash encode
@@ -476,30 +454,6 @@ class Renderer:
         if t is None or t.numel() < n or t.dtype != dtype or t.device != torch.device(dev):
             t = pool[name] = torch.empty((max(n, 1),), dtype=dtype, device=dev)
         return t[:n].view(*shape)
-
-    def _bwd_cut_rays(self, n_rays):
-        """Device index tensor of the interior ray boundaries of the backward chunks (F2B_BWD_CHUNKS / ``bwd_chunks_``)."""
-        if not hasattr(self, "bwd_chunks_"):
-            self.bwd_chunks_ = int(os.environ.get("F2B_BWD_CHUNKS", "1"))
-        k = max(1, min(int(self.bwd_chunks_), 16, (n_rays + 255) // 256))
-        if k <= 1:
-            self._cut_list = []
-            return None
-        key = (n_rays, k)
-        if getattr(self, "_cut_key", None) != key:
-            step = -(-n_rays // k)
-            self._cut_list = [r for r in range(step, n_rays, step)]
-            self._cut_dev = torch.tensor(self._cut_list, dtype=torch.int64, device=self.app_emb_.device) if self._cut_list else None
-            self._cut_key = key
-        return self._cut_dev
-
-    def _ray_chunks(self, n_rays):
-        """Ray ranges marched on separate streams (F2B_RAY_CHUNKS / ``ray_chunks_``; 1 = single stream)."""
-        if not hasattr(self, "ray_chunks_"):
-            self.ray_chunks_ = int(os.environ.get("F2B_RAY_CHUNKS", "1"))
-        k = max(1, min(int(self.ray_chunks_), 4, (n_rays + 255) // 256))
-        step = -(-n_rays // k)
-        return [(r0, min(r0 + step, n_rays)) for r0 in range(0, n_rays, step)]
 
     # ------------------------------------------------------------------------------------------
     def States(self):
@@ -615,24 +569,22 @@ class _RenderFunction(torch.autograd.Function):
         dev = bg.device
         n_q = feat16.shape[0]
         emb = app_emb if pt_emb_idx is not None else None
-        if _lib.lib.f2b_get_mlp_impl() == 1 and field.mlp_.n_hidden_matmuls == 0 and shader.mlp_.n_hidden_matmuls == 1:
-            # fused epilogues (tensor-core kernels): field MLP -> [logit | shader-MLP input row], shader MLP -> [raw | rgb];
-            # the fp32 scene_feat of the ray samples is never materialised (edge points still need all 16 channels)
-            save = grad_on and not MLP_RECOMPUTE
-            f_hidden = torch.empty((1, n_q, 64), dtype=torch.float16, device=dev) if save else None
+        if field.mlp_.n_hidden_matmuls == 0 and shader.mlp_.n_hidden_matmuls == 1:
+            # fused epilogues: field MLP -> [logit | shader-MLP input row], shader MLP -> [raw | rgb]; the fp32 scene_feat of the
+            # ray samples is never materialised (edge points still need all 16 channels).  No hidden activations are saved: the
+            # backward rebuilds them from the input rows (f2b_mlp_bwd2 with hidden0 == NULL), bit-identical
+            f_hidden = s_hidden = None
             logit = torch.empty((n_kept,), dtype=torch.float32, device=dev)
             mlp_in = torch.empty((n_kept, 32), dtype=torch.float16, device=dev)
-            call("f2b_field_shade_fwd", feat16, fparams16, es.dirs, emb, pt_emb_idx, n_kept, logit, mlp_in, f_hidden, stream())
+            call("f2b_field_shade_fwd", feat16, fparams16, es.dirs, emb, pt_emb_idx, n_kept, logit, mlp_in, None, stream())
             if n_q > n_kept:
                 edge32 = torch.empty((n_q - n_kept, 16), dtype=torch.float32, device=dev)
-                call("f2b_mlp_fwd_f32", feat16[n_kept:], fparams16, 0, n_q - n_kept, edge32, None,
-                     f_hidden[0, n_kept:] if save else None, stream())
+                call("f2b_mlp_fwd_f32", feat16[n_kept:], fparams16, 0, n_q - n_kept, edge32, None, None, stream())
             else:
                 edge32 = torch.empty((0, 16), dtype=torch.float32, device=dev)
-            s_hidden = torch.empty((2, n_kept, 64), dtype=torch.float16, device=dev) if save else None
             raw = torch.empty((n_kept, 16), dtype=torch.float16, device=dev)
             rgb = torch.empty((n_kept, 3), dtype=torch.float32, device=dev)
-            call("f2b_shader_mlp_rgb_fwd", mlp_in, sparams16, n_kept, raw, rgb, s_hidden, stream())
+            call("f2b_shader_mlp_rgb_fwd", mlp_in, sparams16, n_kept, raw, rgb, None, stream())
             logit_stride = 1
         else:
             scene_feat, f_hidden = field_forward_from_features(field, fparams16, feat16, save=grad_on)
@@ -645,7 +597,6 @@ class _RenderFunction(torch.autograd.Function):
         scene_feat = (logit, logit_stride)
         edge_feats = edge32.reshape(-1, 2, 16)
         ctx.renderer, ctx.es, ctx.n_kept = renderer, es, n_kept
-        ctx.cuts = renderer._bwd_cuts_ if getattr(renderer, "_bwd_cuts_", None) else [(0, es.pts_idx_bounds.shape[0], 0, n_kept)]
         ctx.pack = (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw,
                     s_hidden, rgb)
         ctx.gs_progress = renderer.global_data_pool_.gradient_scaling_progress_
@@ -674,10 +625,8 @@ class _RenderFunction(torch.autograd.Function):
         if ctx.gs_progress < 1.:                          # GradientScaling::backward draws an unused rand_like (CustomOps.cu:154)
             burn_rand(n_kept * 3, dev)
             burn_rand(n_kept, dev)
-        # ---- backward, optionally in ray chunks (bwd_chunks_ / F2B_BWD_CHUNKS): the dense chain (composite -> sigmoid ->
-        # shader MLP -> input assembly -> field MLP; HBM streaming) of chunk k+1 on the main stream, the hash scatter of
-        # chunk k (L2 reductions) on a side stream.  Co-running them is slower (the scatter's many small blocks crowd out
-        # the persistent tensor-core CTAs), so the default is one chunk; the scatter still runs on the side stream behind an event.
+        # ---- backward: the dense chain (composite -> sigmoid -> shader MLP -> input assembly -> field MLP; HBM streaming) on the
+        # main stream, the hash scatter (L2 reductions) on a side stream behind an event.
         s_scale, f_scale = shader.mlp_.loss_scale_, field.mlp_.loss_scale_
         nh_s, nh_f = shader.mlp_.n_hidden_matmuls, field.mlp_.n_hidden_matmuls
         f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)
@@ -713,23 +662,17 @@ class _RenderFunction(torch.autograd.Function):
             with torch.cuda.stream(side):
                 ops.hash_bwd(*hash_args, pts, anc, stride, dfeat16[s0:s1], grad_mul, d_table)
 
-        for r0, r1, s0, s1 in ctx.cuts:
-            if s1 <= s0:
-                continue
-            nr, ns = r1 - r0, s1 - s0
+        if n_kept > 0:
             # composite backward with the colour activation's backward applied on the way out (fp16 d_raw directly)
-            call("f2b_composite_act_bwd", scene_feat[0], int(scene_feat[1]), rgb, es.dt, es.t, bounds[r0:r1], bg[r0:r1], nr,
-                 d_colors[r0:r1], None if d_disp is None else d_disp[r0:r1], None if d_depth is None else d_depth[r0:r1],
-                 d_weights, float(ctx.gs_progress), raw, float(s_scale), d_logit, 1, d_raw, stream())
-            call("f2b_mlp_bwd2", d_raw[s0:s1], mlp_in[s0:s1], None if s_hidden is None else s_hidden[0, s0:s1],
-                 s_hidden[1, s0:s1] if (nh_s and s_hidden is not None) else None, sparams16, int(nh_s), ns, d_in16[s0:s1], d_sparams,
-                 stream())
-            ops.shader_prep_bwd_f16(d_in16, d_logit, bounds[r0:r1], None if ray_emb_idx is None else ray_emb_idx[r0:r1],
-                                    1.0 / s_scale, f_scale, d_scene16, d_app)
-            call("f2b_mlp_bwd2", d_scene16[s0:s1], feat16[s0:s1], None if f_hidden is None else f_hidden[0, s0:s1],
-                 f_hidden[1, s0:s1] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), ns, dfeat16[s0:s1], d_fparams,
-                 stream())
-            scatter(segments[0][0][s0:s1], segments[0][1][s0:s1], segments[0][2], s0, s1)
+            call("f2b_composite_act_bwd", scene_feat[0], int(scene_feat[1]), rgb, es.dt, es.t, bounds, bg, n_rays, d_colors, d_disp,
+                 d_depth, d_weights, float(ctx.gs_progress), raw, float(s_scale), d_logit, 1, d_raw, stream())
+            call("f2b_mlp_bwd2", d_raw, mlp_in, None if s_hidden is None else s_hidden[0],
+                 s_hidden[1] if (nh_s and s_hidden is not None) else None, sparams16, int(nh_s), n_kept, d_in16, d_sparams, stream())
+            ops.shader_prep_bwd_f16(d_in16, d_logit, bounds, ray_emb_idx, 1.0 / s_scale, f_scale, d_scene16, d_app)
+            call("f2b_mlp_bwd2", d_scene16[:n_kept], feat16[:n_kept], None if f_hidden is None else f_hidden[0, :n_kept],
+                 f_hidden[1, :n_kept] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), n_kept, dfeat16[:n_kept],
+                 d_fparams, stream())
+            scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
         for pts_e, anc_e, stride_e, first, rows in segments[1:]:          # TV-loss edge points: field MLP + scatter only
             if rows > 0:
                 call("f2b_mlp_bwd2", d_scene16[first:first + rows], feat16[first:first + rows],
@@ -770,10 +713,8 @@ class _RenderFunction(torch.autograd.Function):
 
 def slab_groups():
     """Level groups (first level, count) of the data-parallel scatter, top-down; the table-gradient slab above a group's lower
-    boundary is all-reduced behind it while the next group scatters (dist.install_grad_overlap).  F2B_DP_SLABS = 4 (default:
-    12-15 | 8-11 | 4-7 | 0-3), 2 (8-15 | 0-7: fewer launch tails, a larger exposed last slab) or 1."""
-    n = int(os.environ.get("F2B_DP_SLABS", "4"))
-    return {4: ((12, 4), (8, 4), (4, 4), (0, 4)), 2: ((8, 8), (0, 8)), 1: ((0, 16),)}.get(n, ((12, 4), (8, 4), (4, 4), (0, 4)))
+    boundary is all-reduced behind it while the next group scatters (dist.install_grad_overlap): 12-15 | 8-11 | 4-7 | 0-3."""
+    return ((12, 4), (8, 4), (4, 4), (0, 4))
 
 
 def check_backward_nan(renderer):

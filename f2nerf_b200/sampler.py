@@ -10,8 +10,6 @@ blobs come from a reference checkpoint / dump or from ``tests/synth_scene.py`` (
 """
 from dataclasses import dataclass
 
-import os
-
 import torch
 
 from . import ops
@@ -150,15 +148,14 @@ class PersSampler:
         self._generation = getattr(self, "_generation", 0) + 1
         return SlotSamples(self, rays_o, rays_d, rays_noise, self._scratch(n_rays, rays_o.device), self._generation)
 
-    def march_rays(self, slots, r0, r1, background=False):
-        """March rays [r0, r1) into their slots on the CURRENT stream (no host sync).  ``background``: the <= 64-register build of
-        the same kernel (f2b_sampler_march_bg) for a march that shares the SMs with other work."""
+    def march_rays(self, slots, r0, r1):
+        """March rays [r0, r1) into their slots on the CURRENT stream (no host sync)."""
         n = r1 - r0
         if n <= 0:
             return
         S = slots.slot
         totals = torch.empty((2,), dtype=torch.int32, device=slots.rays_o.device)
-        call("f2b_sampler_march_bg" if background else "f2b_sampler_march", self.tree_nodes_gpu_, self.n_nodes, self.pers_trans_gpu_, self.pers_trans_gpu_.numel() // 544,
+        call("f2b_sampler_march", self.tree_nodes_gpu_, self.n_nodes, self.pers_trans_gpu_, self.pers_trans_gpu_.numel() // 544,
              slots.rays_o[r0:r1], slots.rays_d[r0:r1], slots.noise[r0:], n, float(self.global_near_), 1e8, float(self.sample_l_),
              int(self.scale_by_dis_), int(self.max_oct_intersect_per_ray_), int(bool(self.exact_oct_stat_)),
              slots.s_pts[r0 * S:r1 * S], slots.s_dt[r0 * S:r1 * S], slots.s_t[r0 * S:r1 * S], slots.s_anchors[r0 * S:r1 * S],
@@ -195,9 +192,7 @@ class PersSampler:
         ev.record(main)                                            # the ray upload / noise draw queued so far precede the march (the
         stream.wait_event(ev)                                      # scratch it writes is the OTHER set: no reader to wait for)
         with torch.cuda.stream(stream):
-            # F2B_MARCH_BG=1 selects the <= 64-register build: more of it co-resides with the dense backward and takes its issue
-            # slots, so the default stays the 96-register kernel
-            self.march_rays(slots, 0, n_rays, background=os.environ.get("F2B_MARCH_BG", "0") == "1")
+            self.march_rays(slots, 0, n_rays)
             ring = self.__dict__.setdefault("_pinned_totals", [torch.empty((2,), dtype=torch.int32).pin_memory() for _ in range(4)])
             self._pinned_turn = (getattr(self, "_pinned_turn", -1) + 1) % len(ring)
             host_totals = ring[self._pinned_turn]

@@ -63,7 +63,6 @@ const auto kByte = torch::TensorOptions().dtype(torch::kUInt8).device(torch::kCU
 
 void* cur_stream() { return (void*) at::cuda::getCurrentCUDAStream().stream(); }
 void* P(const Tensor& t) { return t.defined() ? t.data_ptr() : nullptr; }
-// F2B_MLP_RECOMPUTE (default 1): the MLP forward saves no hidden activations, f2b_mlp_bwd2(hidden0 = NULL) rebuilds them
 // F2B_FUSED_FORWARD (default 1): VALIDATE-mode Render = march + f2b_render_fwd_fused; F2B_VALIDATE_WEIGHTS (default 1): also pack
 // RenderResult.weights / idx_start_end (costs the step's one host read)
 bool fused_forward() {
@@ -96,10 +95,6 @@ struct ScopedTimer {
   ~ScopedTimer() { if (acc) { *acc += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); ++*cnt; } }
 };
 
-bool mlp_recompute() {
-  static const bool on = [] { const char* e = getenv("F2B_MLP_RECOMPUTE"); return !e || atoi(e) != 0; }();
-  return on;
-}
 float* PF(const Tensor& t) { return t.defined() ? t.data_ptr<float>() : nullptr; }
 int* PI(const Tensor& t) { return t.defined() ? t.data_ptr<int>() : nullptr; }
 
@@ -159,7 +154,7 @@ struct Pack {
   bool grad_on = false;
   float gs_progress = 1.f;
   // saved by forward
-  Tensor fparams16, sparams16, logit, mlp_in, raw, rgb, f_hidden, s_hidden;
+  Tensor fparams16, sparams16, logit, mlp_in, raw, rgb;
 };
 std::mutex g_pack_mu;
 std::unordered_map<int64_t, std::shared_ptr<Pack>> g_packs;
@@ -178,23 +173,19 @@ public:
     F2B_CHECK(f2b_cast_f32_to_f16(field_params.data_ptr<float>(), P(k.fparams16), field_params.numel(), 1.f, cur_stream()));
     F2B_CHECK(f2b_cast_f32_to_f16(shader_params.data_ptr<float>(), P(k.sparams16), shader_params.numel(), 1.f, cur_stream()));
     const bool emb_on = k.pt_emb_idx.defined();
-    const bool save = k.grad_on && !mlp_recompute();
-    if (save) k.f_hidden = torch::empty({1, n_q, 64}, kHalf);
     k.logit = torch::empty({n_kept}, CUDAFloat);
     k.mlp_in = torch::empty({n_kept, 32}, kHalf);
     F2B_CHECK(f2b_field_shade_fwd(P(k.feat16), P(k.fparams16), PF(k.dirs), emb_on ? app_emb.data_ptr<float>() : nullptr,
-                                  emb_on ? PI(k.pt_emb_idx) : nullptr, (int) n_kept, PF(k.logit), P(k.mlp_in),
-                                  P(k.f_hidden), cur_stream()));
+                                  emb_on ? PI(k.pt_emb_idx) : nullptr, (int) n_kept, PF(k.logit), P(k.mlp_in), nullptr,
+                                  cur_stream()));
     Tensor edge32 = torch::empty({n_q - n_kept, 16}, CUDAFloat);
     if (n_q > n_kept) {
       F2B_CHECK(f2b_mlp_fwd_f32((char*) P(k.feat16) + n_kept * 64, P(k.fparams16), 0, (int) (n_q - n_kept), PF(edge32), nullptr,
-                                save ? (void*) ((char*) P(k.f_hidden) + n_kept * 128) : nullptr, cur_stream()));
+                                nullptr, cur_stream()));
     }
-    if (save) k.s_hidden = torch::empty({2, n_kept, 64}, kHalf);
     k.raw = torch::empty({n_kept, 16}, kHalf);
     k.rgb = torch::empty({n_kept, 3}, CUDAFloat);
-    F2B_CHECK(f2b_shader_mlp_rgb_fwd(P(k.mlp_in), P(k.sparams16), (int) n_kept, P(k.raw), PF(k.rgb),
-                                     P(k.s_hidden), cur_stream()));
+    F2B_CHECK(f2b_shader_mlp_rgb_fwd(P(k.mlp_in), P(k.sparams16), (int) n_kept, P(k.raw), PF(k.rgb), nullptr, cur_stream()));
     const int n_rays = k.bounds.size(0);
     Tensor colors = torch::empty({n_rays, 3}, CUDAFloat), disp = torch::empty({n_rays}, CUDAFloat),
            depth = torch::empty({n_rays}, CUDAFloat), weights = torch::empty({n_kept}, CUDAFloat);
@@ -258,12 +249,12 @@ public:
     F2B_CHECK(f2b_composite_act_bwd(PF(k.logit), 1, PF(k.rgb), PF(k.dt), PF(k.t), PI(k.bounds), PF(k.bg), n_rays, PF(d_colors),
                                     PF(d_disp), PF(d_depth), PF(d_weights), k.gs_progress, P(k.raw), s_scale, PF(d_logit), 1,
                                     P(d_raw), cur_stream()));
-    F2B_CHECK(f2b_mlp_bwd2(P(d_raw), P(k.mlp_in), P(k.s_hidden),
-                           k.s_hidden.defined() ? (void*) ((char*) P(k.s_hidden) + n_kept * 128) : nullptr, P(k.sparams16), 1,
-                           (int) n_kept, P(d_in16), PF(d_sparams), cur_stream()));
+    // the forward saved no hidden activations: f2b_mlp_bwd2 (hidden0 == NULL) rebuilds them from the input rows
+    F2B_CHECK(f2b_mlp_bwd2(P(d_raw), P(k.mlp_in), nullptr, nullptr, P(k.sparams16), 1, (int) n_kept, P(d_in16), PF(d_sparams),
+                           cur_stream()));
     F2B_CHECK(f2b_shader_prep_bwd_f16(P(d_in16), PF(d_logit), PI(k.bounds), emb_on ? PI(k.ray_emb_idx) : nullptr, n_rays,
                                       1.f / s_scale, f_scale, P(d_scene16), PF(d_app), cur_stream()));
-    F2B_CHECK(f2b_mlp_bwd2(P(d_scene16), P(k.feat16), P(k.f_hidden), nullptr, P(k.fparams16), 0, (int) n_q, P(dfeat16),
+    F2B_CHECK(f2b_mlp_bwd2(P(d_scene16), P(k.feat16), nullptr, nullptr, P(k.fparams16), 0, (int) n_q, P(dfeat16),
                            PF(d_fparams), cur_stream()));
     F2B_CHECK(f2b_hash_bwd(field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
                            PF(k.pts), PI(k.anchors), 3, (int) n_kept, P(dfeat16), 1, 1.f / f_scale, PF(d_table), cur_stream()));

@@ -77,16 +77,6 @@ int f2b_sampler_march(const void* tree_nodes, int n_nodes, const void* trans, in
                       float* s_pts, float* s_dt, float* s_t, int* s_anchors,
                       int* ray_counts /* [n_rays] */, int* pts_idx_bounds /* [n_rays,2] out */, int* totals /* [2] out */,
                       float* first_oct_dis /* [n_rays] out */, void* stream);
-/* The same march compiled for <= 64 registers per thread (identical arithmetic and results): for the software-pipelined march of
- * the NEXT batch, which runs on a side stream under this batch's backward and must leave the register file to the kernels it
- * shares the SMs with. */
-int f2b_sampler_march_bg(const void* tree_nodes, int n_nodes, const void* trans, int n_trans,
-                      const float* rays_o, const float* rays_d, const float* rays_noise, int n_rays,
-                      float near, float far, float sample_l, int scale_by_dis,
-                      int max_oct_intersect_per_ray, int count_all_hits,
-                      float* s_pts, float* s_dt, float* s_t, int* s_anchors,
-                      int* ray_counts /* [n_rays] */, int* pts_idx_bounds /* [n_rays,2] out */, int* totals /* [2] out */,
-                      float* first_oct_dis /* [n_rays] out */, void* stream);
 int f2b_sampler_gather(const float* rays_d, const int* pts_idx_bounds, int n_rays,
                        const float* s_pts, const float* s_dt, const float* s_t, const int* s_anchors,
                        float* pts, float* dirs, float* dt, float* t, int* anchors, void* stream);
@@ -143,14 +133,13 @@ int f2b_hash_bwd_levels(const int* prim_pool, const float* bias_pool, int n_volu
                         const void* grad_feat, int grad_is_f16, float grad_mul, float* grad_table,
                         int level_lo, int n_levels, void* stream);
 
-/* MLP (no biases, ReLU hidden, linear out padded to 16): params_f16 = [W0 64xin | (W_h 64x64)*n_hidden_matmuls | W_out 16x64],
+/* MLP on the wgmma tensor-core kernels (no biases, ReLU hidden, linear out padded to 16): params_f16 = [W0 64xin | (W_h 64x64)*n_hidden_matmuls | W_out 16x64],
  * each row-major [out][in] (fully_fused_mlp.cu:654-677).  in: [P,32] fp16.  out: [P,16] fp16.
  * hidden_save: nullable, [(n_hidden_matmuls+1), P, 64] fp16 forward activations for backward. */
 int f2b_mlp_fwd(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
                 void* out_f16, void* hidden_save_f16, void* stream);
 /* Same network with the output widened to fp32 in the epilogue — what TCNNWP::Query returns
- * (`feat...to(torch::kFloat32)`, TCNNWP.cpp:112).  out_f32 [P,16] and/or out_f16 [P,16]; with the tensor-core
- * implementation either may be NULL (not both), the CUDA-core twin needs out_f16. */
+ * (`feat...to(torch::kFloat32)`, TCNNWP.cpp:112).  out_f32 [P,16] and/or out_f16 [P,16]; either may be NULL (not both). */
 int f2b_mlp_fwd_f32(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
                     float* out_f32, void* out_f16, void* hidden_save_f16, void* stream);
 /* Backward: dL/dout [P,16] fp16 (already multiplied by loss_scale) -> dL/din [P,32] fp16 (nullable),
@@ -183,36 +172,29 @@ int f2b_field_fwd_slots(const void* table_f16, const int* prim_pool, const float
 
 /* Field MLP on already-encoded features with the shading-feature assembly fused into its epilogue (the fp32 [P,16]
  * scene_feat tensor, `ones_like`/`cat`/ScatterAdd of Renderer.cpp:179-187 and the SH encode + cast of SHShader.cpp:23-26
- * never materialise): logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])).
- * tensor-core implementation only (F2B_EUNSUPPORTED with the CUDA-core twin selected). */
+ * never materialise): logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])). */
 int f2b_field_shade_fwd(const void* feat_f16 /* [P,32] */, const void* field_params_f16, const float* dirs /* [P,3] */,
                         const float* app_emb /* [n_emb,16] or NULL */, const int* pt_emb_idx /* [P] or NULL */, int n_pts,
                         float* logit /* [P] */, void* mlp_in_f16 /* [P,32] */, void* hidden_save_f16 /* [P,64] or NULL */,
                         void* stream);
 /* Shader MLP with the colour activation of SHShader.cpp:27-28 in its epilogue: raw [P,16] fp16 and
- * rgb [P,3] = (1 + 2e-3) * sigmoid(raw[:, :3]) - 1e-3.  tensor-core implementation only. */
+ * rgb [P,3] = (1 + 2e-3) * sigmoid(raw[:, :3]) - 1e-3. */
 int f2b_shader_mlp_rgb_fwd(const void* mlp_in_f16, const void* shader_params_f16, int n_pts, void* raw_f16, float* rgb,
                            void* hidden_save_f16 /* [2,P,64] or NULL */, void* stream);
 /* f2b_mlp_bwd on a row range of a larger saved batch: the two activation layers are passed as separate pointers
  * (hidden1 NULL when n_hidden_matmuls == 0).  dparams is accumulated into, like f2b_mlp_bwd.
- * hidden0 == NULL (tensor-core implementation only): the forward saved nothing — the kernel rebuilds the tile's hidden
+ * hidden0 == NULL: the forward saved nothing — the kernel rebuilds the tile's hidden
  * activations from in_f16 on the tensor pipe (bit-identical to what the forward would have saved) before the backward;
  * 96 B read + 64 B written per sample instead of 224 / 352 + 64 (and the forward does not write 128 / 256 B). */
 int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void* hidden0_f16, const void* hidden1_f16,
                  const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16, float* dparams_f32, void* stream);
 
-/* Implementation selection for f2b_mlp_fwd / f2b_mlp_bwd: 1 = wgmma tensor-core kernels (default when
- * built), 0 = CUDA-core twin (validation).  Env F2B_MLP_IMPL overrides the default. */
-int f2b_set_mlp_impl(int impl);
+/* Which kernels the MLP entry points above run: always 1 = the wgmma tensor-core kernels (recorded by benchmarks). */
 int f2b_get_mlp_impl(void);
+/* The CUDA-core twins of f2b_mlp_fwd / f2b_mlp_bwd (validation references for the tensor-core kernels). */
 int f2b_mlp_fwd_v0(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
                    void* out_f16, void* hidden_save_f16, void* stream);
 int f2b_mlp_bwd_v0(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,
-                   const void* params_f16, int n_hidden_matmuls, int n_pts,
-                   void* din_f16, float* dparams_f32, void* stream);
-int f2b_mlp_fwd_tc(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
-                   void* out_f16, void* hidden_save_f16, void* stream);
-int f2b_mlp_bwd_tc(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,
                    const void* params_f16, int n_hidden_matmuls, int n_pts,
                    void* din_f16, float* dparams_f32, void* stream);
 
@@ -388,12 +370,12 @@ typedef struct f2b_render {
   float* s_pts; float* s_dt; float* s_t; int* s_anchors; int* counts; int* chunk_bounds; int* slot_bounds;
   float* first_oct_dis; int* totals /* [2] */;
   float* logit_s; void* feat_s; float* w0; float* a0; uint8_t* keep; int* kept_counts; int* new_bounds; int* total_kept;
-  /* phase 2: survivors (n_kept rows) + TV-loss edge points (2 * n_edge_pairs rows behind them in feat_q / f_hidden / dfeat16) */
+  /* phase 2: survivors (n_kept rows) + TV-loss edge points (2 * n_edge_pairs rows behind them in feat_q / dfeat16) */
   int n_kept; int n_edge_pairs;
   float* pts; float* dirs; float* dt; float* t; int* anchors; void* feat_q;
   const int* edge_idx; const float* edge_coord; float* e_pts; int* e_anc;
   int* pt_emb_idx;                                       /* [n_kept] scratch, used when app_emb && ray_emb_idx */
-  float* logit; void* mlp_in; void* f_hidden /* nullable */; float* edge32; void* raw; float* rgb; void* s_hidden /* nullable */;
+  float* logit; void* mlp_in; float* edge32; void* raw; float* rgb;
   float* colors; float* disparity; float* depth; float* weights;
   /* backward */
   const float* d_colors; const float* d_disparity; const float* d_depth; const float* d_weights; const float* d_edge /* [2*pairs,16] */;
@@ -420,7 +402,7 @@ int f2b_render_grad_finalize(const f2b_render* r);
  * > 0: normal; <= 0: the reference's empty-batch result, depth = 512, Renderer.cpp:83-97).  ticket: [1] device int scratch.
  * Outputs: colors [R,3], disparity [R], depth [R], kept_counts [R] (survivors per ray), and — nullable — weights_slots
  * [R*slot]: the kept samples' weights at their slots (f2b_gather_kept_weights packs them into RenderResult.weights order).
- * Values are bit-identical to f2b_render_phase1 + f2b_render_phase2_fwd on the same batch.  tensor-core implementation only. */
+ * Values are bit-identical to f2b_render_phase1 + f2b_render_phase2_fwd on the same batch. */
 int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
                          const void* field_params_f16, const void* shader_params_f16, const float* slot_pts, const float* slot_dt,
                          const float* slot_t, const int* slot_anchors, const int* ray_counts, const float* rays_d, const float* bg,

@@ -75,7 +75,7 @@ def main():
     keys = rows[0].keys()
     med = {k: sorted(x[k] for x in rows)[len(rows) // 2] for k in keys}
     print(json.dumps({"config": args.config, "pipeline_march": args.pipeline_march, "median_ms": med, "rows": rows[:6],
-                      "fused_launch": os.environ.get("F2B_FUSED_LAUNCH", "1"), "n_kept": r.n_kept_pts_}))
+                      "n_kept": r.n_kept_pts_}))
 
 
 if __name__ == "__main__":

@@ -92,33 +92,6 @@ def test_sampler_one_pass_equals_two_pass(scene, oracle):
         np.testing.assert_array_equal(N(v).view(np.uint32), two[k].view(np.uint32), err_msg=k)
 
 
-def test_sampler_background_build_is_bit_identical(scene):
-    """f2b_sampler_march_bg (the <= 64-register build of the one-pass march, for a march that shares the SMs with other kernels)
-    against f2b_sampler_march: every output word identical."""
-    from f2nerf_b200 import GlobalDataPool, PersSampler
-    gdp = GlobalDataPool()
-    sampler = PersSampler(gdp, scene["nodes"], scene["trans"], scene["edges"], near=0.01, sample_l=1 / 256, scale_by_dis=True)
-    o, d, dn, cam = make_rays(scene, 777, seed=31)
-    torch.manual_seed(5)
-    noise = sampler.make_noise(777, "cuda").clone()
-    outs = []
-    for bg in (False, True):
-        slots = sampler.begin_march(T(o), T(d), noise.clone())
-        sampler.march_rays(slots, 0, 777, background=bg)
-        n = int(slots.counts.sum())
-        outs.append([N(x).copy() for x in (slots.counts, slots.first_oct_dis, slots.totals[0])] +
-                    [N(x).copy() for x in (slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors)])
-        assert n > 10000
-    cnt = outs[0][0]
-    for a, b in zip(outs[0][:3], outs[1][:3]):
-        np.testing.assert_array_equal(a.view(np.uint32) if a.dtype == np.float32 else a, b.view(np.uint32) if b.dtype == np.float32 else b)
-    for a, b in zip(outs[0][3:], outs[1][3:]):                     # slot layout: compare the filled part of every ray's slot
-        a, b = a.reshape(777, 1024, -1), b.reshape(777, 1024, -1)
-        for r in range(0, 777, 37):
-            x, y = a[r, :cnt[r]], b[r, :cnt[r]]
-            np.testing.assert_array_equal(x.view(np.uint32) if x.dtype == np.float32 else x, y.view(np.uint32) if y.dtype == np.float32 else y)
-
-
 def test_sampler_edge_cases(scene, oracle):
     from f2nerf_b200 import ops
     # rays that miss everything (start far outside, pointing away) and an empty batch
@@ -308,7 +281,7 @@ def test_fused_epilogues_match_operator_sequence(oracle):
 
 
 def test_fused_field_matches_unfused(scene, oracle, hash_params):
-    """f2b_field_fwd (encode fused into the tensor-core MLP) == f2b_hash_fwd -> f2b_mlp_fwd_tc, bit for bit."""
+    """f2b_field_fwd (encode fused into the tensor-core MLP) == f2b_hash_fwd -> f2b_mlp_fwd, bit for bit."""
     from f2nerf_b200 import ops
     s = sample_points(scene, oracle, 100)
     hp = hash_params

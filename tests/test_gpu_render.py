@@ -108,20 +108,23 @@ def test_render_validate_mode_and_empty(scene):
     assert r.weights is None and (N(r.colors) == 0.5).all() and (N(r.depth) == 512.).all()
 
 
-def test_render_mixed_empty_rays_and_ray_chunks(scene):
-    """TRAIN step on a batch where some rays miss the octree entirely; the ray-chunked (multi-stream) schedule
-    must give the same result as the single-stream one, bit for bit (same kernels, same per-ray order)."""
+def test_render_mixed_empty_rays_per_kernel_matches_fused_launches(scene):
+    """TRAIN step on a batch where some rays miss the octree entirely; the per-kernel pipeline (one C-ABI call per kernel)
+    must give the same result as the fused launch sequences, bit for bit (same kernels, same order)."""
     from f2nerf_b200 import TRAIN
     o, d, dn, cam = make_rays(scene, 301, seed=11)                  # odd count: the 16-lane march packs two rays per warp
     o[::7] = 600.                                                   # these rays start far outside and point away
     d[::7] = 1.
     outs = []
-    for chunks in (1, 3):
+    for per_kernel in (False, True):
         gdp, sampler, field, shader, renderer = build(scene)
         gdp.mode_ = TRAIN
-        renderer.ray_chunks_ = chunks
         torch.manual_seed(99)
-        r = renderer.Render(T(o), T(d), None, T(cam))
+        if per_kernel:
+            r = renderer._render_per_kernel(T(o), T(d), T(cam))
+        else:
+            assert renderer._fused_launch_ok(len(o))
+            r = renderer.Render(T(o), T(d), None, T(cam))
         cnt = N(r.idx_start_end[:, 1] - r.idx_start_end[:, 0])
         assert (cnt[::7] == 0).all() and cnt.sum() == r.weights.shape[0] and (cnt > 0).any()
         loss = (r.colors ** 2).mean() + r.disparity.mean() + 0.1 * ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean()

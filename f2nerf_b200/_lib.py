@@ -56,6 +56,7 @@ SIGNATURES = {
     "f2b_field_shade_fwd": [_P, _P, _P, _P, _P, c_int, _P, _P, _P, _P],
     "f2b_shader_mlp_rgb_fwd": [_P, _P, c_int, _P, _P, _P, _P],
     "f2b_mlp_bwd2": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
+    "f2b_field_bwd_scatter": [_P, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_float, _P, _P, _P, _P],
     "f2b_mlp_fwd_v0": [_P, _P, c_int, c_int, _P, _P, _P],
     "f2b_mlp_bwd_v0": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_field_fwd": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P],
@@ -124,7 +125,7 @@ class RenderArgs(ctypes.Structure):
         ("d_sparams", _P), ("d_fparams", _P), ("d_table", _P), ("table_numel", _L), ("table_live", _L), ("d_app", _P),
         ("scatter_mode", _I),
         ("nonfinite", _P),
-        ("stream", _P), ("side_stream", _P),
+        ("stream", _P),
     ]
 
     def set(self, **kw):
@@ -169,7 +170,7 @@ def stream():
 
 
 # kernels launched per entry point (for bench.py's gpu_launches claim; memsets are not counted)
-KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_phase2_fwd": 10, "f2b_render_bwd": 8, "f2b_render_grad_finalize": 2,
+KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_phase2_fwd": 10, "f2b_render_bwd": 6, "f2b_render_grad_finalize": 2,
                     "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_early_stop": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
                     "f2b_abi_version": 0, "f2b_get_mlp_impl": 0}
 LAUNCHES = 0      # running count of product kernels launched through this binding

@@ -61,15 +61,8 @@ hash_fwd_levels_kernel(const __half* __restrict__ table, const int* __restrict__
   }
 }
 
-// Backward: a warp owns 32 CONSECUTIVE samples at one level (samples of a ray are consecutive, so at the
-// coarse levels many lanes fall into the same grid cell and hit the same 8 table entries).  Lanes are grouped
-// into runs of identical (cell, volume); when the warp has few runs, the 16 per-run sums (8 corners x 2
-// channels) are formed with a segmented shuffle scan and only the run's last lane issues the 8 vector
-// reductions red.global.add.v2.f32 — up to 32x fewer L2 atomics at the coarse levels; fine levels (every
-// lane its own run) take the direct path.  fp32 accumulation (the reference accumulates fp16 atomics of
-// grad*128, Hash3DAnchored.cu:145-151, and casts/divides afterwards); zero-gradient rows are skipped (:149).
-constexpr int kDirectHeads = 24;
-
+// Backward: a warp-task is (32 consecutive samples, one level): the task loads the lanes' gradient, point and volume and runs
+// scatter_level (hash.cuh: run merging + L2 reductions).
 // The grid is PERSISTENT and bounded (ctas_per_sm x SM count CTAs striding over the (32 samples, level) tasks): a few resident
 // warps per SM already saturate the reduction pipe, and a bounded grid lets the scatter of one ray chunk run on a side stream
 // next to the tensor-core kernels of the next chunk without crowding their CTAs out (an unbounded grid of 260 k small blocks did).
@@ -92,59 +85,14 @@ __device__ __forceinline__ void hash_bwd_task(int64_t group, int l, int lane, co
   }
   const bool live = valid && !(g0 == 0.f && g1 == 0.f);
   if (!__any_sync(0xffffffffu, live)) return;
-  g0 *= grad_mul; g1 *= grad_mul;
-  Corner8 c;
+  float x0 = 0.f, x1 = 0.f, x2 = 0.f;
   int v = -1;
   if (live) {
     const float p0 = __ldg(pts + i * 3), p1 = __ldg(pts + i * 3 + 1), p2 = __ldg(pts + i * 3 + 2);
-    const float x0 = fmul(fadd(p0, 1.f), .5f), x1 = fmul(fadd(p1, 1.f), .5f), x2 = fmul(fadd(p2, 1.f), .5f);
+    x0 = fmul(fadd(p0, 1.f), .5f); x1 = fmul(fadd(p1, 1.f), .5f); x2 = fmul(fadd(p2, 1.f), .5f);
     v = __ldg(vol + i * vol_stride);
-    const int tv = l * n_volumes + v;
-    corners(x0, x1, x2, level_scale(l), prim_pool + tv * 3, bias_pool + tv * 3, (unsigned)local_size, c);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; k++) { c.idx[k] = 0; c.w[k] = 0.f; }
-    c.cell[0] = c.cell[1] = c.cell[2] = 0;
   }
-  // run heads: key differs from the previous lane (dead lanes never merge)
-  const unsigned pcx = __shfl_up_sync(0xffffffffu, c.cell[0], 1), pcy = __shfl_up_sync(0xffffffffu, c.cell[1], 1),
-                 pcz = __shfl_up_sync(0xffffffffu, c.cell[2], 1);
-  const int prev_v = __shfl_up_sync(0xffffffffu, v, 1);       // dead lanes carry v = -1 and never merge
-  const bool head = (lane == 0) || !live || c.cell[0] != pcx || c.cell[1] != pcy || c.cell[2] != pcz || v != prev_v;
-  const unsigned heads = __ballot_sync(0xffffffffu, head);
-  float* base = grad_table + size_t(l) * local_size;
-  if (__popc(heads) > kDirectHeads) {                         // mostly singleton runs: direct reductions
-    if (live) {
-#pragma unroll
-      for (int k = 0; k < 8; k++)
-        atomicAdd(reinterpret_cast<float2*>(base + size_t(c.idx[k]) * 2), make_float2(c.w[k] * g0, c.w[k] * g1));
-    }
-    return;
-  }
-  // segmented inclusive scan within runs; the last lane of each run holds the run total
-  const unsigned below = heads & ((2u << lane) - 1u);         // heads at or below my lane
-  const int run_start = 31 - __clz(below);
-  float s[16];
-#pragma unroll
-  for (int k = 0; k < 8; k++) { s[2 * k] = c.w[k] * g0; s[2 * k + 1] = c.w[k] * g1; }
-  // only ceil(log2(longest run)) stages move data; the rest would be no-ops (warp-uniform early exit)
-  const int max_run = __reduce_max_sync(0xffffffffu, lane - run_start + 1);
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    if (o >= max_run) break;
-    const bool take = (lane - o) >= run_start;
-#pragma unroll
-    for (int k = 0; k < 16; k++) {
-      const float u = __shfl_up_sync(0xffffffffu, s[k], o);
-      if (take) s[k] += u;
-    }
-  }
-  const bool tail = (lane == 31) || ((heads >> (lane + 1)) & 1u);
-  if (live && tail) {
-#pragma unroll
-    for (int k = 0; k < 8; k++)
-      atomicAdd(reinterpret_cast<float2*>(base + size_t(c.idx[k]) * 2), make_float2(s[2 * k], s[2 * k + 1]));
-  }
+  scatter_level(l, lane, g0 * grad_mul, g1 * grad_mul, x0, x1, x2, v, live, prim_pool, bias_pool, n_volumes, local_size, grad_table);
 }
 
 template <bool GRAD_F16>

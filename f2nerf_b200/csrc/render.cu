@@ -97,8 +97,8 @@ extern "C" int f2b_render_phase2_fwd(const f2b_render* r) {
 extern "C" int f2b_render_bwd(const f2b_render* r) {
   F2B_REQUIRE(r, "f2b_render_bwd: null argument block");
   // the forward saved no hidden activations: f2b_mlp_bwd2 (hidden0 == NULL) rebuilds them from the input rows
-  const int64_t nk = r->n_kept, ne = 2 * int64_t(r->n_edge_pairs), nq = nk + ne;
-  cudaStream_t st = as_stream(r->stream), side = as_stream(r->side_stream);
+  const int64_t nk = r->n_kept, ne = 2 * int64_t(r->n_edge_pairs);
+  cudaStream_t st = as_stream(r->stream);
   const bool emb = r->app_emb && r->ray_emb_idx;
   F2B_CUDA(cudaMemsetAsync(r->d_sparams, 0, sizeof(float) * r->n_shader_params, st), "f2b_render_bwd");
   F2B_CUDA(cudaMemsetAsync(r->d_fparams, 0, sizeof(float) * r->n_field_params, st), "f2b_render_bwd");
@@ -116,31 +116,26 @@ extern "C" int f2b_render_bwd(const f2b_render* r) {
     F2B_TRY(f2b_mlp_bwd2(r->d_raw, r->mlp_in, nullptr, nullptr, r->sparams16, 1, (int)nk, r->d_in16, r->d_sparams, r->stream));
     F2B_TRY(f2b_shader_prep_bwd_f16(r->d_in16, r->d_logit, r->new_bounds, emb ? r->ray_emb_idx : nullptr, r->n_rays,
                                     1.f / r->shader_loss_scale, r->field_loss_scale, r->d_scene16, emb ? r->d_app : nullptr, r->stream));
-    F2B_TRY(f2b_mlp_bwd2(r->d_scene16, r->feat_q, nullptr, nullptr, r->fparams16, 0, (int)nk, r->dfeat16, r->d_fparams, r->stream));
   }
+  if (r->scatter_mode == 0) {
+    // field-MLP backward + hash scatter fused per segment: each tile's dL/dfeat rows go straight from shared memory into the
+    // table gradient (L2 reductions) while other CTAs run their MMAs; dfeat16 is not written
+    if (nk > 0)
+      F2B_TRY(f2b_field_bwd_scatter(r->d_scene16, r->feat_q, r->fparams16, (int)nk, r->pts, r->anchors, 3, r->prim, r->bias, r->n_volumes,
+                                    r->local_size, r->table_grad_mul, r->d_fparams, r->d_table, nullptr, r->stream));
+    if (ne > 0)
+      F2B_TRY(f2b_field_bwd_scatter(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), r->fparams16, (int)ne, r->e_pts, r->e_anc, 1,
+                                    r->prim, r->bias, r->n_volumes, r->local_size, r->table_grad_mul, r->d_fparams, r->d_table, nullptr,
+                                    r->stream));
+    return F2B_OK;
+  }
+  // scatter_mode 1: dL/dfeat rows to dfeat16; the caller scatters them level slab by level slab
+  if (nk > 0)
+    F2B_TRY(f2b_mlp_bwd2(r->d_scene16, r->feat_q, nullptr, nullptr, r->fparams16, 0, (int)nk, r->dfeat16, r->d_fparams, r->stream));
   if (ne > 0)
     F2B_TRY(f2b_mlp_bwd2(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), nullptr, nullptr, r->fparams16, 0, (int)ne,
                          off(r->dfeat16, nk * 64), r->d_fparams, r->stream));
-  if (r->scatter_mode != 0) return F2B_OK;
-  // the scatter (L2 reductions) on the side stream behind the dense chain, joined before returning
-  cudaEvent_t fork, join;
-  F2B_CUDA(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming), "f2b_render_bwd");
-  F2B_CUDA(cudaEventCreateWithFlags(&join, cudaEventDisableTiming), "f2b_render_bwd");
-  cudaEventRecord(fork, st);
-  cudaStreamWaitEvent(side, fork, 0);
-  int rc = F2B_OK;
-  if (nk > 0)
-    rc = f2b_hash_bwd(r->prim, r->bias, r->n_volumes, r->local_size, r->pts, r->anchors, 3, (int)nk, r->dfeat16, 1, r->table_grad_mul,
-                      r->d_table, r->side_stream);
-  if (rc == F2B_OK && ne > 0)
-    rc = f2b_hash_bwd(r->prim, r->bias, r->n_volumes, r->local_size, r->e_pts, r->e_anc, 1, (int)ne, off(r->dfeat16, nk * 64), 1,
-                      r->table_grad_mul, r->d_table, r->side_stream);
-  cudaEventRecord(join, side);
-  cudaStreamWaitEvent(st, join, 0);
-  cudaEventDestroy(fork);
-  cudaEventDestroy(join);
-  (void)nq;
-  return rc;
+  return F2B_OK;
 }
 
 extern "C" int f2b_render_grad_finalize(const f2b_render* r) {

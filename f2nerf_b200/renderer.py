@@ -520,21 +520,23 @@ class _FusedRenderFunction(torch.autograd.Function):
         f_scale = field.mlp_.loss_scale_
         grad_mul = (1.0 / f_scale) * (getattr(renderer, "grad_premul_", 1.0) if slab_hook is not None else 1.0)
         B = dict(d_logit=f32(n_kept), d_raw=f16(n_kept, 16), d_in16=f16(n_kept, 32), d_scene16=f16(n_kept + n_edge, 16),
-                 dfeat16=f16(n_kept + n_edge, 32), d_sparams=f32(ra.n_shader_params), d_fparams=f32(ra.n_field_params),
+                 d_sparams=f32(ra.n_shader_params), d_fparams=f32(ra.n_field_params),
                  d_table=renderer._table_grad_buffer(ctx.table_shape, dev),
                  nonfinite=torch.empty((2,), dtype=torch.int32, device=dev))
+        # dL/dfeat rows reach HBM only for the slab scatter below; otherwise f2b_render_bwd scatters them from shared memory
+        B["dfeat16"] = f16(n_kept + n_edge, 32) if slab_hook is not None else None
         if emb_on:
             B["d_app"] = torch.empty(ctx.emb_shape, dtype=torch.float32, device=dev)
-        side = renderer._side_stream(dev, 2)
         ra.set(d_colors=d_colors, d_disparity=d_disp, d_depth=d_depth, d_weights=d_weights, d_edge=d_edge,
                gs_progress=float(ctx.gs_progress), shader_loss_scale=float(shader.mlp_.loss_scale_), field_loss_scale=float(f_scale),
                table_grad_mul=float(grad_mul),
                # floats to zero-fill: the live prefix only when the buffer's dead tail is known to be zero already
                table_numel=min(B["d_table"].numel(), 17 * int(field.local_size_)) if renderer._table_grad_tail_zero else B["d_table"].numel(),
                table_live=min(B["d_table"].numel(), 17 * int(field.local_size_)), scatter_mode=int(slab_hook is not None),
-               stream=main.cuda_stream, side_stream=side.cuda_stream, **B)
+               stream=main.cuda_stream, **B)
         call("f2b_render_bwd", ra)
         if slab_hook is not None:                         # data parallel: level slabs top-down, all-reduce of each behind it (dist.py)
+            side = renderer._side_stream(dev, 2)
             hash_args = (field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_))
             jobs = [(T["pts"], T["anchors"], 3, 0, n_kept)] + ([(T["e_pts"], T["e_anc"], 1, n_kept, n_kept + n_edge)] if n_edge else [])
             ev = torch.cuda.Event()
@@ -625,13 +627,14 @@ class _RenderFunction(torch.autograd.Function):
         if ctx.gs_progress < 1.:                          # GradientScaling::backward draws an unused rand_like (CustomOps.cu:154)
             burn_rand(n_kept * 3, dev)
             burn_rand(n_kept, dev)
-        # ---- backward: the dense chain (composite -> sigmoid -> shader MLP -> input assembly -> field MLP; HBM streaming) on the
-        # main stream, the hash scatter (L2 reductions) on a side stream behind an event.
+        # ---- backward: the dense chain (composite -> sigmoid -> shader MLP -> input assembly -> field MLP) on the main stream.
+        # The default field MLP (no hidden matmul, activations not saved) runs its backward and the hash scatter (L2 reductions)
+        # as one kernel per segment, f2b_field_bwd_scatter; otherwise the scatter runs on a side stream behind an event.
         s_scale, f_scale = shader.mlp_.loss_scale_, field.mlp_.loss_scale_
         nh_s, nh_f = shader.mlp_.n_hidden_matmuls, field.mlp_.n_hidden_matmuls
         f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)
         d_logit = torch.empty((n_kept,), dtype=torch.float32, device=dev)
-        d_raw, d_in16, d_scene16, dfeat16 = f16(n_kept, 16), f16(n_kept, 32), f16(n_q, 16), f16(n_q, 32)
+        d_raw, d_in16, d_scene16 = f16(n_kept, 16), f16(n_kept, 32), f16(n_q, 16)
         d_sparams, d_fparams = zeros(sparams16.numel()), zeros(fparams16.numel())
         d_table = torch.zeros_like(field.feat_pool_)
         d_app = torch.zeros_like(renderer.app_emb_) if ray_emb_idx is not None else None
@@ -650,7 +653,13 @@ class _RenderFunction(torch.autograd.Function):
         # [l*S, (l+2)*S): the scatter then runs per level group, top-down, after the dense chain; the hook is called after each.
         slab_hook = getattr(renderer, "grad_slab_hook_", None)
         grad_mul = (1.0 / f_scale) * (getattr(renderer, "grad_premul_", 1.0) if slab_hook is not None else 1.0)
+        fused = slab_hook is None and nh_f == 0 and f_hidden is None
+        dfeat16 = None if fused else f16(n_q, 32)
         jobs = []
+
+        def field_bwd_scatter(pts, anc, stride, s0, s1):
+            call("f2b_field_bwd_scatter", d_scene16[s0:s1], feat16[s0:s1], fparams16, s1 - s0, pts, anc, int(stride), *hash_args,
+                 float(grad_mul), d_fparams, d_table, None, stream())
 
         def scatter(pts, anc, stride, s0, s1):            # on the side stream, behind everything queued on main so far
             if slab_hook is not None:
@@ -669,12 +678,17 @@ class _RenderFunction(torch.autograd.Function):
             call("f2b_mlp_bwd2", d_raw, mlp_in, None if s_hidden is None else s_hidden[0],
                  s_hidden[1] if (nh_s and s_hidden is not None) else None, sparams16, int(nh_s), n_kept, d_in16, d_sparams, stream())
             ops.shader_prep_bwd_f16(d_in16, d_logit, bounds, ray_emb_idx, 1.0 / s_scale, f_scale, d_scene16, d_app)
-            call("f2b_mlp_bwd2", d_scene16[:n_kept], feat16[:n_kept], None if f_hidden is None else f_hidden[0, :n_kept],
-                 f_hidden[1, :n_kept] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), n_kept, dfeat16[:n_kept],
-                 d_fparams, stream())
-            scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
+            if fused:
+                field_bwd_scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
+            else:
+                call("f2b_mlp_bwd2", d_scene16[:n_kept], feat16[:n_kept], None if f_hidden is None else f_hidden[0, :n_kept],
+                     f_hidden[1, :n_kept] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), n_kept,
+                     dfeat16[:n_kept], d_fparams, stream())
+                scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
         for pts_e, anc_e, stride_e, first, rows in segments[1:]:          # TV-loss edge points: field MLP + scatter only
-            if rows > 0:
+            if rows > 0 and fused:
+                field_bwd_scatter(pts_e, anc_e, stride_e, first, first + rows)
+            elif rows > 0:
                 call("f2b_mlp_bwd2", d_scene16[first:first + rows], feat16[first:first + rows],
                      None if f_hidden is None else f_hidden[0, first:first + rows],
                      f_hidden[1, first:first + rows] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), rows,

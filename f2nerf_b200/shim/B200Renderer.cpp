@@ -223,7 +223,7 @@ public:
     const float s_scale = shader->mlp_->loss_scale_, f_scale = field->mlp_->loss_scale_;
     Tensor d_logit = torch::empty({n_kept}, CUDAFloat);
     Tensor d_raw = torch::empty({n_kept, 16}, kHalf), d_in16 = torch::empty({n_kept, 32}, kHalf);
-    Tensor d_scene16 = torch::empty({n_q, 16}, kHalf), dfeat16 = torch::empty({n_q, 32}, kHalf);
+    Tensor d_scene16 = torch::empty({n_q, 16}, kHalf);
     Tensor d_sparams = torch::zeros({k.sparams16.numel()}, CUDAFloat), d_fparams = torch::zeros({k.fparams16.numel()}, CUDAFloat);
     const int64_t table_numel = ctx->saved_data["table_numel"].toInt();
     const int local_size = ((field->pool_size_ / N_LEVELS) >> 4) << 4;
@@ -254,14 +254,15 @@ public:
                            cur_stream()));
     F2B_CHECK(f2b_shader_prep_bwd_f16(P(d_in16), PF(d_logit), PI(k.bounds), emb_on ? PI(k.ray_emb_idx) : nullptr, n_rays,
                                       1.f / s_scale, f_scale, P(d_scene16), PF(d_app), cur_stream()));
-    F2B_CHECK(f2b_mlp_bwd2(P(d_scene16), P(k.feat16), nullptr, nullptr, P(k.fparams16), 0, (int) n_q, P(dfeat16),
-                           PF(d_fparams), cur_stream()));
-    F2B_CHECK(f2b_hash_bwd(field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
-                           PF(k.pts), PI(k.anchors), 3, (int) n_kept, P(dfeat16), 1, 1.f / f_scale, PF(d_table), cur_stream()));
+    // field-MLP backward + hash scatter, one kernel per segment (ray samples, TV-loss edge points), as f2b_render_bwd issues them
+    F2B_CHECK(f2b_field_bwd_scatter(P(d_scene16), P(k.feat16), P(k.fparams16), (int) n_kept, PF(k.pts), PI(k.anchors), 3,
+                                    field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
+                                    1.f / f_scale, PF(d_fparams), PF(d_table), nullptr, cur_stream()));
     if (n_q > n_kept) {
-      F2B_CHECK(f2b_hash_bwd(field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
-                             PF(k.e_pts), PI(k.e_anc), 1, (int) (n_q - n_kept), (char*) P(dfeat16) + n_kept * 64, 1, 1.f / f_scale,
-                             PF(d_table), cur_stream()));
+      F2B_CHECK(f2b_field_bwd_scatter((char*) P(d_scene16) + n_kept * 32, (char*) P(k.feat16) + n_kept * 64, P(k.fparams16),
+                                      (int) (n_q - n_kept), PF(k.e_pts), PI(k.e_anc), 1, field->prim_pool_.data_ptr<int>(),
+                                      field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size, 1.f / f_scale, PF(d_fparams),
+                                      PF(d_table), nullptr, cur_stream()));
     }
     d_sparams = d_sparams / s_scale;
     d_fparams = d_fparams / f_scale;

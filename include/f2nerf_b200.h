@@ -188,6 +188,15 @@ int f2b_shader_mlp_rgb_fwd(const void* mlp_in_f16, const void* shader_params_f16
  * 96 B read + 64 B written per sample instead of 224 / 352 + 64 (and the forward does not write 128 / 256 B). */
 int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void* hidden0_f16, const void* hidden1_f16,
                  const void* params_f16, int n_hidden_matmuls, int n_pts, void* din_f16, float* dparams_f32, void* stream);
+/* Field-MLP backward (32->64->16, no hidden matmul, activations rebuilt from feat_f16 like f2b_mlp_bwd2 with hidden0 == NULL)
+ * and f2b_hash_bwd of its dL/dfeat rows in ONE kernel: each 128-row tile's dL/dfeat stays in shared memory and is scattered
+ * into grad_table_f32 (times grad_mul) right behind the tile's MMAs.  Same table-gradient reductions as f2b_hash_bwd(grad_is_f16
+ * = 1) on f2b_mlp_bwd2's fp16 rows; dparams_f32 is accumulated into.  pts [P,3], vol[i * vol_stride] as in f2b_hash_bwd.
+ * din_f16 [P,32] (nullable) also receives the fp16 dL/dfeat rows, bit-identical to f2b_mlp_bwd2's. */
+int f2b_field_bwd_scatter(const void* dout_f16, const void* feat_f16, const void* params_f16, int n_pts, const float* pts,
+                          const int* vol, int vol_stride, const int* prim_pool, const float* bias_pool, int n_volumes,
+                          int local_size, float grad_mul, float* dparams_f32, float* grad_table_f32, void* din_f16 /* nullable */,
+                          void* stream);
 
 /* Which kernels the MLP entry points above run: always 1 = the wgmma tensor-core kernels (recorded by benchmarks). */
 int f2b_get_mlp_impl(void);
@@ -349,7 +358,7 @@ int f2b_weight_var_bwd(const float* weights, const int* idx_start_end, int n_out
  *                          field MLP + shader-input epilogue -> edge-point MLP -> shader MLP + colour activation ->
  *                          composite                                                             (Renderer.cpp:127-208)
  *   f2b_render_bwd         zero-fills -> composite/activation bwd -> shader MLP bwd -> input-assembly bwd -> field MLP bwd
- *                          (ray samples, edge points) -> [scatter_mode 0: hash scatter of both on side_stream, joined]
+ *                          (ray samples, edge points) with, in scatter_mode 0, the hash scatter fused into it (f2b_field_bwd_scatter)
  *   f2b_render_grad_finalize  un-scale the two MLP gradients (TCNNWP.cpp:225-229) and raise the per-MLP non-finite flags
  *                          (dL/dparams, and dL/dinput through d_app / the live table gradient; TCNNWP.cpp:231-240)
  * ------------------------------------------------------------------------------------------ */
@@ -380,11 +389,11 @@ typedef struct f2b_render {
   /* backward */
   const float* d_colors; const float* d_disparity; const float* d_depth; const float* d_weights; const float* d_edge /* [2*pairs,16] */;
   float gs_progress, shader_loss_scale, field_loss_scale, table_grad_mul;
-  float* d_logit; void* d_raw; void* d_in16; void* d_scene16; void* dfeat16;
+  float* d_logit; void* d_raw; void* d_in16; void* d_scene16; void* dfeat16 /* scatter_mode 1 only */;
   float* d_sparams; float* d_fparams; float* d_table; int64_t table_numel; int64_t table_live; float* d_app;
   int scatter_mode;                                      /* 0: scatter inside f2b_render_bwd; 1: the caller scatters (level slabs) */
   int* nonfinite;                                        /* [2] device ints: shader MLP, field MLP */
-  void* stream; void* side_stream;
+  void* stream;
 } f2b_render;
 int f2b_render_sizeof(void);                 /* sizeof(f2b_render) as the library was built: bindings compare it with their own */
 int f2b_render_phase1(const f2b_render* r);

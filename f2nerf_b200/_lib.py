@@ -57,6 +57,8 @@ SIGNATURES = {
     "f2b_shader_mlp_rgb_fwd": [_P, _P, c_int, _P, _P, _P, _P],
     "f2b_mlp_bwd2": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_field_bwd_scatter": [_P, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_float, _P, _P, _P, _P],
+    "f2b_shade_field_bwd_scatter": [_P, _P, _P, _P, _P, c_float, c_float, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_float,
+                                    _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_mlp_fwd_v0": [_P, _P, c_int, c_int, _P, _P, _P],
     "f2b_mlp_bwd_v0": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_field_fwd": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P],
@@ -125,6 +127,7 @@ class RenderArgs(ctypes.Structure):
         ("d_sparams", _P), ("d_fparams", _P), ("d_table", _P), ("table_numel", _L), ("table_live", _L), ("d_app", _P),
         ("scatter_mode", _I),
         ("nonfinite", _P),
+        ("tile_ticket", _P),
         ("stream", _P),
     ]
 

@@ -100,40 +100,44 @@ extern "C" int f2b_render_bwd(const f2b_render* r) {
   const int64_t nk = r->n_kept, ne = 2 * int64_t(r->n_edge_pairs);
   cudaStream_t st = as_stream(r->stream);
   const bool emb = r->app_emb && r->ray_emb_idx;
+  char* const d_edge16 = r->scatter_mode == 0 ? off(r->d_scene16, 0) : off(r->d_scene16, nk * 32);   // the edge points' dL/dout rows
   F2B_CUDA(cudaMemsetAsync(r->d_sparams, 0, sizeof(float) * r->n_shader_params, st), "f2b_render_bwd");
   F2B_CUDA(cudaMemsetAsync(r->d_fparams, 0, sizeof(float) * r->n_field_params, st), "f2b_render_bwd");
   F2B_CUDA(cudaMemsetAsync(r->d_table, 0, sizeof(float) * r->table_numel, st), "f2b_render_bwd");
   F2B_CUDA(cudaMemsetAsync(r->nonfinite, 0, 2 * sizeof(int), st), "f2b_render_bwd");
   if (emb) F2B_CUDA(cudaMemsetAsync(r->d_app, 0, sizeof(float) * 16 * r->n_emb, st), "f2b_render_bwd");
   if (ne > 0) {                                                    // dL/d edge features -> the field MLP's fp16, loss-scaled dL/dout rows
-    if (r->d_edge) F2B_TRY(f2b_cast_f32_to_f16(r->d_edge, off(r->d_scene16, nk * 32), ne * 16, r->field_loss_scale, r->stream));
-    else F2B_CUDA(cudaMemsetAsync(off(r->d_scene16, nk * 32), 0, ne * 32, st), "f2b_render_bwd");
+    if (r->d_edge) F2B_TRY(f2b_cast_f32_to_f16(r->d_edge, d_edge16, ne * 16, r->field_loss_scale, r->stream));
+    else F2B_CUDA(cudaMemsetAsync(d_edge16, 0, ne * 32, st), "f2b_render_bwd");
   }
-  if (nk > 0) {
+  if (nk > 0)
     F2B_TRY(f2b_composite_act_bwd(r->logit, 1, r->rgb, r->dt, r->t, r->new_bounds, r->bg, r->n_rays, r->d_colors, r->d_disparity,
                                   r->d_depth, r->d_weights, r->gs_progress, r->raw, r->shader_loss_scale, r->d_logit, 1, r->d_raw,
                                   r->stream));
-    F2B_TRY(f2b_mlp_bwd2(r->d_raw, r->mlp_in, nullptr, nullptr, r->sparams16, 1, (int)nk, r->d_in16, r->d_sparams, r->stream));
-    F2B_TRY(f2b_shader_prep_bwd_f16(r->d_in16, r->d_logit, r->new_bounds, emb ? r->ray_emb_idx : nullptr, r->n_rays,
-                                    1.f / r->shader_loss_scale, r->field_loss_scale, r->d_scene16, emb ? r->d_app : nullptr, r->stream));
-  }
   if (r->scatter_mode == 0) {
-    // field-MLP backward + hash scatter fused per segment: each tile's dL/dfeat rows go straight from shared memory into the
-    // table gradient (L2 reductions) while other CTAs run their MMAs; dfeat16 is not written
+    // ray samples: shader-MLP backward, input-assembly backward, field-MLP backward and hash scatter in one kernel (the MMAs run
+    // under the scatter's L2 reductions; d_in16 and the rays' dL/dout rows stay in shared memory).  Edge points: field-MLP
+    // backward + hash scatter fused
     if (nk > 0)
-      F2B_TRY(f2b_field_bwd_scatter(r->d_scene16, r->feat_q, r->fparams16, (int)nk, r->pts, r->anchors, 3, r->prim, r->bias, r->n_volumes,
-                                    r->local_size, r->table_grad_mul, r->d_fparams, r->d_table, nullptr, r->stream));
+      F2B_TRY(f2b_shade_field_bwd_scatter(r->d_raw, r->mlp_in, r->sparams16, r->d_logit, emb ? r->pt_emb_idx : nullptr,
+                                          1.f / r->shader_loss_scale, r->field_loss_scale, r->feat_q, r->fparams16, (int)nk, r->pts,
+                                          r->anchors, 3, r->prim, r->bias, r->n_volumes, r->local_size, r->table_grad_mul, r->d_sparams,
+                                          r->d_fparams, r->d_table, emb ? r->d_app : nullptr, r->tile_ticket, nullptr, nullptr, nullptr,
+                                          r->stream));
     if (ne > 0)
-      F2B_TRY(f2b_field_bwd_scatter(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), r->fparams16, (int)ne, r->e_pts, r->e_anc, 1,
-                                    r->prim, r->bias, r->n_volumes, r->local_size, r->table_grad_mul, r->d_fparams, r->d_table, nullptr,
-                                    r->stream));
+      F2B_TRY(f2b_field_bwd_scatter(d_edge16, off(r->feat_q, nk * 64), r->fparams16, (int)ne, r->e_pts, r->e_anc, 1, r->prim, r->bias,
+                                    r->n_volumes, r->local_size, r->table_grad_mul, r->d_fparams, r->d_table, nullptr, r->stream));
     return F2B_OK;
   }
   // scatter_mode 1: dL/dfeat rows to dfeat16; the caller scatters them level slab by level slab
-  if (nk > 0)
+  if (nk > 0) {
+    F2B_TRY(f2b_mlp_bwd2(r->d_raw, r->mlp_in, nullptr, nullptr, r->sparams16, 1, (int)nk, r->d_in16, r->d_sparams, r->stream));
+    F2B_TRY(f2b_shader_prep_bwd_f16(r->d_in16, r->d_logit, r->new_bounds, emb ? r->ray_emb_idx : nullptr, r->n_rays,
+                                    1.f / r->shader_loss_scale, r->field_loss_scale, r->d_scene16, emb ? r->d_app : nullptr, r->stream));
     F2B_TRY(f2b_mlp_bwd2(r->d_scene16, r->feat_q, nullptr, nullptr, r->fparams16, 0, (int)nk, r->dfeat16, r->d_fparams, r->stream));
+  }
   if (ne > 0)
-    F2B_TRY(f2b_mlp_bwd2(off(r->d_scene16, nk * 32), off(r->feat_q, nk * 64), nullptr, nullptr, r->fparams16, 0, (int)ne,
+    F2B_TRY(f2b_mlp_bwd2(d_edge16, off(r->feat_q, nk * 64), nullptr, nullptr, r->fparams16, 0, (int)ne,
                          off(r->dfeat16, nk * 64), r->d_fparams, r->stream));
   return F2B_OK;
 }

@@ -519,12 +519,16 @@ class _FusedRenderFunction(torch.autograd.Function):
         slab_hook = getattr(renderer, "grad_slab_hook_", None)
         f_scale = field.mlp_.loss_scale_
         grad_mul = (1.0 / f_scale) * (getattr(renderer, "grad_premul_", 1.0) if slab_hook is not None else 1.0)
-        B = dict(d_logit=f32(n_kept), d_raw=f16(n_kept, 16), d_in16=f16(n_kept, 32), d_scene16=f16(n_kept + n_edge, 16),
+        B = dict(d_logit=f32(n_kept), d_raw=f16(n_kept, 16),
                  d_sparams=f32(ra.n_shader_params), d_fparams=f32(ra.n_field_params),
                  d_table=renderer._table_grad_buffer(ctx.table_shape, dev),
-                 nonfinite=torch.empty((2,), dtype=torch.int32, device=dev))
-        # dL/dfeat rows reach HBM only for the slab scatter below; otherwise f2b_render_bwd scatters them from shared memory
-        B["dfeat16"] = f16(n_kept + n_edge, 32) if slab_hook is not None else None
+                 nonfinite=torch.empty((2,), dtype=torch.int32, device=dev), tile_ticket=torch.empty((1,), dtype=torch.int32, device=dev))
+        # dL/dinput, dL/dout and dL/dfeat rows of the ray samples reach HBM only for the slab scatter below; otherwise
+        # f2b_render_bwd keeps them in shared memory and d_scene16 holds the edge points' rows only
+        if slab_hook is not None:
+            B.update(d_in16=f16(n_kept, 32), d_scene16=f16(n_kept + n_edge, 16), dfeat16=f16(n_kept + n_edge, 32))
+        else:
+            B.update(d_in16=None, d_scene16=f16(n_edge, 16), dfeat16=None)
         if emb_on:
             B["d_app"] = torch.empty(ctx.emb_shape, dtype=torch.float32, device=dev)
         ra.set(d_colors=d_colors, d_disparity=d_disp, d_depth=d_depth, d_weights=d_weights, d_edge=d_edge,
@@ -599,7 +603,7 @@ class _RenderFunction(torch.autograd.Function):
         scene_feat = (logit, logit_stride)
         edge_feats = edge32.reshape(-1, 2, 16)
         ctx.renderer, ctx.es, ctx.n_kept = renderer, es, n_kept
-        ctx.pack = (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw,
+        ctx.pack = (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, pt_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw,
                     s_hidden, rgb)
         ctx.gs_progress = renderer.global_data_pool_.gradient_scaling_progress_
         ctx.grad_on = grad_on
@@ -612,7 +616,7 @@ class _RenderFunction(torch.autograd.Function):
         if ctx.pack is None:
             raise RuntimeError("Renderer.Render backward: the saved activations were released by a previous backward "
                                "(like tiny-cuda-nn's context, TCNNWP.cpp:207, the graph can be traversed once)")
-        (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw, s_hidden,
+        (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, pt_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw, s_hidden,
          rgb) = ctx.pack
         if not ctx.grad_on:
             raise RuntimeError("Renderer.Render backward: forward ran without grad (VALIDATE mode / no_grad)")
@@ -628,21 +632,17 @@ class _RenderFunction(torch.autograd.Function):
             burn_rand(n_kept * 3, dev)
             burn_rand(n_kept, dev)
         # ---- backward: the dense chain (composite -> sigmoid -> shader MLP -> input assembly -> field MLP) on the main stream.
-        # The default field MLP (no hidden matmul, activations not saved) runs its backward and the hash scatter (L2 reductions)
-        # as one kernel per segment, f2b_field_bwd_scatter; otherwise the scatter runs on a side stream behind an event.
+        # With the default MLPs (field without, shader with one hidden matmul, activations not saved) everything behind the
+        # composite runs fused with the hash scatter (L2 reductions): f2b_shade_field_bwd_scatter for the ray samples,
+        # f2b_field_bwd_scatter for the edge points.  Otherwise the scatter runs on a side stream behind an event.
         s_scale, f_scale = shader.mlp_.loss_scale_, field.mlp_.loss_scale_
         nh_s, nh_f = shader.mlp_.n_hidden_matmuls, field.mlp_.n_hidden_matmuls
         f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)
         d_logit = torch.empty((n_kept,), dtype=torch.float32, device=dev)
-        d_raw, d_in16, d_scene16 = f16(n_kept, 16), f16(n_kept, 32), f16(n_q, 16)
+        d_raw = f16(n_kept, 16)
         d_sparams, d_fparams = zeros(sparams16.numel()), zeros(fparams16.numel())
         d_table = torch.zeros_like(field.feat_pool_)
         d_app = torch.zeros_like(renderer.app_emb_) if ray_emb_idx is not None else None
-        if n_q > n_kept:
-            if d_edge is not None:
-                d_scene16[n_kept:] = (d_edge.reshape(-1, 16) * f_scale).to(torch.float16)
-            else:
-                d_scene16[n_kept:].zero_()
         main = torch.cuda.current_stream(dev)
         side = renderer._side_stream(dev, 2)
         bounds = es.pts_idx_bounds
@@ -654,11 +654,21 @@ class _RenderFunction(torch.autograd.Function):
         slab_hook = getattr(renderer, "grad_slab_hook_", None)
         grad_mul = (1.0 / f_scale) * (getattr(renderer, "grad_premul_", 1.0) if slab_hook is not None else 1.0)
         fused = slab_hook is None and nh_f == 0 and f_hidden is None
+        shade_fused = fused and nh_s == 1 and s_hidden is None
         dfeat16 = None if fused else f16(n_q, 32)
+        # the ray samples' dL/dinput and dL/dout rows stay in shared memory when shade_fused: d_scene16 then holds the edge rows only
+        d_in16 = None if shade_fused else f16(n_kept, 32)
+        row0 = n_kept if shade_fused else 0              # d_scene16 row of sample `row0`
+        d_scene16 = f16(n_q - row0, 16)
+        if n_q > n_kept:
+            if d_edge is not None:
+                d_scene16[n_kept - row0:] = (d_edge.reshape(-1, 16) * f_scale).to(torch.float16)
+            else:
+                d_scene16[n_kept - row0:].zero_()
         jobs = []
 
         def field_bwd_scatter(pts, anc, stride, s0, s1):
-            call("f2b_field_bwd_scatter", d_scene16[s0:s1], feat16[s0:s1], fparams16, s1 - s0, pts, anc, int(stride), *hash_args,
+            call("f2b_field_bwd_scatter", d_scene16[s0 - row0:s1 - row0], feat16[s0:s1], fparams16, s1 - s0, pts, anc, int(stride), *hash_args,
                  float(grad_mul), d_fparams, d_table, None, stream())
 
         def scatter(pts, anc, stride, s0, s1):            # on the side stream, behind everything queued on main so far
@@ -675,6 +685,12 @@ class _RenderFunction(torch.autograd.Function):
             # composite backward with the colour activation's backward applied on the way out (fp16 d_raw directly)
             call("f2b_composite_act_bwd", scene_feat[0], int(scene_feat[1]), rgb, es.dt, es.t, bounds, bg, n_rays, d_colors, d_disp,
                  d_depth, d_weights, float(ctx.gs_progress), raw, float(s_scale), d_logit, 1, d_raw, stream())
+        if n_kept > 0 and shade_fused:
+            pts, anc, stride = segments[0][:3]
+            call("f2b_shade_field_bwd_scatter", d_raw, mlp_in, sparams16, d_logit, pt_emb_idx, float(1.0 / s_scale), float(f_scale),
+                 feat16, fparams16, n_kept, pts, anc, int(stride), *hash_args, float(grad_mul), d_sparams, d_fparams, d_table, d_app,
+                 torch.empty((1,), dtype=torch.int32, device=dev), None, None, None, stream())
+        elif n_kept > 0:
             call("f2b_mlp_bwd2", d_raw, mlp_in, None if s_hidden is None else s_hidden[0],
                  s_hidden[1] if (nh_s and s_hidden is not None) else None, sparams16, int(nh_s), n_kept, d_in16, d_sparams, stream())
             ops.shader_prep_bwd_f16(d_in16, d_logit, bounds, ray_emb_idx, 1.0 / s_scale, f_scale, d_scene16, d_app)

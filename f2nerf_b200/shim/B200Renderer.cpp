@@ -222,8 +222,9 @@ public:
     if (k.gs_progress < 1.f) { burn_rand(n_kept * 3); burn_rand(n_kept); }       // GradientScaling::backward's rand_like
     const float s_scale = shader->mlp_->loss_scale_, f_scale = field->mlp_->loss_scale_;
     Tensor d_logit = torch::empty({n_kept}, CUDAFloat);
-    Tensor d_raw = torch::empty({n_kept, 16}, kHalf), d_in16 = torch::empty({n_kept, 32}, kHalf);
-    Tensor d_scene16 = torch::empty({n_q, 16}, kHalf);
+    Tensor d_raw = torch::empty({n_kept, 16}, kHalf);
+    Tensor d_edge16 = torch::empty({n_q - n_kept, 16}, kHalf);      // the edge points' field dL/dout rows (the rays' stay on chip)
+    Tensor ticket = torch::empty({1}, CUDAInt);
     Tensor d_sparams = torch::zeros({k.sparams16.numel()}, CUDAFloat), d_fparams = torch::zeros({k.fparams16.numel()}, CUDAFloat);
     const int64_t table_numel = ctx->saved_data["table_numel"].toInt();
     const int local_size = ((field->pool_size_ / N_LEVELS) >> 4) << 4;
@@ -243,23 +244,21 @@ public:
     const bool emb_on = k.ray_emb_idx.defined();
     Tensor d_app = emb_on ? torch::zeros({ctx->saved_data["n_emb"].toInt(), 16}, CUDAFloat) : Tensor();
     if (n_q > n_kept) {
-      if (d_edge.defined()) d_scene16.slice(0, n_kept, n_q).copy_((d_edge.reshape({-1, 16}) * f_scale).to(torch::kFloat16));
-      else d_scene16.slice(0, n_kept, n_q).zero_();
+      if (d_edge.defined()) d_edge16.copy_((d_edge.reshape({-1, 16}) * f_scale).to(torch::kFloat16));
+      else d_edge16.zero_();
     }
     F2B_CHECK(f2b_composite_act_bwd(PF(k.logit), 1, PF(k.rgb), PF(k.dt), PF(k.t), PI(k.bounds), PF(k.bg), n_rays, PF(d_colors),
                                     PF(d_disp), PF(d_depth), PF(d_weights), k.gs_progress, P(k.raw), s_scale, PF(d_logit), 1,
                                     P(d_raw), cur_stream()));
-    // the forward saved no hidden activations: f2b_mlp_bwd2 (hidden0 == NULL) rebuilds them from the input rows
-    F2B_CHECK(f2b_mlp_bwd2(P(d_raw), P(k.mlp_in), nullptr, nullptr, P(k.sparams16), 1, (int) n_kept, P(d_in16), PF(d_sparams),
-                           cur_stream()));
-    F2B_CHECK(f2b_shader_prep_bwd_f16(P(d_in16), PF(d_logit), PI(k.bounds), emb_on ? PI(k.ray_emb_idx) : nullptr, n_rays,
-                                      1.f / s_scale, f_scale, P(d_scene16), PF(d_app), cur_stream()));
-    // field-MLP backward + hash scatter, one kernel per segment (ray samples, TV-loss edge points), as f2b_render_bwd issues them
-    F2B_CHECK(f2b_field_bwd_scatter(P(d_scene16), P(k.feat16), P(k.fparams16), (int) n_kept, PF(k.pts), PI(k.anchors), 3,
-                                    field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
-                                    1.f / f_scale, PF(d_fparams), PF(d_table), nullptr, cur_stream()));
+    // as f2b_render_bwd issues them: the ray samples' shader-MLP, input-assembly and field-MLP backward with their hash scatter in
+    // one kernel (activations rebuilt from the input rows), then the TV-loss edge points' field-MLP backward + scatter
+    F2B_CHECK(f2b_shade_field_bwd_scatter(P(d_raw), P(k.mlp_in), P(k.sparams16), PF(d_logit), emb_on ? PI(k.pt_emb_idx) : nullptr,
+                                          1.f / s_scale, f_scale, P(k.feat16), P(k.fparams16), (int) n_kept, PF(k.pts), PI(k.anchors), 3,
+                                          field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_,
+                                          local_size, 1.f / f_scale, PF(d_sparams), PF(d_fparams), PF(d_table), PF(d_app), PI(ticket),
+                                          nullptr, nullptr, nullptr, cur_stream()));
     if (n_q > n_kept) {
-      F2B_CHECK(f2b_field_bwd_scatter((char*) P(d_scene16) + n_kept * 32, (char*) P(k.feat16) + n_kept * 64, P(k.fparams16),
+      F2B_CHECK(f2b_field_bwd_scatter(P(d_edge16), (char*) P(k.feat16) + n_kept * 64, P(k.fparams16),
                                       (int) (n_q - n_kept), PF(k.e_pts), PI(k.e_anc), 1, field->prim_pool_.data_ptr<int>(),
                                       field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size, 1.f / f_scale, PF(d_fparams),
                                       PF(d_table), nullptr, cur_stream()));

@@ -197,6 +197,20 @@ int f2b_field_bwd_scatter(const void* dout_f16, const void* feat_f16, const void
                           const int* vol, int vol_stride, const int* prim_pool, const float* bias_pool, int n_volumes,
                           int local_size, float grad_mul, float* dparams_f32, float* grad_table_f32, void* din_f16 /* nullable */,
                           void* stream);
+/* The per-sample backward of the ray samples in ONE kernel: the shader-MLP backward (32->64->64->16, activations rebuilt from
+ * mlp_in_f16 like f2b_mlp_bwd2 with n_hidden_matmuls = 1 and hidden0 == NULL) -> f2b_shader_prep_bwd_f16's input-assembly
+ * backward -> f2b_field_bwd_scatter.  d_raw_f16 [P,16] is the shader MLP's dL/dout, d_logit [P] the composite's.  Same values as
+ * that sequence: the field's dL/dout rows bit-identical, the same table-gradient reductions; weight gradients accumulate into
+ * d_sparams_f32 / d_fparams_f32.  pt_emb_idx [P] (per-sample camera index) and d_app_emb [n_emb,16] go together: when given,
+ * d_app_emb[pt_emb_idx[p]] += d mlp_in[p,0:16] * inv_loss_scale; both NULL without appearance embedding.  ticket: one device
+ * int of scratch (tiles are handed out through it; zeroed here).  Nullable outputs, written only when given: d_in16 [P,32] the
+ * shader's fp16 dL/dinput rows, d_scene16 [P,16] the field's fp16 dL/dout rows, dfeat16 [P,32] the field's fp16 dL/dfeat rows. */
+int f2b_shade_field_bwd_scatter(const void* d_raw_f16, const void* mlp_in_f16, const void* sparams_f16, const float* d_logit,
+                                const int* pt_emb_idx, float inv_loss_scale, float field_loss_scale, const void* feat_f16,
+                                const void* fparams_f16, int n_pts, const float* pts, const int* vol, int vol_stride,
+                                const int* prim_pool, const float* bias_pool, int n_volumes, int local_size, float grad_mul,
+                                float* d_sparams_f32, float* d_fparams_f32, float* grad_table_f32, float* d_app_emb, int* ticket,
+                                void* d_in16, void* d_scene16, void* dfeat16, void* stream);
 
 /* Which kernels the MLP entry points above run: always 1 = the wgmma tensor-core kernels (recorded by benchmarks). */
 int f2b_get_mlp_impl(void);
@@ -358,7 +372,9 @@ int f2b_weight_var_bwd(const float* weights, const int* idx_start_end, int n_out
  *                          field MLP + shader-input epilogue -> edge-point MLP -> shader MLP + colour activation ->
  *                          composite                                                             (Renderer.cpp:127-208)
  *   f2b_render_bwd         zero-fills -> composite/activation bwd -> shader MLP bwd -> input-assembly bwd -> field MLP bwd
- *                          (ray samples, edge points) with, in scatter_mode 0, the hash scatter fused into it (f2b_field_bwd_scatter)
+ *                          (ray samples, edge points); scatter_mode 0 runs the ray samples' part and their hash scatter as one
+ *                          kernel (f2b_shade_field_bwd_scatter) and the edge points' field MLP bwd + scatter as another
+ *                          (f2b_field_bwd_scatter)
  *   f2b_render_grad_finalize  un-scale the two MLP gradients (TCNNWP.cpp:225-229) and raise the per-MLP non-finite flags
  *                          (dL/dparams, and dL/dinput through d_app / the live table gradient; TCNNWP.cpp:231-240)
  * ------------------------------------------------------------------------------------------ */
@@ -389,10 +405,14 @@ typedef struct f2b_render {
   /* backward */
   const float* d_colors; const float* d_disparity; const float* d_depth; const float* d_weights; const float* d_edge /* [2*pairs,16] */;
   float gs_progress, shader_loss_scale, field_loss_scale, table_grad_mul;
-  float* d_logit; void* d_raw; void* d_in16; void* d_scene16; void* dfeat16 /* scatter_mode 1 only */;
+  float* d_logit; void* d_raw;
+  void* d_in16 /* scatter_mode 1 only */;
+  void* d_scene16;                                       /* [n_kept + 2*pairs, 16]; scatter_mode 0: the edge rows [2*pairs, 16] only */
+  void* dfeat16 /* scatter_mode 1 only */;
   float* d_sparams; float* d_fparams; float* d_table; int64_t table_numel; int64_t table_live; float* d_app;
   int scatter_mode;                                      /* 0: scatter inside f2b_render_bwd; 1: the caller scatters (level slabs) */
   int* nonfinite;                                        /* [2] device ints: shader MLP, field MLP */
+  int* tile_ticket;                                      /* [1] device int scratch of f2b_shade_field_bwd_scatter (scatter_mode 0) */
   void* stream;
 } f2b_render;
 int f2b_render_sizeof(void);                 /* sizeof(f2b_render) as the library was built: bindings compare it with their own */

@@ -4,8 +4,9 @@
   python scripts/bwd_probe.py [--out profiles/h100_bwd_probe.json] [--red-rate profiles/h100_red_rate.json] [--iters 60]
 
 Runs one TRAIN step through Renderer._render_per_kernel and keeps the inputs of the field-MLP backward + hash scatter of the
-ray samples (dL/dout rows, encoded features, fp16 field parameters, compacted points / anchors; the TV-loss edge segment is
-reported by size).  Then times, with CUDA events (median of --iters launches after warm-up, table gradient zeroed before each):
+ray samples (encoded features, fp16 field parameters, compacted points / anchors; the TV-loss edge segment is reported by size).
+That step runs the rays' shader backward fused into the same kernel (f2b_shade_field_bwd_scatter), so their field dL/dout rows
+are rebuilt here with the unfused kernels, f2b_mlp_bwd2 (shader) and f2b_shader_prep_bwd_f16.  Then times, with CUDA events (median of --iters launches after warm-up, table gradient zeroed before each):
   f2b_mlp_bwd2 (field, rays) | f2b_hash_bwd (rays) | the two in sequence | f2b_field_bwd_scatter (rays, the fused kernel).
 The reductions the scatter issues are counted on the host (numpy restatement of the cell key of corners() and of the run rule
 of scatter_level, hash.cuh), so the achieved lane-reduction rate can be set against the microbenchmark's v2f32 `spread` peak
@@ -80,9 +81,9 @@ def main():
     kept = []
     real_call = R.call
 
-    def spy(name, *a):                       # keep the inputs of the field backward + scatter of each segment
-        if name == "f2b_field_bwd_scatter":
-            kept.append([t.clone() if isinstance(t, torch.Tensor) else t for t in a])
+    def spy(name, *a):                       # keep the inputs of the backward behind the composite, per segment
+        if name in ("f2b_shade_field_bwd_scatter", "f2b_field_bwd_scatter", "f2b_composite_act_bwd"):
+            kept.append([name] + [t.clone() if isinstance(t, torch.Tensor) else t for t in a])
         return real_call(name, *a)
 
     R.call = spy
@@ -95,9 +96,18 @@ def main():
         torch.cuda.synchronize()
     finally:
         R.call = real_call
-    assert kept, "the per-kernel backward did not run f2b_field_bwd_scatter"
-    (dout, feat, fparams16, n, pts, anc, stride, prim, bias, n_vol, S, grad_mul, d_fp, d_table, _, _) = kept[0]
-    edge_rows = int(kept[1][3]) if len(kept) > 1 else 0
+    names = [k[0] for k in kept]
+    assert names[:2] == ["f2b_composite_act_bwd", "f2b_shade_field_bwd_scatter"], names
+    bounds = kept[0][1 + 5]
+    (d_raw, mlp_in, sp16, d_logit, pt_emb, inv_s, f_scale, feat, fparams16, n, pts, anc, stride, prim, bias, n_vol, S, grad_mul,
+     d_sp, d_fp, d_table, d_app) = kept[1][1:23]
+    edge_rows = int(kept[2][1 + 3]) if len(kept) > 2 else 0
+    d_in16 = torch.empty((n, 32), dtype=torch.float16, device=dev)
+    dout = torch.empty((n, 16), dtype=torch.float16, device=dev)
+    call("f2b_mlp_bwd2", d_raw, mlp_in, None, None, sp16, 1, n, d_in16, torch.zeros_like(d_sp), stream())
+    ray_emb = emb.to(torch.int32).contiguous() if pt_emb is not None else None
+    call("f2b_shader_prep_bwd_f16", d_in16, d_logit, bounds, ray_emb, bounds.shape[0], float(inv_s), float(f_scale), dout,
+         None if d_app is None else torch.zeros_like(d_app), stream())
     din = torch.empty((n, 32), dtype=torch.float16, device=dev)
     dp = torch.zeros_like(d_fp)
     table = torch.zeros_like(d_table)

@@ -1,15 +1,31 @@
 #!/bin/bash
 # One GPU-box pass: parity tests, reference parity, sanitizer on the end-to-end step, bench.  Logs (small) -> $O (default ci_logs/).
+# Selections are files and node ids, not -k substrings (-k also matches "matches", "prefetched", "unfused" and module names).
+# The tensor-core and fused-kernel tests each run in a process of their own: a faulting kernel must not poison the other tests.
+P=tests/test_gpu_parity.py
+OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
+     "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
+     tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py)
+MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_bwd_fused.py
+      --ignore=tests/test_gpu_shade_fused.py)
+for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
+if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
+  echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_ref_parity.py
+  exit 0
+fi
 O=${O:-ci_logs}
 mkdir -p "$O"
 echo "== gpu: $(nvidia-smi -L) / nproc $(nproc)"
-timeout 900 python -m pytest tests -m gpu -q --deselect tests/test_ref_parity.py -p no:cacheprovider -k "not tc and not fused" > $O/pytest_gpu.log 2>&1
+timeout 1800 python -m pytest "${MAIN[@]}" -q -p no:cacheprovider > $O/pytest_gpu.log 2>&1
 tail -n 40 $O/pytest_gpu.log
-# tensor-core kernels in their own processes (a faulting kernel must not poison the other tests)
-for K in "tc-0" "tc-1" "fused" "tiles"; do
-  timeout 300 python -m pytest tests/test_gpu_parity.py -m gpu -q -p no:cacheprovider -k "$K" > $O/pytest_$K.log 2>&1
-  echo "--- -k $K"; tail -n 25 $O/pytest_$K.log | cut -c1-250
+for T in "${OWN[@]}"; do
+  L=${T##*/}; L=$O/pytest_${L//.py/}.log; L=${L//::/_}
+  timeout 600 python -m pytest "$T" -m gpu -q -p no:cacheprovider > "$L" 2>&1
+  echo "--- $T"; tail -n 25 "$L" | cut -c1-250
 done
+# the backward kernels against float64 / CPU-oracle references (multi-tile schedules, ~1 M-sample sizes)
+timeout 1200 python -m pytest tests/test_gpu_bwd_reference.py -m gpu -q -p no:cacheprovider --durations=10 > $O/pytest_bwd_reference.log 2>&1
+echo "--- tests/test_gpu_bwd_reference.py"; tail -n 40 $O/pytest_bwd_reference.log | cut -c1-250
 timeout 600 python -m pytest tests/test_ref_parity.py -m gpu -q -p no:cacheprovider > $O/pytest_ref.log 2>&1
 tail -n 60 $O/pytest_ref.log
 if [ "${SANITIZE:-0}" = "1" ]; then

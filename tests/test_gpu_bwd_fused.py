@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from conftest import make_rays
+from test_gpu_bwd_reference import ray_layout
 from test_gpu_parity import N, T, assert_close, sample_points
 from test_gpu_render import build
 
@@ -13,10 +14,12 @@ pytestmark = pytest.mark.gpu
 
 def segment(scene, oracle, hp, kind, n):
     """(pts [n,3], volume ids, stride): ray samples (consecutive samples share coarse cells: merged runs) with anchors [n,3]
-    (stride 3), or edge-like point pairs with a flat volume id (stride 1)."""
+    (stride 3), or edge-like point pairs with a flat volume id (stride 1).  Beyond the oracle-sampled rays' samples, synthetic rays."""
     if kind == "rays":
         s = sample_points(scene, oracle)
-        assert s["pts"].shape[0] >= n
+        if s["pts"].shape[0] < n:
+            pts, anchors, _ = ray_layout(n, hp["V"], np.random.default_rng(n))
+            return pts, anchors, 3
         return np.ascontiguousarray(s["pts"][:n]), np.ascontiguousarray(s["anchors"][:n]), 3
     rng = np.random.default_rng(n)
     a = rng.random((n // 2 + 1, 3), dtype=np.float32) * 2 - 1
@@ -27,7 +30,7 @@ def segment(scene, oracle, hp, kind, n):
 
 
 @pytest.mark.parametrize("kind,n", [("rays", 1), ("rays", 31), ("rays", 32), ("rays", 127), ("rays", 128), ("rays", 129),
-                                    ("rays", 5000), ("edges", 4099)])
+                                    ("rays", 5000), ("rays", 12 * 132 * 128 + 51), ("edges", 4099)])   # 12*132*128+51: 4-5 tiles per CTA
 def test_field_bwd_scatter_matches_unfused(scene, oracle, hash_params, kind, n):
     from f2nerf_b200 import ops
     from f2nerf_b200._lib import call, stream

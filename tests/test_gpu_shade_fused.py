@@ -19,7 +19,7 @@ def rays_of(n, rng):
 
 
 @pytest.mark.parametrize("emb", [False, True])
-@pytest.mark.parametrize("n", [1, 31, 32, 127, 128, 129, 5000])
+@pytest.mark.parametrize("n", [1, 31, 32, 127, 128, 129, 5000, 2 * 132 * 128 + 51])   # the last: CTAs with two and three tiles
 def test_shade_field_bwd_scatter_matches_unfused(scene, oracle, hash_params, n, emb):
     from f2nerf_b200 import ops
     from f2nerf_b200._lib import call, stream

@@ -7,7 +7,7 @@ this package is the thin host-side mirror of the reference's operator surface
 """
 from . import _lib  # noqa: F401  (fails loudly when the CUDA extension is missing)
 from .dataset import RayGenerator
-from .eval import RenderWholeImage
+from .eval import RenderAllImages, RenderPath, RenderWholeImage, TestImages
 from .field import Hash3DAnchored, TCNNWP
 from .ops import CustomOps, FlexOps
 from .optim import FusedAdam
@@ -15,5 +15,5 @@ from .renderer import Renderer, RenderResult, check_backward_nan
 from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultFlex
 from .shader import SHShader
 
-__all__ = ["FusedAdam", "RayGenerator", "RenderWholeImage", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
+__all__ = ["FusedAdam", "RayGenerator", "RenderWholeImage", "TestImages", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

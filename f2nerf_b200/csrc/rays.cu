@@ -5,6 +5,8 @@
 // Dataset::RandRaysData (src/Dataset/Dataset.cpp:290): with the images resident in HBM one small kernel each.
 // The fp32 operation order of the undistortion was read off the reference build's SASS (nvcc 12.9; ptxas
 // fuses further mul+sub pairs that the PTX still shows separately) and is spelled out with explicit roundings, so rays are bit-identical to the reference's (tests/test_ref_parity.py).
+// f2b_camera_rays is the whole-camera path of the evaluation modes (Dataset::RaysOfCamera / RaysFromPose), an ATen sequence in the
+// reference, in one kernel (tests/test_gpu_eval.py).
 #include "common.cuh"
 
 namespace f2b {
@@ -19,23 +21,20 @@ __device__ __forceinline__ void distort(const Dist& d, float u, float v, float u
   dv = ffma(ffma(v2, 2.f, r2), d.p1, ffma(v, radial, fmul(uv, d.two_p2)));
 }
 
-__global__ void __launch_bounds__(128)
-img2world_kernel(int n_rays, const float* __restrict__ poses, const float* __restrict__ intri,
-                 const float* __restrict__ dist_params, const int* __restrict__ cam_indices,
-                 const int* __restrict__ ij, float* __restrict__ rays_o, float* __restrict__ rays_d) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rays) return;
-  const int cam = __ldg(cam_indices + r);
-  const float pi = fadd((float)__ldg(ij + 2 * r), .5f), pj = fadd((float)__ldg(ij + 2 * r + 1), .5f);   // (ij + .5f), Dataset.cu:128
-  const float* K = intri + size_t(cam) * 9;
-  const float fx = __ldg(K), cx = __ldg(K + 2), fy = __ldg(K + 4), cy = __ldg(K + 5);
-  const float u0 = fdiv(fsub(pj, cx), fx), v0 = fdiv(fsub(pi, cy), fy);              // OpenCV style
-  const float* dp = dist_params + size_t(cam) * 4;
+__device__ __forceinline__ Dist load_dist(const float* dp) {
   Dist d;
   d.k1 = __ldg(dp); d.k2 = __ldg(dp + 1); d.p1 = __ldg(dp + 2); d.p2 = __ldg(dp + 3);
   d.two_p1 = fadd(d.p1, d.p1); d.two_p2 = fadd(d.p2, d.p2);
+  return d;
+}
+
+// iterative_camera_undistortion (Dataset.cu:30-69) on the OpenCV-style point (u0, v0).  It is inlined twice in the reference
+// build, into Img2WorldRayKernel and into CameraUndistortKernel (:71-76); ptxas schedules the two loops differently but makes
+// the same contractions (the same 140 FP instructions per iteration, FFMA for FFMA; only two FADD subtractions list their
+// operands the other way round), so one function serves both kernels.
+__device__ __forceinline__ void undistort(const Dist& d, const float u0, const float v0, float& u_out, float& v_out) {
   float u = u0, v = v0;
-  for (int it = 0; it < 100; it++) {                                                   // iterative_camera_undistortion
+  for (int it = 0; it < 100; it++) {
     const float s0 = fmaxf(fabsf(fmul(u, 1e-6f)), 1.1920929e-7f), s1 = fmaxf(fabsf(fmul(v, 1e-6f)), 1.1920929e-7f);
     const float u2 = fmul(u, u), uv = fmul(u, v), v2 = fmul(v, v);
     float du, dv, b0x, b0y, f0x, f0y, b1x, b1y, f1x, f1y;
@@ -54,12 +53,61 @@ img2world_kernel(int n_rays, const float* __restrict__ poses, const float* __res
     u = fsub(u, sx); v = fsub(v, sy);
     if (ffma(sx, sx, fmul(sy, sy)) < 1e-10f) break;                                   // squaredNorm() < kMaxStepNorm (NaN keeps iterating)
   }
+  u_out = u; v_out = v;
+}
+
+__global__ void __launch_bounds__(128)
+img2world_kernel(int n_rays, const float* __restrict__ poses, const float* __restrict__ intri,
+                 const float* __restrict__ dist_params, const int* __restrict__ cam_indices,
+                 const int* __restrict__ ij, float* __restrict__ rays_o, float* __restrict__ rays_d) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rays) return;
+  const int cam = __ldg(cam_indices + r);
+  const float pi = fadd((float)__ldg(ij + 2 * r), .5f), pj = fadd((float)__ldg(ij + 2 * r + 1), .5f);   // (ij + .5f), Dataset.cu:128
+  const float* K = intri + size_t(cam) * 9;
+  const float fx = __ldg(K), cx = __ldg(K + 2), fy = __ldg(K + 4), cy = __ldg(K + 5);
+  const float u0 = fdiv(fsub(pj, cx), fx), v0 = fdiv(fsub(pi, cy), fy);              // OpenCV style
+  float u, v;
+  undistort(load_dist(dist_params + size_t(cam) * 4), u0, v0, u, v);
   const float nv = -v;                                                                 // dir = (u, -v, -1), OpenGL style
   const float* P = poses + size_t(cam) * 12;
 #pragma unroll
   for (int k = 0; k < 3; k++) {
     rays_d[size_t(r) * 3 + k] = ffma(u, __ldg(P + 4 * k), ffma(nv, __ldg(P + 4 * k + 1), -__ldg(P + 4 * k + 2)));
     rays_o[size_t(r) * 3 + k] = __ldg(P + 4 * k + 3);
+  }
+}
+
+// ATen's CUDA linspace(0, end, n) (RangeFactories.cu) at index idx: two-sided, step = end / (n - 1) computed on the host in
+// fp32; the lower half is start + step*idx (exact to round(step*idx) with start 0, fused or not), the upper half
+// end - step*(n-1-idx), which nvcc contracts into one FFMA.
+__device__ __forceinline__ float linspace_at(float end, float step, int n, int idx) {
+  if (n == 1) return 0.f;
+  if (idx < n / 2) return fmul(step, (float)idx);
+  return ffma(-step, (float)(n - 1 - idx), end);
+}
+
+// Dataset::RaysOfCamera / RaysFromPose (Dataset.cpp:177-218) -> Img2WorldRay (:152-175): an out_h x out_w meshgrid of
+// linspace(0, height-1, out_h) x linspace(0, width-1, out_w) pixel rows/columns, + .5, ATen's division by the CPU scalars
+// fx / fy (a multiply by the host-rounded reciprocal, div_true_kernel_cuda), CameraUndistortKernel (Dataset.cu:71-95; its two
+// sign flips cancel exactly), and torch::matmul([1,3,3], [N,3,1]), whose cuBLAS kernel sums k = 0, 1, 2 in order.
+__global__ void __launch_bounds__(128)
+camera_rays_kernel(int out_h, int out_w, float end_i, float step_i, float end_j, float step_j, const float* __restrict__ pose,
+                   const float* __restrict__ intri, const float* __restrict__ dist_params, float* __restrict__ rays_o,
+                   float* __restrict__ rays_d) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= out_h * out_w) return;
+  const int a = r / out_w, b = r - a * out_w;
+  const float pi = fadd(linspace_at(end_i, step_i, out_h, a), .5f), pj = fadd(linspace_at(end_j, step_j, out_w, b), .5f);
+  const float fx = __ldg(intri), cx = __ldg(intri + 2), fy = __ldg(intri + 4), cy = __ldg(intri + 5);
+  const float u0 = fmul(fsub(pj, cx), frcp(fx)), v0 = fmul(fsub(pi, cy), frcp(fy));
+  float u, v;
+  undistort(load_dist(dist_params), u0, v0, u, v);
+  const float nv = -v;
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    rays_d[size_t(r) * 3 + k] = fsub(ffma(__ldg(pose + 4 * k + 1), nv, fmul(__ldg(pose + 4 * k), u)), __ldg(pose + 4 * k + 2));
+    rays_o[size_t(r) * 3 + k] = __ldg(pose + 4 * k + 3);
   }
 }
 
@@ -85,6 +133,21 @@ extern "C" int f2b_img2world_rays(const float* poses, const float* intri, const 
   img2world_kernel<<<div_up(n_rays, 128), 128, 0, as_stream(stream)>>>(n_rays, poses, intri, dist_params, cam_indices, ij,
                                                                       rays_o, rays_d);
   return check_launch("f2b_img2world_rays");
+}
+
+extern "C" int f2b_camera_rays(const float* pose, const float* intri, const float* dist_params, int height, int width,
+                               int out_h, int out_w, float* rays_o, float* rays_d, void* stream) {
+  F2B_REQUIRE(pose && intri && dist_params && rays_o && rays_d, "f2b_camera_rays: null pointer");
+  F2B_REQUIRE(out_h >= 1 && out_h <= height && out_w >= 1 && out_w <= width, "f2b_camera_rays: grid %dx%d outside image %dx%d",
+              out_h, out_w, height, width);
+  F2B_REQUIRE(int64_t(out_h) * out_w < (int64_t(1) << 31), "f2b_camera_rays: %d x %d rays overflow int32", out_h, out_w);
+  // torch::linspace(0.f, H - 1.f, n): end and step in fp32 on the host, exactly as ATen forms them
+  const float end_i = float(height) - 1.f, end_j = float(width) - 1.f;
+  const float step_i = out_h > 1 ? (end_i - 0.f) / float(out_h - 1) : 0.f, step_j = out_w > 1 ? (end_j - 0.f) / float(out_w - 1) : 0.f;
+  const int n = out_h * out_w;
+  camera_rays_kernel<<<div_up(n, 128), 128, 0, as_stream(stream)>>>(out_h, out_w, end_i, step_i, end_j, step_j, pose, intri,
+                                                                    dist_params, rays_o, rays_d);
+  return check_launch("f2b_camera_rays");
 }
 
 extern "C" int f2b_gather_pixels(const float* images, const int* cam_indices, const int* ij, int height, int width,

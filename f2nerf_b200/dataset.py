@@ -6,7 +6,8 @@ image tensor (50 x 540 x 960 x 3 fp32), copies three tensors host->device and la
 tables AND the images live in HBM; the index draws stay the same ``torch.randint`` calls on the same (CPU) generator in
 the same order — so a shared ``torch.manual_seed`` reproduces the reference's batch — and everything after the draws
 is two small kernels behind the C ABI (``f2b_img2world_rays``, ``f2b_gather_pixels``): one 48 KB host->device copy per
-batch instead of three plus a CPU gather.  Image loading, pose normalisation and the train/test split
+batch instead of three plus a CPU gather.  The whole-camera rays of the evaluation modes (``RaysOfCamera`` /
+``RaysFromPose``, Dataset.cpp:177-218) are one more kernel, ``f2b_camera_rays``.  Image loading, pose normalisation and the train/test split
 (``Dataset::Dataset``, Dataset.cpp:16-190) are out of scope: the tensors are handed in.
 """
 import torch
@@ -18,12 +19,15 @@ DATA_TRAIN_SET, DATA_TEST_SET, DATA_VAL_SET = 1, 2, 4           # Dataset.h
 
 class RayGenerator:
     def __init__(self, poses, intri, dist_params, bounds, images=None, height=None, width=None, train_set=None, val_set=(),
-                 test_set=(), device="cuda"):
+                 test_set=(), device="cuda", render_poses=None):
         """poses [n,3,4], intri [n,3,3], dist_params [n,4], bounds [n,2] (float32, as ``Dataset`` holds them);
-        images [n,H,W,3] float32 in [0,1] or None (then pass height/width and no colours are returned)."""
+        images [n,H,W,3] float32 in [0,1] or None (then pass height/width and no colours are returned);
+        render_poses [m,3,4] or None: the novel-view path ``RenderPath`` follows, normalised like ``Dataset::render_poses_``
+        (Dataset.cpp:58-70)."""
         dev = torch.device(device)
         f = lambda t: torch.as_tensor(t, dtype=torch.float32).to(dev).contiguous()
         self.poses_, self.intri_, self.dist_params_, self.bounds_ = f(poses), f(intri), f(dist_params), f(bounds)
+        self.render_poses_ = None if render_poses is None else f(render_poses).reshape(-1, 3, 4)
         self.n_images_ = self.poses_.shape[0]
         self.image_tensors_ = None if images is None else f(images)
         self.height_ = int(height if images is None else self.image_tensors_.shape[1])
@@ -64,3 +68,29 @@ class RayGenerator:
             call("f2b_gather_pixels", self.image_tensors_, cam_d, ij_d, self.height_, self.width_, batch_size, gt, stream())
         bounds = self.bounds_[cam_d.long()].contiguous()
         return (rays_o, rays_d, bounds), gt, cam_d
+
+    def _camera_rays(self, pose, intri, dist_params, out_h, out_w):
+        n = out_h * out_w
+        dev = self.poses_.device
+        rays_o = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        rays_d = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        call("f2b_camera_rays", pose, intri, dist_params, self.height_, self.width_, out_h, out_w, rays_o, rays_d, stream())
+        return rays_o, rays_d
+
+    def RaysOfCamera(self, idx, reso_level=1):
+        """Dataset::RaysOfCamera (Dataset.cpp:177-196) -> (rays_o, rays_d, bounds) [H*W,3|3|2] on the device, ray a*W + b
+        through pixel (a, b).  ``reso_level`` is ignored, as in the reference."""
+        idx = int(idx)
+        rays_o, rays_d = self._camera_rays(self.poses_[idx], self.intri_[idx], self.dist_params_[idx], self.height_, self.width_)
+        bounds = self.bounds_[idx].expand(rays_o.shape[0], 2).contiguous()
+        return rays_o, rays_d, bounds
+
+    def RaysFromPose(self, pose, reso_level=1):
+        """Dataset::RaysFromPose (Dataset.cpp:198-218): the (height // reso_level) x (width // reso_level) grid spread over
+        the full image, camera 0's intrinsics and distortion, the near / far bounds of all cameras (device reductions,
+        no host sync) -> (rays_o, rays_d, bounds) on the device."""
+        out_h, out_w = self.height_ // int(reso_level), self.width_ // int(reso_level)
+        pose = torch.as_tensor(pose, dtype=torch.float32).to(self.poses_.device).reshape(3, 4).contiguous()
+        rays_o, rays_d = self._camera_rays(pose, self.intri_[0], self.dist_params_[0], out_h, out_w)
+        near_far = torch.stack([self.bounds_[:, 0].min(), self.bounds_[:, 1].max()])
+        return rays_o, rays_d, near_far.expand(rays_o.shape[0], 2).contiguous()

@@ -278,6 +278,13 @@ int f2b_octree_mark_invisible(void* tree_nodes, int n_nodes, const float* intri,
 int f2b_img2world_rays(const float* poses, const float* intri, const float* dist_params, const int* cam_indices,
                        const int* ij, int n_rays, float* rays_o /* [n,3] */, float* rays_d /* [n,3], not normalised */,
                        void* stream);
+/* Whole-camera rays: Dataset::RaysOfCamera (out_h = height, out_w = width) and Dataset::RaysFromPose(pose, reso)
+ * (out_h = height / reso, out_w = width / reso) -> Img2WorldRay (src/Dataset/Dataset.cpp:152-218).  pose [3,4], intri [3,3],
+ * dist_params [4] of one camera; grid pixel (a, b) of linspace(0, height-1, out_h) x linspace(0, width-1, out_w) is ray
+ * a*out_w + b.  Bit-identical to the reference's ATen sequence (linspace, scalar division, CameraUndistortKernel, matmul).
+ * 1 <= out_h <= height, 1 <= out_w <= width, out_h*out_w < 2^31. */
+int f2b_camera_rays(const float* pose, const float* intri, const float* dist_params, int height, int width, int out_h,
+                    int out_w, float* rays_o /* [out_h*out_w,3] */, float* rays_d /* [out_h*out_w,3] */, void* stream);
 /* out[r] = images[cam_indices[r], ij[r,0], ij[r,1], 0:3]; images fp32 [n_img, height, width, 3] resident on the device. */
 int f2b_gather_pixels(const float* images, const int* cam_indices, const int* ij, int height, int width, int n,
                       float* out /* [n,3] */, void* stream);

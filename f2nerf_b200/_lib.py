@@ -96,6 +96,8 @@ SIGNATURES = {
     "f2b_render_fwd_fused": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_gather_kept_weights": [_P, _P, c_int, c_int, _P, _P],
 }
+TRACE_FN = ctypes.CFUNCTYPE(None, ctypes.c_char_p, c_int, c_void_p)      # f2b_trace_fn
+SIGNATURES["f2b_set_trace"] = [TRACE_FN]
 
 
 
@@ -179,6 +181,29 @@ KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_
                     "f2b_abi_version": 0, "f2b_get_mlp_impl": 0}
 LAUNCHES = 0      # running count of product kernels launched through this binding
 TRACE = None      # set to a list to record (name, start_event, end_event, int_args) per call (bench.py)
+# launch sequences traced per entry point inside them (f2b_set_trace) rather than as one call
+_SEQUENCES = ("f2b_render_phase1", "f2b_render_phase2_fwd", "f2b_render_bwd")
+
+
+def _call_traced_sequence(fn, conv):
+    """One launch sequence with the library's trace callback installed for this call only: an event pair on the library's
+    stream around every entry point the sequence calls, appended to TRACE under that entry point's name."""
+    begin = {}
+
+    def hook(name, end, s):
+        ev = torch.cuda.Event(enable_timing=True)
+        ev.record(torch.cuda.ExternalStream(s) if s else torch.cuda.default_stream())     # (ExternalStream(0): a pool stream)
+        if end:
+            TRACE.append((name.decode(), begin.pop(name), ev, []))
+        else:
+            begin[name] = ev
+
+    cb = TRACE_FN(hook)
+    lib.f2b_set_trace(cb)
+    try:
+        return fn(*conv)
+    finally:
+        lib.f2b_set_trace(TRACE_FN())                  # NULL
 
 
 def call(name, *args):
@@ -187,7 +212,9 @@ def call(name, *args):
     fn = getattr(lib, name)
     conv = [ptr(a) if isinstance(a, torch.Tensor) or a is None else (ctypes.byref(a) if isinstance(a, ctypes.Structure) else a)
             for a in args]
-    if TRACE is not None:
+    if TRACE is not None and name in _SEQUENCES:
+        rc = _call_traced_sequence(fn, conv)
+    elif TRACE is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         rc = fn(*conv)

@@ -224,28 +224,14 @@ def field_forward(field, table16, params16, points, anchors, anchor_stride, save
     return out, (feat16 if save_feat else None), hidden
 
 
-def field_forward_from_features(field, params16, feat16, save):
-    """MLP on already-encoded features (rows re-used from the early-stop pass): -> (out fp32 [n,16], hidden)."""
-    out32, _, hidden = ops.mlp_fwd_f32(feat16, params16, field.mlp_.n_hidden_matmuls, save_hidden=save)
-    return out32, hidden
-
-
-def field_backward(field, params16, points, anchors, anchor_stride, feat16, hidden, d_out_f32, d_out_f16=None, segments=None):
-    """dL/d out [n,16] (fp32, or already ``half(d * loss_scale)`` in ``d_out_f16``) ->
-    (dL/d feat_pool fp32 [pool,2], dL/d mlp params fp32).
-    ``segments``: optional list of (points, anchors, anchor_stride, first_row, n_rows) covering the rows of
-    ``feat16`` — the scatter then runs once per segment into the same table gradient, so callers holding the
-    query in pieces (ray samples + edge points) need not concatenate them."""
+def field_backward(field, params16, points, anchors, anchor_stride, feat16, hidden, d_out_f32):
+    """dL/d out [n,16] fp32 -> (dL/d feat_pool fp32 [pool,2], dL/d mlp params fp32)."""
     scale = field.mlp_.loss_scale_
-    d16 = d_out_f16 if d_out_f16 is not None else ops.cast_f32_to_f16(d_out_f32, scale)
+    d16 = ops.cast_f32_to_f16(d_out_f32, scale)
     dfeat16, dparams = ops.mlp_bwd(d16, feat16, hidden, params16, field.mlp_.n_hidden_matmuls, need_din=True)
     grad_table = torch.zeros_like(field.feat_pool_)
-    if segments is None:
-        segments = [(points, anchors, anchor_stride, 0, dfeat16.shape[0])]
-    for pts, anc, stride, first, rows in segments:
-        if rows > 0:
-            ops.hash_bwd(field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_, pts, anc, stride,
-                         dfeat16[first:first + rows], 1.0 / scale, grad_table)
+    ops.hash_bwd(field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_, points, anchors, anchor_stride, dfeat16,
+                 1.0 / scale, grad_table)
     dparams = dparams / scale
     return grad_table, dparams
 

@@ -3,8 +3,10 @@ through sampler -> field (no-grad early-stop pass) -> compaction -> field -> sha
 
 ``Renderer.Render`` returns the reference's ``RenderResult`` (Renderer.h:18-27) and is connected by
 ONE autograd node to the four leaves the trainer optimises (``feat_pool_``, the two ``mlp_.params_``,
-``app_emb_`` — ExpRunner.cpp:54,129-136); its backward is a fixed sequence of C-ABI kernels
-(composite bwd -> shader MLP bwd -> field MLP bwd -> hash scatter) instead of ~60 autograd nodes.
+``app_emb_`` — ExpRunner.cpp:54,129-136).  Forward and backward are the fixed launch sequences of
+csrc/render.cu (f2b_render_phase1 / _phase2_fwd / _bwd / _grad_finalize), one foreign call each, instead of
+~60 autograd nodes; a per-kernel trace (``TRACE`` in _lib.py) times every entry point inside them.  Only the
+shipped MLP shapes (field 32->64->16, shader 32->64->64->16) are supported.
 Host syncs per call: 2 (sample total, survivor total) against the reference's >= 11 ``.item()`` calls.
 """
 import os
@@ -15,9 +17,8 @@ import torch
 
 from . import _lib, ops
 from ._lib import call, stream
-from .field import field_backward, field_forward, field_forward_from_features
 from .rng import burn_mlp_output, burn_rand
-from .sampler import TRAIN, VALIDATE, LazySampleResult, SampleResultFlex
+from .sampler import TRAIN, LazySampleResult
 
 N_EDGE_PTS = 8192
 
@@ -75,6 +76,8 @@ class ForwardRenderResult:
 class Renderer:
     def __init__(self, global_data_pool, pts_sampler, scene_field, shader, n_images, use_app_emb=False,
                  bg_color="rand_noise", device="cuda"):
+        if scene_field.mlp_.n_hidden_matmuls != 0 or shader.mlp_.n_hidden_matmuls != 1:
+            raise NotImplementedError("Renderer: MLP shapes 32->64->16 / 32->64->64->16 only")
         self.global_data_pool_ = global_data_pool
         self.pts_sampler_, self.scene_field_, self.shader_ = pts_sampler, scene_field, shader
         self.use_app_emb_ = bool(use_app_emb)
@@ -100,126 +103,18 @@ class Renderer:
         n_rays = rays_o.shape[0]
         if self.global_data_pool_.mode_ != TRAIN and self._fused_forward_ok(n_rays):
             return self.render_forward(rays_o, rays_d)
-        if self._fused_launch_ok(n_rays):
-            return self._render_fused_launches(rays_o, rays_d, emb_idx)
-        return self._render_per_kernel(rays_o, rays_d, emb_idx)
-
-    def _render_per_kernel(self, rays_o, rays_d, emb_idx=None):
-        """Renderer::Render (Renderer.cpp:52-213) with one C-ABI call per kernel: the pipeline of ``_render_fused_launches`` for
-        per-kernel tracing (bench.py's breakdown) and for MLP depths the fused launch sequences do not cover."""
-        gdp = self.global_data_pool_
-        field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
-        n_rays, dev = rays_o.shape[0], rays_o.device
-        train = gdp.mode_ == TRAIN
-        # ---- phase 1: march -> early-stop field pass -> survivors, in the march's slot layout (no host sync) ----
-        pf = sampler.take_prefetched(rays_o, rays_d) if n_rays > 0 else None
-        if pf is not None:                                           # marched during the previous backward (prefetch_next)
-            slots = pf["slots"]
-            gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
-            gen.set_offset(gen.get_offset() + pf["noise_inc"])       # the noise draw happened ahead of time (same numbers)
-            torch.cuda.current_stream(dev).wait_event(pf["done"])
-        else:
-            slots = sampler.begin_march(rays_o, rays_d)              # draws the ray noise (RNG order: noise, bg, ...)
-        self.sample_result_ = LazySampleResult(slots)                # the reference-layout view, built only on access
-        bg = self._bg(n_rays, dev)
-        if n_rays <= 0:
-            z = torch.zeros
-            return RenderResult(bg, z((0, 1), device=dev), z((0,), device=dev), None, z((0,), device=dev), None, None)
-        S = slots.slot
-        with torch.no_grad():
-            table16 = field.table_f16()
-            fparams16 = field.mlp_.params_f16()
-            # the encoded features of ALL samples are kept: survivors re-use them in the gradient pass instead of
-            # gathering the table a second time (identical values: same points, same table)
-            logit_s = self._buf("logit", (n_rays * S,), torch.float32, dev)
-            feat_s = self._buf("feat", (n_rays * S, 32), torch.float16, dev)
-            weights0 = self._buf("w0", (n_rays * S,), torch.float32, dev)
-            alphas0 = self._buf("a0", (n_rays * S,), torch.float32, dev)
-            keep = self._buf("keep", (n_rays * S,), torch.uint8, dev)
-            kept_counts = self._buf("kept", (n_rays,), torch.int32, dev)
-            main = torch.cuda.current_stream(dev)
-            if pf is None:
-                sampler.march_rays(slots, 0, n_rays)
-            ops.field_fwd_slots(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_,
-                                fparams16, slots.s_pts[:n_rays * S], slots.s_anchors[:n_rays * S],
-                                slots.counts[:n_rays], n_rays, S, logit_s, feat_s)
-            ops.early_stop_rays(logit_s, 1, slots.s_dt, slots.slot_bounds[:n_rays], weights0, alphas0, keep, kept_counts)
-            new_bounds, total = ops.count_scan(kept_counts, n_rays)
-            vals = torch.cat([total] + [t.reshape(-1) for t in slots.totals]).tolist()      # THE host sync of the step
-            n_kept = int(vals[0])
-            n_all, n_all_oct = int(sum(vals[1::2])), int(sum(vals[2::2]))
-            sampler.note_totals(n_rays, n_all_oct)
-            slots.noted = True
-            self.n_sampled_pts_, self.n_kept_pts_ = n_all, n_kept     # host-side counts of this call (no extra sync)
-            if train:
-                gdp.sampled_pts_per_ray_ = gdp.sampled_pts_per_ray_ * .9 + (n_all / n_rays) * .1
-            if n_all <= 0:
-                if train:
-                    gdp.meaningful_sampled_pts_per_ray_ *= .9
-                z = torch.zeros
-                return RenderResult(bg, z((n_rays, 1), device=dev), z((n_rays,), device=dev), None,
-                                    torch.full((n_rays,), 512., device=dev), None, None)
-            burn_mlp_output(n_all, dev)                   # RNG parity: the reference's MLP output is a torch::rand (rng.py)
-            side = None
-            if train:
-                # octree occupancy votes only feed the NEXT iteration's march: run them beside the gradient pass
-                side = self._side_stream(dev, 1)
-                side.wait_stream(main)
-                with torch.cuda.stream(side):
-                    sampler.update_oct_nodes_raw(slots.slot_bounds, slots.s_anchors, weights0, alphas0)
-                gdp.meaningful_sampled_pts_per_ray_ = gdp.meaningful_sampled_pts_per_ray_ * .9 + (n_kept / n_rays) * .1
-            n_edge = 2 * N_EDGE_PTS if train else 0
-            feat_q = torch.empty((n_kept + n_edge, 32), dtype=torch.float16, device=dev)
-            f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
-            pts, dirs, dt, t = f32(n_kept, 3), f32(n_kept, 3), f32(n_kept), f32(n_kept)
-            anchors = torch.empty((n_kept, 3), dtype=torch.int32, device=dev)
-            ops.compact_slots(keep, slots.slot_bounds, new_bounds, slots.rays_d, slots.s_pts, slots.s_dt, slots.s_t,
-                              slots.s_anchors, feat_s, (pts, dirs, dt, t, anchors), feat_q)
-            es = SampleResultFlex(pts, dirs, dt, t, anchors, new_bounds, slots.first_oct_dis.clone())
-            if train:                                                                 # TV-loss edge points
-                edge_pts, edge_anchors = sampler.GetEdgeSamples(N_EDGE_PTS)
-                e_pts, e_anc = edge_pts.reshape(N_EDGE_PTS * 2, 3), edge_anchors.reshape(N_EDGE_PTS * 2)
-                e_pts, e_anc = e_pts.contiguous(), e_anc.contiguous()
-                feat_q[n_kept:] = ops.hash_fwd(table16, field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_,
-                                               e_pts, e_anc, 1)
-                segments = [(pts, anchors, 3, 0, n_kept), (e_pts, e_anc, 1, n_kept, n_edge)]
-            else:
-                segments = [(pts, anchors, 3, 0, n_kept)]
-            burn_mlp_output(n_kept + n_edge, dev)         # second AnchoredQuery (Renderer.cpp:165/172) ...
-            burn_mlp_output(n_kept, dev)                  # ... and the shader MLP (SHShader.cpp:27)
-            pt_emb_idx = ray_emb_idx = None
-            if train and self.use_app_emb_:
-                ray_emb_idx = emb_idx.to(torch.int32).contiguous()
-                pt_emb_idx = ops.scatter_idx(n_kept, new_bounds, ray_emb_idx)
-
-        grad_on = torch.is_grad_enabled() and train
-        args = (self, es, segments, None, pt_emb_idx, ray_emb_idx, bg, feat_q, n_kept, grad_on)
-        colors, disparity, depth, weights, edge_feats = _RenderFunction.apply(
-            field.feat_pool_, field.mlp_.params_, shader.mlp_.params_, self.app_emb_, *args)
-        if not train:
-            edge_feats = None
-        if side is not None:
-            torch.cuda.current_stream(dev).wait_stream(side)      # joined before weights0 / alphas0 can be recycled
-        return RenderResult(colors, es.first_oct_dis, disparity, edge_feats, depth, weights, new_bounds)
+        return self._render_fused_launches(rays_o, rays_d, emb_idx)
 
     # ------------------------------------------------------------------------------------------
-    def _fused_launch_ok(self, n_rays):
-        """One foreign call per phase (f2b_render_phase1 / _phase2_fwd / _bwd, csrc/render.cu) instead of one per kernel: the
-        default.  Per-kernel tracing (bench.py's breakdown) and other MLP depths take ``_render_per_kernel``."""
-        if n_rays <= 0 or _lib.TRACE is not None:
-            return False
-        return self.scene_field_.mlp_.n_hidden_matmuls == 0 and self.shader_.mlp_.n_hidden_matmuls == 1
-
     def _render_fused_launches(self, rays_o, rays_d, emb_idx):
-        """Renderer::Render (Renderer.cpp:52-213): identical kernels, order, streams and RNG draws as ``_render_per_kernel``,
-        issued through the three launch sequences of csrc/render.cu."""
+        """Renderer::Render (Renderer.cpp:52-213) through the three launch sequences of csrc/render.cu."""
         gdp = self.global_data_pool_
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
         train = gdp.mode_ == TRAIN
         main = torch.cuda.current_stream(dev)
         grad_on = torch.is_grad_enabled() and train                  # as the CALLER has it (everything up to the node is grad-free)
-        pf = sampler.take_prefetched(rays_o, rays_d)
+        pf = sampler.take_prefetched(rays_o, rays_d) if n_rays > 0 else None
         if pf is not None:                                           # marched during the previous backward (prefetch_next)
             slots = pf["slots"]
             gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
@@ -229,6 +124,9 @@ class Renderer:
             slots = sampler.begin_march(rays_o, rays_d)              # draws the ray noise (RNG order: noise, bg, ...)
         self.sample_result_ = LazySampleResult(slots)
         bg = self._bg(n_rays, dev)
+        if n_rays == 0:                                              # an empty batch (Renderer.cpp:83-97); a pending prefetch stays
+            z = torch.zeros
+            return RenderResult(bg, z((0, 1), device=dev), z((0,), device=dev), None, z((0,), device=dev), None, None)
         S = slots.slot
         with torch.no_grad():
             table16 = field.table_f16()
@@ -258,7 +156,7 @@ class Renderer:
                    first_oct_dis=slots.first_oct_dis, totals=heads[1:], logit_s=logit_s, feat_s=feat_s, w0=weights0, a0=alphas0,
                    keep=keep, kept_counts=kept_counts, new_bounds=new_bounds, total_kept=heads, stream=stream())
             if pf is not None:
-                heads[1:].copy_(slots.totals[0])                      # the prefetched march's own totals
+                heads[1:].copy_(slots.totals)                         # the prefetched march's own totals
             call("f2b_render_phase1", ra)
             if pf is not None:
                 _lib.LAUNCHES -= 3                                    # march (2 kernels) + slot bounds ran with the prefetch
@@ -310,7 +208,7 @@ class Renderer:
             n_kept, n_all, n_all_oct = heads.tolist()                 # THE host sync of the step
             sampler.note_totals(n_rays, n_all_oct)
             slots.noted = True
-            slots.totals = [heads[1:]]
+            slots.totals = heads[1:]
             self.n_sampled_pts_, self.n_kept_pts_ = n_all, n_kept
             if train:
                 gdp.sampled_pts_per_ray_ = gdp.sampled_pts_per_ray_ * .9 + (n_all / n_rays) * .1
@@ -352,10 +250,8 @@ class Renderer:
 
     def _fused_forward_ok(self, n_rays):
         """VALIDATE mode takes no gradient, no occupancy votes and no TV-loss edge points: march + ONE kernel
-        (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 (or per-kernel tracing / other MLP depths) keeps the operator pipeline."""
-        if n_rays <= 0 or _lib.TRACE is not None or os.environ.get("F2B_FUSED_FORWARD", "1") != "1":
-            return False
-        return self.scene_field_.mlp_.n_hidden_matmuls == 0 and self.shader_.mlp_.n_hidden_matmuls == 1
+        (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 keeps the operator pipeline (the launch sequences)."""
+        return n_rays > 0 and os.environ.get("F2B_FUSED_FORWARD", "1") == "1"
 
     def render_forward(self, rays_o, rays_d, out=None, lane=0):
         """Renderer::Render (Renderer.cpp:52-213) for a batch that takes no gradient (VALIDATE mode): the march, then hash encode
@@ -367,7 +263,7 @@ class Renderer:
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
         slots = sampler.begin_march(rays_o, rays_d, lane=lane)
-        sampler.march_rays(slots, 0, n_rays)
+        sampler.march_rays(slots)
         if lane == 0:
             self.sample_result_ = LazySampleResult(slots)
         bg = self._bg(n_rays, dev)
@@ -384,9 +280,9 @@ class Renderer:
             stamps[lane] = stamps.get(lane, 0) + 1
             call("f2b_render_fwd_fused", table16, field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_),
                  fparams16, sparams16, slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors, slots.counts, slots.rays_d, bg, n_rays, S,
-                 slots.totals[0], ticket, colors, disparity, depth, kept, w_slots, stream())
+                 slots.totals, ticket, colors, disparity, depth, kept, w_slots, stream())
         res = ForwardRenderResult(colors, slots.first_oct_dis, disparity, depth, kept, w_slots, S, self, (lane, stamps[lane]),
-                                  slots.totals[0])
+                                  slots.totals)
         res._keep = (slots, table16, fparams16, sparams16, bg, ticket)          # alive until the result dies (stream-ordered reuse)
         return res
 
@@ -561,184 +457,6 @@ class _FusedRenderFunction(torch.autograd.Function):
         renderer.nonfinite_flag_ = bad if prev is None else (prev | bad)
         ctx.keepalive = None                              # saved activations die with the backward, not with `res`
         return B["d_table"], B["d_fparams"], B["d_sparams"], B.get("d_app"), None, None, None, None
-
-
-class _RenderFunction(torch.autograd.Function):
-    """Second half of Renderer::Render (Renderer.cpp:152-208) with its whole backward."""
-
-    @staticmethod
-    def forward(ctx, feat_pool, field_params, shader_params, app_emb, renderer, es, q_pts, q_anchors, pt_emb_idx,
-                ray_emb_idx, bg, feat16, n_kept, grad_on):
-        field, shader = renderer.scene_field_, renderer.shader_
-        fparams16 = ops.cast_f32_to_f16(field_params)
-        sparams16 = ops.cast_f32_to_f16(shader_params)
-        dev = bg.device
-        n_q = feat16.shape[0]
-        emb = app_emb if pt_emb_idx is not None else None
-        if field.mlp_.n_hidden_matmuls == 0 and shader.mlp_.n_hidden_matmuls == 1:
-            # fused epilogues: field MLP -> [logit | shader-MLP input row], shader MLP -> [raw | rgb]; the fp32 scene_feat of the
-            # ray samples is never materialised (edge points still need all 16 channels).  No hidden activations are saved: the
-            # backward rebuilds them from the input rows (f2b_mlp_bwd2 with hidden0 == NULL), bit-identical
-            f_hidden = s_hidden = None
-            logit = torch.empty((n_kept,), dtype=torch.float32, device=dev)
-            mlp_in = torch.empty((n_kept, 32), dtype=torch.float16, device=dev)
-            call("f2b_field_shade_fwd", feat16, fparams16, es.dirs, emb, pt_emb_idx, n_kept, logit, mlp_in, None, stream())
-            if n_q > n_kept:
-                edge32 = torch.empty((n_q - n_kept, 16), dtype=torch.float32, device=dev)
-                call("f2b_mlp_fwd_f32", feat16[n_kept:], fparams16, 0, n_q - n_kept, edge32, None, None, stream())
-            else:
-                edge32 = torch.empty((0, 16), dtype=torch.float32, device=dev)
-            raw = torch.empty((n_kept, 16), dtype=torch.float16, device=dev)
-            rgb = torch.empty((n_kept, 3), dtype=torch.float32, device=dev)
-            call("f2b_shader_mlp_rgb_fwd", mlp_in, sparams16, n_kept, raw, rgb, None, stream())
-            logit_stride = 1
-        else:
-            scene_feat, f_hidden = field_forward_from_features(field, fparams16, feat16, save=grad_on)
-            mlp_in = ops.shader_prep(scene_feat[:n_kept], es.dirs, emb, pt_emb_idx) if n_kept > 0 else \
-                torch.empty((0, 32), dtype=torch.float16, device=bg.device)
-            raw, s_hidden = ops.mlp_fwd(mlp_in, sparams16, shader.mlp_.n_hidden_matmuls, save_hidden=grad_on)
-            rgb = ops.shader_act(raw)
-            logit, logit_stride, edge32 = scene_feat, 16, scene_feat[n_kept:]
-        colors, disparity, depth, weights = ops.composite_fwd(logit, logit_stride, rgb, es.dt, es.t, es.pts_idx_bounds, bg)
-        scene_feat = (logit, logit_stride)
-        edge_feats = edge32.reshape(-1, 2, 16)
-        ctx.renderer, ctx.es, ctx.n_kept = renderer, es, n_kept
-        ctx.pack = (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, pt_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw,
-                    s_hidden, rgb)
-        ctx.gs_progress = renderer.global_data_pool_.gradient_scaling_progress_
-        ctx.grad_on = grad_on
-        return colors, disparity, depth, weights, edge_feats
-
-    @staticmethod
-    def backward(ctx, d_colors, d_disp, d_depth, d_weights, d_edge):
-        renderer, es, n_kept = ctx.renderer, ctx.es, ctx.n_kept
-        field, shader, gdp = renderer.scene_field_, renderer.shader_, renderer.global_data_pool_
-        if ctx.pack is None:
-            raise RuntimeError("Renderer.Render backward: the saved activations were released by a previous backward "
-                               "(like tiny-cuda-nn's context, TCNNWP.cpp:207, the graph can be traversed once)")
-        (fparams16, sparams16, q_pts, q_anchors, ray_emb_idx, pt_emb_idx, bg, scene_feat, feat16, f_hidden, mlp_in, raw, s_hidden,
-         rgb) = ctx.pack
-        if not ctx.grad_on:
-            raise RuntimeError("Renderer.Render backward: forward ran without grad (VALIDATE mode / no_grad)")
-        segments = q_pts
-        n_q, dev = feat16.shape[0], feat16.device
-        n_rays = es.pts_idx_bounds.shape[0]
-        zeros = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
-        d_colors = d_colors.contiguous() if d_colors is not None else zeros(n_rays, 3)
-        d_disp = d_disp.contiguous() if d_disp is not None else None
-        d_depth = d_depth.contiguous() if d_depth is not None else None
-        d_weights = d_weights.contiguous() if d_weights is not None else None
-        if ctx.gs_progress < 1.:                          # GradientScaling::backward draws an unused rand_like (CustomOps.cu:154)
-            burn_rand(n_kept * 3, dev)
-            burn_rand(n_kept, dev)
-        # ---- backward: the dense chain (composite -> sigmoid -> shader MLP -> input assembly -> field MLP) on the main stream.
-        # With the default MLPs (field without, shader with one hidden matmul, activations not saved) everything behind the
-        # composite runs fused with the hash scatter (L2 reductions): f2b_shade_field_bwd_scatter for the ray samples,
-        # f2b_field_bwd_scatter for the edge points.  Otherwise the scatter runs on a side stream behind an event.
-        s_scale, f_scale = shader.mlp_.loss_scale_, field.mlp_.loss_scale_
-        nh_s, nh_f = shader.mlp_.n_hidden_matmuls, field.mlp_.n_hidden_matmuls
-        f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)
-        d_logit = torch.empty((n_kept,), dtype=torch.float32, device=dev)
-        d_raw = f16(n_kept, 16)
-        d_sparams, d_fparams = zeros(sparams16.numel()), zeros(fparams16.numel())
-        d_table = torch.zeros_like(field.feat_pool_)
-        d_app = torch.zeros_like(renderer.app_emb_) if ray_emb_idx is not None else None
-        main = torch.cuda.current_stream(dev)
-        side = renderer._side_stream(dev, 2)
-        bounds = es.pts_idx_bounds
-        hash_args = (field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_))
-
-        # Data parallel: ``grad_slab_hook_`` (f2nerf_b200.dist.install_grad_overlap) wants the table gradient slab by slab, so that
-        # the NCCL all-reduce of a finished slab runs while the lower level groups still scatter.  Level l only writes floats
-        # [l*S, (l+2)*S): the scatter then runs per level group, top-down, after the dense chain; the hook is called after each.
-        slab_hook = getattr(renderer, "grad_slab_hook_", None)
-        grad_mul = (1.0 / f_scale) * (getattr(renderer, "grad_premul_", 1.0) if slab_hook is not None else 1.0)
-        fused = slab_hook is None and nh_f == 0 and f_hidden is None
-        shade_fused = fused and nh_s == 1 and s_hidden is None
-        dfeat16 = None if fused else f16(n_q, 32)
-        # the ray samples' dL/dinput and dL/dout rows stay in shared memory when shade_fused: d_scene16 then holds the edge rows only
-        d_in16 = None if shade_fused else f16(n_kept, 32)
-        row0 = n_kept if shade_fused else 0              # d_scene16 row of sample `row0`
-        d_scene16 = f16(n_q - row0, 16)
-        if n_q > n_kept:
-            if d_edge is not None:
-                d_scene16[n_kept - row0:] = (d_edge.reshape(-1, 16) * f_scale).to(torch.float16)
-            else:
-                d_scene16[n_kept - row0:].zero_()
-        jobs = []
-
-        def field_bwd_scatter(pts, anc, stride, s0, s1):
-            call("f2b_field_bwd_scatter", d_scene16[s0 - row0:s1 - row0], feat16[s0:s1], fparams16, s1 - s0, pts, anc, int(stride), *hash_args,
-                 float(grad_mul), d_fparams, d_table, None, stream())
-
-        def scatter(pts, anc, stride, s0, s1):            # on the side stream, behind everything queued on main so far
-            if slab_hook is not None:
-                jobs.append((pts, anc, stride, s0, s1))
-                return
-            ev = torch.cuda.Event()
-            ev.record(main)
-            side.wait_event(ev)
-            with torch.cuda.stream(side):
-                ops.hash_bwd(*hash_args, pts, anc, stride, dfeat16[s0:s1], grad_mul, d_table)
-
-        if n_kept > 0:
-            # composite backward with the colour activation's backward applied on the way out (fp16 d_raw directly)
-            call("f2b_composite_act_bwd", scene_feat[0], int(scene_feat[1]), rgb, es.dt, es.t, bounds, bg, n_rays, d_colors, d_disp,
-                 d_depth, d_weights, float(ctx.gs_progress), raw, float(s_scale), d_logit, 1, d_raw, stream())
-        if n_kept > 0 and shade_fused:
-            pts, anc, stride = segments[0][:3]
-            call("f2b_shade_field_bwd_scatter", d_raw, mlp_in, sparams16, d_logit, pt_emb_idx, float(1.0 / s_scale), float(f_scale),
-                 feat16, fparams16, n_kept, pts, anc, int(stride), *hash_args, float(grad_mul), d_sparams, d_fparams, d_table, d_app,
-                 torch.empty((1,), dtype=torch.int32, device=dev), None, None, None, stream())
-        elif n_kept > 0:
-            call("f2b_mlp_bwd2", d_raw, mlp_in, None if s_hidden is None else s_hidden[0],
-                 s_hidden[1] if (nh_s and s_hidden is not None) else None, sparams16, int(nh_s), n_kept, d_in16, d_sparams, stream())
-            ops.shader_prep_bwd_f16(d_in16, d_logit, bounds, ray_emb_idx, 1.0 / s_scale, f_scale, d_scene16, d_app)
-            if fused:
-                field_bwd_scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
-            else:
-                call("f2b_mlp_bwd2", d_scene16[:n_kept], feat16[:n_kept], None if f_hidden is None else f_hidden[0, :n_kept],
-                     f_hidden[1, :n_kept] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), n_kept,
-                     dfeat16[:n_kept], d_fparams, stream())
-                scatter(segments[0][0], segments[0][1], segments[0][2], 0, n_kept)
-        for pts_e, anc_e, stride_e, first, rows in segments[1:]:          # TV-loss edge points: field MLP + scatter only
-            if rows > 0 and fused:
-                field_bwd_scatter(pts_e, anc_e, stride_e, first, first + rows)
-            elif rows > 0:
-                call("f2b_mlp_bwd2", d_scene16[first:first + rows], feat16[first:first + rows],
-                     None if f_hidden is None else f_hidden[0, first:first + rows],
-                     f_hidden[1, first:first + rows] if (nh_f and f_hidden is not None) else None, fparams16, int(nh_f), rows,
-                     dfeat16[first:first + rows], d_fparams, stream())
-                scatter(pts_e, anc_e, stride_e, first, first + rows)
-        if slab_hook is not None:
-            ev = torch.cuda.Event()
-            ev.record(main)
-            side.wait_event(ev)
-            with torch.cuda.stream(side):
-                for lo, nl in slab_groups():
-                    for pts_j, anc_j, stride_j, s0, s1 in jobs:
-                        call("f2b_hash_bwd_levels", *hash_args, pts_j, anc_j, int(stride_j), int(s1 - s0), dfeat16[s0:s1], 1, float(grad_mul),
-                             d_table, lo, nl, stream())
-                    slab_hook(d_table, lo, int(field.local_size_))          # issued on the side stream: NCCL orders itself behind it
-        main.wait_stream(side)
-        if slab_hook is not None:
-            renderer.grad_slab_finish_()                  # the main stream waits for the slab all-reduces: d_table leaves here averaged
-        d_sparams = d_sparams / s_scale
-        d_fparams = d_fparams / f_scale
-        # NaN back-off of TCNNWPFunction::backward (TCNNWP.cpp:231-240): the reference tests dL/dparams AND dL/dinput of
-        # each MLP.  The shader MLP's input gradient reaches d_app (and the field MLP's dL/dout), the field MLP's input
-        # gradient reaches every table-gradient entry its samples touch, so those stand in for the fp16 tensors
-        # themselves (a non-finite fp16 element cannot disappear on the way: w * inf / NaN stays non-finite).
-        live = min(d_table.shape[0], (17 * int(field.local_size_)) // 2)
-        ok_s = torch.isfinite(d_sparams).all()
-        if d_app is not None:
-            ok_s = ok_s & torch.isfinite(d_app).all()
-        ok_f = torch.isfinite(d_fparams).all() & torch.isfinite(d_table[:live]).all()
-        bad = torch.stack([~ok_s, ~ok_f])                          # [shader, field], device-side, no sync here
-        prev = getattr(renderer, "nonfinite_flag_", None)
-        renderer.nonfinite_flag_ = bad if prev is None else (prev | bad)      # OR: a second backward must not erase a hit
-        ctx.pack = None                               # saved activations (~1 GB at 4 M samples) die with the backward, not with `res`
-        return d_table, d_fparams, d_sparams, d_app, None, None, None, None, None, None, None, None, None, None
 
 
 def slab_groups():

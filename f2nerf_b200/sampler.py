@@ -48,10 +48,10 @@ class SlotSamples:
         dev = rays_o.device
         R = max(self.n_rays, 1)
         self.counts = torch.empty((R,), dtype=torch.int32, device=dev)
-        self.chunk_bounds = torch.empty((R, 2), dtype=torch.int32, device=dev)      # chunk-local cumsum (unused by the renderer)
+        self.chunk_bounds = torch.empty((R, 2), dtype=torch.int32, device=dev)      # the march's cumsum bounds (unused by the renderer)
         self.slot_bounds = torch.empty((self.n_rays, 2), dtype=torch.int32, device=dev)
         self.first_oct_dis = torch.empty((self.n_rays, 1), dtype=torch.float32, device=dev)
-        self.totals = []                                                            # one device [2] tensor per marched chunk
+        self.totals = torch.empty((2,), dtype=torch.int32, device=dev)              # [samples, octree hits], written by the march
 
 
 class LazySampleResult:
@@ -130,7 +130,7 @@ class PersSampler:
         """PersSampler::GetSamples (PersSampler.cu:317-434).  ``bounds_raw`` is ignored like in the
         reference (it marches [global_near_, 1e8]).  One host sync (sample total) instead of two."""
         slots = self.begin_march(rays_o_raw, rays_d_raw, rays_noise)
-        self.march_rays(slots, 0, slots.n_rays)
+        self.march_rays(slots)
         return self.materialize(slots)
 
     # ---- slot-layout pieces (used by Renderer.Render; GetSamples = begin_march + march_rays + materialize) ----------
@@ -148,20 +148,17 @@ class PersSampler:
         self._generation = getattr(self, "_generation", 0) + 1
         return SlotSamples(self, rays_o, rays_d, rays_noise, self._scratch(n_rays, rays_o.device), self._generation)
 
-    def march_rays(self, slots, r0, r1):
-        """March rays [r0, r1) into their slots on the CURRENT stream (no host sync)."""
-        n = r1 - r0
+    def march_rays(self, slots):
+        """March the batch into its slots on the CURRENT stream (no host sync)."""
+        n = slots.n_rays
         if n <= 0:
             return
-        S = slots.slot
-        totals = torch.empty((2,), dtype=torch.int32, device=slots.rays_o.device)
         call("f2b_sampler_march", self.tree_nodes_gpu_, self.n_nodes, self.pers_trans_gpu_, self.pers_trans_gpu_.numel() // 544,
-             slots.rays_o[r0:r1], slots.rays_d[r0:r1], slots.noise[r0:], n, float(self.global_near_), 1e8, float(self.sample_l_),
+             slots.rays_o, slots.rays_d, slots.noise, n, float(self.global_near_), 1e8, float(self.sample_l_),
              int(self.scale_by_dis_), int(self.max_oct_intersect_per_ray_), int(bool(self.exact_oct_stat_)),
-             slots.s_pts[r0 * S:r1 * S], slots.s_dt[r0 * S:r1 * S], slots.s_t[r0 * S:r1 * S], slots.s_anchors[r0 * S:r1 * S],
-             slots.counts[r0:r1], slots.chunk_bounds[r0:r1], totals, slots.first_oct_dis[r0:r1], stream())
-        call("f2b_slot_bounds", slots.counts[r0:r1], n, S, r0, slots.slot_bounds[r0:r1], stream())
-        slots.totals.append(totals)
+             slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors, slots.counts, slots.chunk_bounds, slots.totals,
+             slots.first_oct_dis, stream())
+        call("f2b_slot_bounds", slots.counts, n, slots.slot, 0, slots.slot_bounds, stream())
 
     # ---- software pipelining of the march (it reads no trainable state: only rays, noise and the octree) ------------------
     def prefetch_march(self, rays_o_raw, rays_d_raw, stream, pending_rand_numel=()):
@@ -192,11 +189,11 @@ class PersSampler:
         ev.record(main)                                            # the ray upload / noise draw queued so far precede the march (the
         stream.wait_event(ev)                                      # scratch it writes is the OTHER set: no reader to wait for)
         with torch.cuda.stream(stream):
-            self.march_rays(slots, 0, n_rays)
+            self.march_rays(slots)
             ring = self.__dict__.setdefault("_pinned_totals", [torch.empty((2,), dtype=torch.int32).pin_memory() for _ in range(4)])
             self._pinned_turn = (getattr(self, "_pinned_turn", -1) + 1) % len(ring)
             host_totals = ring[self._pinned_turn]
-            host_totals.copy_(slots.totals[0], non_blocking=True)      # [samples, octree hits] of the batch, on the host by the
+            host_totals.copy_(slots.totals, non_blocking=True)         # [samples, octree hits] of the batch, on the host by the
             done = torch.cuda.Event()                                  # time the consuming Render asks (it waits on `done`)
             done.record(stream)
         # no record_stream: every tensor the side stream touches stays referenced from the prefetch record / the slots until the
@@ -233,8 +230,7 @@ class PersSampler:
         bounds = torch.empty((R, 2), dtype=torch.int32, device=dev)
         total = torch.zeros((1,), dtype=torch.int32, device=dev)
         call("f2b_count_scan", slots.counts, R, bounds, total, stream())
-        vals = torch.cat([total] + [t.reshape(-1) for t in slots.totals]).tolist()          # the one sync
-        n_all_pts, n_all_oct = int(vals[0]), int(sum(vals[2::2]))
+        n_all_pts, _, n_all_oct = torch.cat([total, slots.totals]).tolist()              # the one sync
         if not getattr(slots, "noted", False):
             self.note_totals(R, n_all_oct)
             slots.noted = True

@@ -427,6 +427,11 @@ int f2b_render_phase1(const f2b_render* r);
 int f2b_render_phase2_fwd(const f2b_render* r);
 int f2b_render_bwd(const f2b_render* r);
 int f2b_render_grad_finalize(const f2b_render* r);
+/* Optional per-kernel trace of the four sequences above: fn(entry_point, 0, stream) right before and fn(entry_point, 1, stream)
+ * right after each entry point a sequence calls (its C-ABI name; f2b_render_grad_finalize reports its own kernels under its own
+ * name), on the host thread that issues the sequence.  NULL (the default) turns tracing off.  Process-wide, not thread-safe. */
+typedef void (*f2b_trace_fn)(const char* entry_point, int end, void* stream);
+int f2b_set_trace(f2b_trace_fn fn);
 
 /* ---- forward-only (VALIDATE / no-grad) Renderer::Render behind the march as ONE kernel --------------------------------
  * Replaces Renderer.cpp:107-208 for a batch that takes no gradient (ExpRunner::RenderWholeImage, ExpRunner.cpp:257-293):

@@ -3,10 +3,10 @@
 
   python scripts/bwd_probe.py [--out profiles/h100_bwd_probe.json] [--red-rate profiles/h100_red_rate.json] [--iters 60]
 
-Runs one TRAIN step through Renderer._render_per_kernel and keeps the inputs of the field-MLP backward + hash scatter of the
-ray samples (encoded features, fp16 field parameters, compacted points / anchors; the TV-loss edge segment is reported by size).
-That step runs the rays' shader backward fused into the same kernel (f2b_shade_field_bwd_scatter), so their field dL/dout rows
-are rebuilt here with the unfused kernels, f2b_mlp_bwd2 (shader) and f2b_shader_prep_bwd_f16.  Then times, with CUDA events (median of --iters launches after warm-up, table gradient zeroed before each):
+Runs the forward of one TRAIN step through Renderer.Render (capture_step) and keeps the inputs of the field-MLP backward + hash
+scatter of the ray samples (encoded features, fp16 field parameters, compacted points / anchors; the TV-loss edge segment is
+reported by size).  The step's backward runs the rays' shader backward fused into the same kernel (f2b_shade_field_bwd_scatter),
+so their field dL/dout rows are rebuilt here with the unfused kernels, f2b_mlp_bwd2 (shader) and f2b_shader_prep_bwd_f16.  Then times, with CUDA events (median of --iters launches after warm-up, table gradient zeroed before each):
   f2b_mlp_bwd2 (field, rays) | f2b_hash_bwd (rays) | the two in sequence | f2b_field_bwd_scatter (rays, the fused kernel).
 The reductions the scatter issues are counted on the host (numpy restatement of the cell key of corners() and of the run rule
 of scatter_level, hash.cuh), so the achieved lane-reduction rate can be set against the microbenchmark's v2f32 `spread` peak
@@ -51,6 +51,49 @@ def count_reductions(pts, vol, din, scales, bias, n_volumes):
     return total
 
 
+def capture_step(prob, rays_o, rays_d, emb, gt):
+    """The forward of one TRAIN step through Render with the argument block ``ra`` of the launch sequences and the tensors it points
+    to (``keepalive``) kept; dL/dcolors of the probes' loss from autograd, and from it dL/draw + dL/dlogit by one f2b_composite_act_bwd
+    call: the inputs of the backward behind the composite as f2b_render_bwd sees them.  -> dict with the tensors the probes read."""
+    import torch
+    from f2nerf_b200 import renderer as R
+    from f2nerf_b200._lib import call, stream
+    renderer, field, shader = prob["renderer"], prob["field"], prob["shader"]
+    seen = {}
+    real = R._FusedRenderFunction.forward
+
+    def keep(ctx, feat_pool, field_params, shader_params, app_emb, rnd, ra, keepalive, grad_on):
+        seen.update(ra=ra, keepalive=keepalive)
+        return real(ctx, feat_pool, field_params, shader_params, app_emb, rnd, ra, keepalive, grad_on)
+
+    R._FusedRenderFunction.forward = staticmethod(keep)
+    try:
+        res = renderer.Render(rays_o, rays_d, None, emb)
+    finally:
+        R._FusedRenderFunction.forward = staticmethod(real)
+    loss = torch.sqrt((res.colors - gt) ** 2 + 1e-4).mean() + ((res.edge_feats[:, 0] - res.edge_feats[:, 1]) ** 2).mean() * 1e-1
+    (d_colors,) = torch.autograd.grad(loss, res.colors)
+    ra, keepalive = seen["ra"], seen["keepalive"]
+    T, n = keepalive[-1], ra.n_kept
+    bounds, bg = keepalive[4], keepalive[6]
+    d_logit = torch.empty((n,), dtype=torch.float32, device=rays_o.device)
+    d_raw = torch.empty((n, 16), dtype=torch.float16, device=rays_o.device)
+    call("f2b_composite_act_bwd", T["logit"], 1, T["rgb"], T["dt"], T["t"], bounds, bg, ra.n_rays, d_colors.contiguous(), None, None,
+         None, float(renderer.global_data_pool_.gradient_scaling_progress_), T["raw"], float(shader.mlp_.loss_scale_), d_logit, 1,
+         d_raw, stream())
+    torch.cuda.synchronize()
+    f_scale = float(field.mlp_.loss_scale_)
+    pt_emb = T.get("pt_emb_idx")
+    return dict(slots=keepalive[0], bounds=bounds, d_raw=d_raw, d_logit=d_logit, mlp_in=T["mlp_in"][:n], sp16=keepalive[3],
+                fp16=keepalive[2], feat=T["feat_q"], pts=T["pts"][:n], anc=T["anchors"][:n], pt_emb=pt_emb, n=n, edge_rows=2 * ra.n_edge_pairs,
+                inv_s=1.0 / float(shader.mlp_.loss_scale_), f_scale=f_scale, grad_mul=1.0 / f_scale,
+                hash_args=(field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_)),
+                d_sp=torch.zeros(ra.n_shader_params, dtype=torch.float32, device=rays_o.device),
+                d_fp=torch.zeros(ra.n_field_params, dtype=torch.float32, device=rays_o.device),
+                d_table=torch.zeros_like(field.feat_pool_),
+                d_app=torch.zeros_like(renderer.app_emb_) if pt_emb is not None else None)
+
+
 def gpu_info():
     try:
         out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -69,7 +112,7 @@ def main():
     args = ap.parse_args()
     import torch
     import bench
-    from f2nerf_b200 import ops, renderer as R
+    from f2nerf_b200 import ops
     from f2nerf_b200._lib import call, stream
 
     dev = torch.device("cuda", 0)
@@ -78,30 +121,12 @@ def main():
     prob = bench.build_problem(0, 1, bargs, dev)
     o, d, cam, gt = prob["host"]
     rays_o, rays_d, emb, gt = (torch.from_numpy(a).to(dev) for a in (o, d, cam, gt))
-    kept = []
-    real_call = R.call
-
-    def spy(name, *a):                       # keep the inputs of the backward behind the composite, per segment
-        if name in ("f2b_shade_field_bwd_scatter", "f2b_field_bwd_scatter", "f2b_composite_act_bwd"):
-            kept.append([name] + [t.clone() if isinstance(t, torch.Tensor) else t for t in a])
-        return real_call(name, *a)
-
-    R.call = spy
-    try:
-        for p in (prob["field"].feat_pool_, prob["field"].mlp_.params_, prob["shader"].mlp_.params_, prob["renderer"].app_emb_):
-            p.grad = None
-        res = prob["renderer"]._render_per_kernel(rays_o, rays_d, emb)
-        loss = torch.sqrt((res.colors - gt) ** 2 + 1e-4).mean() + ((res.edge_feats[:, 0] - res.edge_feats[:, 1]) ** 2).mean() * 1e-1
-        loss.backward()
-        torch.cuda.synchronize()
-    finally:
-        R.call = real_call
-    names = [k[0] for k in kept]
-    assert names[:2] == ["f2b_composite_act_bwd", "f2b_shade_field_bwd_scatter"], names
-    bounds = kept[0][1 + 5]
-    (d_raw, mlp_in, sp16, d_logit, pt_emb, inv_s, f_scale, feat, fparams16, n, pts, anc, stride, prim, bias, n_vol, S, grad_mul,
-     d_sp, d_fp, d_table, d_app) = kept[1][1:23]
-    edge_rows = int(kept[2][1 + 3]) if len(kept) > 2 else 0
+    c = capture_step(prob, rays_o, rays_d, emb, gt)
+    bounds, d_raw, mlp_in, sp16, d_logit, pt_emb, inv_s, f_scale, feat, fparams16, n, pts, anc, grad_mul, d_sp, d_fp, d_table, d_app = (
+        c[k] for k in ("bounds", "d_raw", "mlp_in", "sp16", "d_logit", "pt_emb", "inv_s", "f_scale", "feat", "fp16", "n", "pts", "anc",
+                       "grad_mul", "d_sp", "d_fp", "d_table", "d_app"))
+    prim, bias, n_vol, S = c["hash_args"]
+    stride, edge_rows = 3, c["edge_rows"]
     d_in16 = torch.empty((n, 32), dtype=torch.float16, device=dev)
     dout = torch.empty((n, 16), dtype=torch.float16, device=dev)
     call("f2b_mlp_bwd2", d_raw, mlp_in, None, None, sp16, 1, n, d_in16, torch.zeros_like(d_sp), stream())

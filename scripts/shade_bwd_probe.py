@@ -4,9 +4,10 @@ sequence against f2b_shade_field_bwd_scatter, which runs them as one warp-specia
 
   python scripts/shade_bwd_probe.py [--out profiles/h100_shade_bwd_probe.json] [--red-rate profiles/h100_red_rate.json] [--iters 60]
 
-Runs one TRAIN step through Renderer._render_per_kernel and keeps the inputs of f2b_shade_field_bwd_scatter (shader dL/dout,
-shader input rows, d_logit, field input rows, both MLPs' fp16 parameters, points / anchors, camera indices) and of the step's
-f2b_sampler_march.  Then times, with CUDA events (median of --iters launches after warm-up, gradients zeroed before each):
+Runs the forward of one TRAIN step through Renderer.Render (bwd_probe.capture_step) and keeps the inputs of
+f2b_shade_field_bwd_scatter (shader dL/dout, shader input rows, d_logit, field input rows, both MLPs' fp16 parameters, points /
+anchors, camera indices) and of the step's f2b_sampler_march (the batch marched once more through PersSampler.march_rays).
+Then times, with CUDA events (median of --iters launches after warm-up, gradients zeroed before each):
   sequence  f2b_mlp_bwd2 (shader, recompute) -> f2b_shader_prep_bwd_f16 -> f2b_field_bwd_scatter, as the parent issued them;
   fused     f2b_shade_field_bwd_scatter alone;
   +march    the fused kernel with the march of a ray batch launched just before it on a second stream (as in training, where
@@ -34,8 +35,8 @@ def main():
     args = ap.parse_args()
     import torch
     import bench
-    from bwd_probe import count_reductions, gpu_info
-    from f2nerf_b200 import ops, renderer as R, sampler as SM
+    from bwd_probe import capture_step, count_reductions, gpu_info
+    from f2nerf_b200 import ops, sampler as SM
     from f2nerf_b200._lib import call, stream
 
     dev = torch.device("cuda", 0)
@@ -44,37 +45,33 @@ def main():
     prob = bench.build_problem(0, 1, bargs, dev)
     o, d, cam, gt = prob["host"]
     rays_o, rays_d, emb, gt = (torch.from_numpy(a).to(dev) for a in (o, d, cam, gt))
-    kept = {}
-    real_r, real_s = R.call, SM.call
-
-    def spy(real):
-        def f(name, *a):
-            if name in ("f2b_shade_field_bwd_scatter", "f2b_composite_act_bwd", "f2b_sampler_march") and name not in kept:
-                kept[name] = [t.clone() if isinstance(t, torch.Tensor) else t for t in a]
-            return real(name, *a)
-        return f
-
-    R.call, SM.call = spy(real_r), spy(real_s)
-    try:
-        for p in (prob["field"].feat_pool_, prob["field"].mlp_.params_, prob["shader"].mlp_.params_, prob["renderer"].app_emb_):
-            p.grad = None
-        res = prob["renderer"]._render_per_kernel(rays_o, rays_d, emb)
-        loss = torch.sqrt((res.colors - gt) ** 2 + 1e-4).mean() + ((res.edge_feats[:, 0] - res.edge_feats[:, 1]) ** 2).mean() * 1e-1
-        loss.backward()
-        torch.cuda.synchronize()
-    finally:
-        R.call, SM.call = real_r, real_s
-    assert "f2b_shade_field_bwd_scatter" in kept and "f2b_sampler_march" in kept, sorted(kept)
-    (d_raw, mlp_in, sp16, d_logit, pt_emb, inv_s, f_scale, feat, fp16_, n, pts, anc, stride, prim, bias, n_vol, S, grad_mul,
-     d_sp, d_fp, d_table, d_app, ticket, _, _, _, _) = kept["f2b_shade_field_bwd_scatter"]
-    bounds = kept["f2b_composite_act_bwd"][5]
+    c = capture_step(prob, rays_o, rays_d, emb, gt)
+    d_raw, mlp_in, sp16, d_logit, pt_emb, inv_s, f_scale, feat, fp16_, n, pts, anc, grad_mul, d_sp, d_fp, d_table, d_app, bounds = (
+        c[k] for k in ("d_raw", "mlp_in", "sp16", "d_logit", "pt_emb", "inv_s", "f_scale", "feat", "fp16", "n", "pts", "anc",
+                       "grad_mul", "d_sp", "d_fp", "d_table", "d_app", "bounds"))
+    stride = 3
+    ticket = torch.empty((1,), dtype=torch.int32, device=dev)
     n_rays = bounds.shape[0]
+    kept = {}
+    real_s = SM.call
+
+    def spy(name, *a):
+        if name == "f2b_sampler_march":
+            kept[name] = [t.clone() if isinstance(t, torch.Tensor) else t for t in a]
+        return real_s(name, *a)
+
+    SM.call = spy
+    try:
+        prob["renderer"].pts_sampler_.march_rays(c["slots"])
+    finally:
+        SM.call = real_s
     ray_emb = emb.to(torch.int32).contiguous() if pt_emb is not None else None
     f16 = lambda *s: torch.empty(s, dtype=torch.float16, device=dev)
     d_in16, d_scene16, dfeat16 = f16(n, 32), f16(n, 16), f16(n, 32)
     sp, fp, table = torch.zeros_like(d_sp), torch.zeros_like(d_fp), torch.zeros_like(d_table)
     app = torch.zeros_like(d_app) if d_app is not None else None
-    hash_args = (prim, bias, n_vol, S)
+    hash_args = c["hash_args"]
+    prim, bias, n_vol, S = hash_args
 
     def seq():
         call("f2b_mlp_bwd2", d_raw, mlp_in, None, None, sp16, 1, n, d_in16, sp, stream())

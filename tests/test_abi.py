@@ -71,3 +71,17 @@ def test_table_grad_buffer_reuse_rules():
     d = r._table_grad_buffer((32, 2), "cpu")                       # another shape: never a view of the old storage
     assert d.shape == (32, 2) and float(d.abs().sum()) == 0.0
     assert slab_groups() == ((12, 4), (8, 4), (4, 4), (0, 4))
+
+
+def test_renderer_refuses_other_mlp_depths():
+    """The launch sequences are built for the shipped field 32->64->16 and shader 32->64->64->16 only: a Renderer over other
+    depths is refused at construction (the stand-alone operators keep both depths)."""
+    import pytest
+    from f2nerf_b200 import GlobalDataPool, Hash3DAnchored, Renderer, SHShader
+    gdp = GlobalDataPool()
+    for field_layers, shader_layers in ((2, 2), (1, 1)):
+        field = Hash3DAnchored(gdp, log2_table_size=8, n_hidden_layers=field_layers, device="cpu")
+        shader = SHShader(gdp, n_hiddens=shader_layers, device="cpu")
+        with pytest.raises(NotImplementedError, match="MLP shapes"):
+            Renderer(gdp, None, field, shader, n_images=2, device="cpu")
+    Renderer(gdp, None, Hash3DAnchored(gdp, log2_table_size=8, device="cpu"), SHShader(gdp, device="cpu"), n_images=2, device="cpu")

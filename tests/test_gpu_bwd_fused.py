@@ -4,10 +4,8 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import make_rays
 from test_gpu_bwd_reference import ray_layout
 from test_gpu_parity import N, T, assert_close, sample_points
-from test_gpu_render import build
 
 pytestmark = pytest.mark.gpu
 
@@ -67,30 +65,3 @@ def test_field_bwd_scatter_matches_unfused(scene, oracle, hash_params, kind, n):
         np.testing.assert_allclose(N(table), N(table_ref), rtol=1e-5, atol=1e-6 * max(float(table_ref.abs().max()), 1e-30))
         assert float(table[(17 * S) // 2 + 1:].abs().max()) == 0.0
 
-
-def test_train_step_fused_launches_match_per_kernel(scene):
-    """A TRAIN step through Render (f2b_render_bwd) and through _render_per_kernel (one C-ABI call per kernel) both run the fused
-    field backward + scatter: the same forward bit for bit, the same gradients up to the order of the fp32 reductions."""
-    from f2nerf_b200 import TRAIN
-    o, d, dn, cam = make_rays(scene, 300, seed=5)
-    outs = []
-    for per_kernel in (False, True):
-        gdp, sampler, field, shader, renderer = build(scene)
-        gdp.mode_ = TRAIN
-        torch.manual_seed(7)
-        if per_kernel:
-            r = renderer._render_per_kernel(T(o), T(d), T(cam))
-        else:
-            assert renderer._fused_launch_ok(len(o))
-            r = renderer.Render(T(o), T(d), None, T(cam))
-        loss = (r.colors ** 2).mean() + r.disparity.mean() + 0.1 * ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean()
-        loss.backward()
-        assert r.edge_feats.shape[0] > 0
-        outs.append(dict(colors=N(r.colors), weights=N(r.weights), table=N(field.feat_pool_.grad), fmlp=N(field.mlp_.params_.grad),
-                         smlp=N(shader.mlp_.params_.grad), emb=N(renderer.app_emb_.grad)))
-    a, b = outs
-    for k in ("colors", "weights"):
-        np.testing.assert_array_equal(a[k], b[k])
-    assert float(np.abs(a["table"]).max()) > 0
-    for k in ("table", "fmlp", "smlp", "emb"):
-        assert_close(a[k], b[k], rtol=1e-4, atol_frac=1e-5, name=k)

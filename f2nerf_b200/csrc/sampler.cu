@@ -116,7 +116,10 @@ __device__ __forceinline__ bool next_hit(Dfs& s, const TreeNode* __restrict__ no
 
 // ---------------------------------------------------------------------------------------------------------
 // The march: two rays per warp, 16 lanes each (the march is latency bound: at 4 lanes/ray 4096 rays would be
-// only 512 warps on 528 SM sub-partitions).  Each step has two phases:
+// only 512 warps on 528 SM sub-partitions).  Measured on the headline batch (H100 SXM at 400 W, profiles/h100_march_probe.json):
+// 8 and 4 lanes per ray cut the static instructions per ray-step from ~76 to ~59 / ~44, but the march then takes
+// 1.36 / 1.80 ms instead of 1.15 ms alone and longer under the backward too, so 16 lanes stay.  What does help is a
+// shorter step: one store per lane and step, and the noise read issued before phase A (1.05 ms).  Each step has two phases:
 //   A  lane g < 12 evaluates perspective projection g: xz, 1/xz1, the Jacobian factors T0..T2 and the value V;
 //   B  the 4 x 12 block {T0,T1,T2,V} x projections is transposed through 192 B of shared memory and lane
 //      (r, c) = (g >> 2, g & 3) forms ONE of the 12 mixing sums S[r][c] = sum_i weight[r][i] * T_c[i] serially
@@ -128,6 +131,7 @@ __device__ __forceinline__ bool next_hit(Dfs& s, const TreeNode* __restrict__ no
 // Every lane advances t / walks the octree redundantly (private DFS stack in shared memory).
 constexpr int kL16 = 16;
 constexpr int kRaysPerBlock16 = 2;
+enum { kOutNone, kOutSv, kOutDt, kOutT, kOutTrans, kOutNode, kOutConst };   // what a lane stores per sample
 
 template <int MODE>   // 0: count only, 1: fill at pts_idx_bounds, 2: one pass into per-ray scratch slots of 1024 samples
 __global__ void __launch_bounds__(32, 1)
@@ -166,6 +170,28 @@ march16_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__
   if (MODE == 1) { out_base = bounds[ray * 2]; cap = bounds[ray * 2 + 1] - int(out_base); }
   else if (MODE == 2) out_base = size_t(ray) * F2B_MAX_SAMPLE_PER_RAY;
 
+  // Output of a step: every lane of the ray stores at most ONE 32-bit word, through one predicated store, instead of
+  // taking its own branch per output array.  Lanes (r, 3) hold pts[r]; the other lanes take dt, t, anchors and dirs.
+  int role = kOutNone, comp = 0, stride = 1;
+  unsigned* obase = nullptr;
+  unsigned cbits = 0;                                            // the value of a kOutConst lane
+  if (FILL) {
+    const int m = g < 12 ? (ocol == 3 ? -1 : 3 * (g >> 2) + ocol) : 9 + g - 12;
+    // m: -1 pts; 0 dt; 1 t; 2 anchors[0]; 3 anchors[1]; 4 anchors[2] (MODE 1); 5..7 dirs (MODE 1)
+    if (m < 0)       { role = kOutSv;    obase = reinterpret_cast<unsigned*>(o_pts); stride = 3; comp = orow; }
+    else if (m == 0) { role = kOutDt;    obase = reinterpret_cast<unsigned*>(o_dt); }
+    else if (m == 1) { role = kOutT;     obase = reinterpret_cast<unsigned*>(o_t); }
+    else if (m == 2) { role = kOutTrans; obase = reinterpret_cast<unsigned*>(o_anchors); stride = MODE == 1 ? 3 : 2; }
+    else if (m == 3) { role = kOutNode;  obase = reinterpret_cast<unsigned*>(o_anchors); stride = MODE == 1 ? 3 : 2; comp = 1; }
+    else if (MODE == 1 && m == 4) { role = kOutConst; obase = reinterpret_cast<unsigned*>(o_anchors); stride = 3; comp = 2; }
+    else if (MODE == 1 && m <= 7) {
+      role = kOutConst; obase = reinterpret_cast<unsigned*>(o_dirs); stride = 3; comp = m - 5;
+      cbits = __float_as_uint(comp == 0 ? d[0] : (comp == 1 ? d[1] : d[2]));
+    }
+    if (!active) role = kOutNone;
+  }
+  unsigned* const optr = obase ? obase + out_base * stride + comp : nullptr;
+
   Hit hit;
   hit.node = 0; hit.trans_idx = 0; hit.near = 0.f; hit.far = 0.f;
   bool have = next_hit(dfs, nodes, o, d, near0, far0, hit);
@@ -197,6 +223,7 @@ march16_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__
       rclip = fmaxf(fdiv(fsqrt(ffma(ex, ex, ffma(ey, ey, fmul(ez, ez)))), cd.w), 1.f);
       loaded_trans = cur_trans;
     }
+    const float nz = __ldg(noise + k);                         // issued first: its latency hides under phase A
     // ---- phase A: my projection -------------------------------------------------------------------
     const float X = ffma(t, d[0], o[0]), Y = ffma(t, d[1], o[1]), Z = ffma(t, d[2], o[2]);
     const float xz0 = fadd(ffma(X, pa[0], fmul(Y, pa[1])), ffma(Z, pa[2], pa[3]));
@@ -227,24 +254,19 @@ march16_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__
     const float p0 = __shfl_sync(0xffffffffu, pj, 0, 16), p1 = __shfl_sync(0xffffffffu, pj, 4, 16),
                 p2 = __shfl_sync(0xffffffffu, pj, 8, 16);
     const float den = fadd(fsqrt(ffma(p0, p0, ffma(p1, p1, fmul(p2, p2)))), 1e-6f);
-    float step = fdiv(fmul(sample_l, __ldg(noise + k)), den);
+    float step = fdiv(fmul(sample_l, nz), den);
     if (scale_by_dis) step = fmul(rclip, step);
 
     if (running) {
       if (!first) {
-        if (FILL && active) {
-          const size_t idx = out_base + k;
-          if (ocol == 3 && g < 12) {
-            o_pts[idx * 3 + orow] = Sv;                          // the warped point: S[0..2][3] live in lanes 3, 7, 11
-          } else if (g == 0) {
-            o_dt[idx] = fmul(step, den);
-            o_t[idx] = t;
-          } else if (g == 1) {
-            if (MODE == 1) { o_anchors[idx * 3] = cur_trans; o_anchors[idx * 3 + 1] = cur_node; o_anchors[idx * 3 + 2] = 0; }
-            else { o_anchors[idx * 2] = cur_trans; o_anchors[idx * 2 + 1] = cur_node; }
-          } else if (g == 2) {
-            if (MODE == 1) { o_dirs[idx * 3] = d[0]; o_dirs[idx * 3 + 1] = d[1]; o_dirs[idx * 3 + 2] = d[2]; }
-          }
+        if (FILL && role != kOutNone) {
+          unsigned v = cbits;
+          v = role == kOutSv ? __float_as_uint(Sv) : v;
+          v = role == kOutDt ? __float_as_uint(fmul(step, den)) : v;
+          v = role == kOutT ? __float_as_uint(t) : v;
+          v = role == kOutTrans ? unsigned(cur_trans) : v;
+          v = role == kOutNode ? unsigned(cur_node) : v;
+          optr[size_t(k) * stride] = v;
         }
         k++;
       }

@@ -78,6 +78,7 @@ SIGNATURES = {
     "f2b_img2world_rays": [_P, _P, _P, _P, _P, c_int, _P, _P, _P],
     "f2b_camera_rays": [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P],
     "f2b_gather_pixels": [_P, _P, _P, c_int, c_int, c_int, _P, _P],
+    "f2b_image_metrics": [_P, _P, c_int, c_int, _P, _P, _P, _P, _P],
     "f2b_adam_step": [_P, _P, _P, _P, c_i64, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                       ctypes.c_double, c_i64, _P, _P],
     "f2b_early_stop": [_P, c_int, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P],
@@ -178,7 +179,7 @@ def stream():
 # kernels launched per entry point (for bench.py's gpu_launches claim; memsets are not counted)
 KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_phase2_fwd": 10, "f2b_render_bwd": 6, "f2b_render_grad_finalize": 2,
                     "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_early_stop": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
-                    "f2b_abi_version": 0, "f2b_get_mlp_impl": 0}
+                    "f2b_abi_version": 0, "f2b_get_mlp_impl": 0, "f2b_image_metrics": 2}
 LAUNCHES = 0      # running count of product kernels launched through this binding
 TRACE = None      # set to a list to record (name, start_event, end_event, int_args) per call (bench.py)
 # launch sequences traced per entry point inside them (f2b_set_trace) rather than as one call

@@ -14,12 +14,19 @@ rows of the image; chunks alternate between two streams / scratch sets so a chun
 The evaluation modes keep everything on the device: rays from ``RayGenerator.RaysOfCamera`` / ``RaysFromPose``
 (``f2b_camera_rays``), images rendered back to back by the same tiled loop, and for ``TestImages`` the reference's
 quantisation and MSE as device tensor ops with one host sync for all PSNRs.  Image writing is left to the caller.
+
+``TestImages`` also scores every view the way the paper's numbers are computed, by the reference's evaluation script
+(scripts/eval.py): 8-bit PSNR and SSIM of the PNGs ``TestImages`` would write, in one kernel per view
+(``f2b_image_metrics``, csrc/metrics.cu); ``ImageMetrics`` scores any image pair the same way.  LPIPS is not computed.
 """
+import numpy as np
 import torch
 
+from ._lib import call, stream
 from .sampler import VALIDATE
 
 RAY_BATCH_SIZE = 8192          # ExpRunner.cpp:268
+_METRICS_WORK_BYTES = 16 * 1024   # F2B_METRICS_WORK_BYTES (include/f2nerf_b200.h)
 
 
 def _to_dev(x, dev):
@@ -111,17 +118,78 @@ def quantify(x):
     return (x.clip(0., 1.) * 255.).to(torch.uint8).to(torch.float32) / torch.full((), 255., dtype=torch.float32, device=x.device)
 
 
+def ssim_taps(filter_size=11, filter_sigma=1.5):
+    """rgb_ssim's 1D Gaussian blur filter (scripts/eval.py:41-45) by the same float64 numpy expression, so that the device never
+    evaluates ``exp`` for it: exp(-0.5 ((k - hw + shift) / sigma)^2) for k < filter_size, divided by its numpy sum."""
+    hw = filter_size // 2
+    shift = (2 * hw - filter_size + 1) / 2
+    filt = np.exp(-0.5 * ((np.arange(filter_size) - hw + shift) / filter_sigma) ** 2)
+    return filt / np.sum(filt)
+
+
+SSIM_TAPS = ssim_taps()        # host memory; f2b_image_metrics reads it during each call
+
+
+def psnr_8bit(sse, n_values):
+    """skimage's peak_signal_noise_ratio on two uint8 images (scripts/eval.py:98): data range 255 (the dtype's), MSE the float64
+    mean of the squared differences, 10 log10(255^2 / MSE); ``inf`` for equal images, as skimage gives.  ``sse`` is the exact
+    integer sum, so the MSE is the one numpy forms."""
+    if sse == 0:
+        return float("inf")
+    return float(10. * np.log10(65025. / (np.float64(sse) / np.float64(n_values))))
+
+
+def _image_metrics(pred, gt):
+    """f2b_image_metrics on one contiguous [H,W,3] fp32 pair on the current device -> device tensors (sse int64 [1], ssim_sum
+    float64 [1]).  No host sync."""
+    sse = torch.empty((1,), dtype=torch.int64, device=pred.device)
+    ssim_sum = torch.empty((1,), dtype=torch.float64, device=pred.device)
+    work = torch.empty((_METRICS_WORK_BYTES,), dtype=torch.uint8, device=pred.device)
+    call("f2b_image_metrics", pred, gt, pred.shape[0], pred.shape[1], SSIM_TAPS.ctypes.data, work, sse, ssim_sum, stream())
+    return sse, ssim_sum
+
+
+def _ssim_count(H, W):
+    return (H - 10) * (W - 10) * 3                               # the 'valid' convolution's outputs, all channels
+
+
+@torch.no_grad()
+def ImageMetrics(pred, gt):
+    """The PSNR and SSIM of the reference's evaluation script (scripts/eval.py:94-100) for one image pair, on the device ->
+    {"psnr_8bit": float, "ssim": float}.  ``pred`` and ``gt`` are [H,W,3] CUDA tensors with values in [0,1] and H, W >= 11
+    (smaller images raise F2BError).  Both are scored as the 8-bit images the script reads:
+    - pred as ``TestImages`` writes it (Utils::WriteImageTensor, ImageIO.cpp:28-32): trunc(clip(x,0,1) * 255).  Raw and
+      ``quantify``-ed colours give the same bytes.
+    - gt as rint(clip(x,0,1) * 255), the stored byte of an image loaded as u8 / 255.
+    PSNR is skimage's peak_signal_noise_ratio (``psnr_8bit``).  SSIM is rgb_ssim(gt / 255., pred / 255., max_val=1) (:29-75) in
+    float64: separable 11-tap Gaussian (sigma 1.5, ``ssim_taps``), 'valid' convolution, k1 = 0.01, k2 = 0.03, variances clipped
+    at 0, covariance clipped to +-sqrt(var0 var1), mean over the three channels.  LPIPS is not computed."""
+    for name, t in (("pred", pred), ("gt", gt)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dim() != 3 or t.shape[2] != 3:
+            raise ValueError(f"ImageMetrics: {name} must be a [H,W,3] CUDA tensor")
+    if pred.shape != gt.shape or pred.device != gt.device:
+        raise ValueError(f"ImageMetrics: pred {tuple(pred.shape)} on {pred.device} and gt {tuple(gt.shape)} on {gt.device} differ")
+    H, W = pred.shape[0], pred.shape[1]
+    with torch.cuda.device(pred.device):
+        sse, ssim_sum = _image_metrics(pred.to(torch.float32).contiguous(), gt.to(torch.float32).contiguous())
+        sse, ssim_sum = torch.cat([sse.double(), ssim_sum]).tolist()
+    return {"psnr_8bit": psnr_8bit(int(sse), H * W * 3), "ssim": ssim_sum / _ssim_count(H, W)}
+
+
 @torch.no_grad()
 def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
     """ExpRunner::TestImages (ExpRunner.cpp:343-391) on ``dataset.test_set_`` ->
-    {"psnr": {idx: float}, "mean_psnr": float, "colors": [[H,W,3]], "disparity": [[H,W,1]], "first_oct_dis": [[H,W,1]]}
+    {"psnr": {idx: float}, "mean_psnr": float, "colors": [[H,W,3]], "disparity": [[H,W,1]], "first_oct_dis": [[H,W,1]],
+     "psnr_8bit": {idx: float}, "mean_psnr_8bit": float, "ssim": {idx: float}, "mean_ssim": float}
     (device tensors, colours quantised like the reference's PNGs).  The MSE against ``dataset.image_tensors_`` is
-    accumulated in float64 on the device and PSNR = 20 log10(1 / sqrt(mse)) (:369); the test images render back to back and
-    all PSNRs come to the host in one copy at the end."""
+    accumulated in float64 on the device and PSNR = 20 log10(1 / sqrt(mse)) (:369).  "psnr_8bit" and "ssim" are what the
+    reference's evaluation script reports for the written PNGs (``ImageMetrics``, scripts/eval.py:94-100), computed from the
+    quantised colours behind each view's render.  The test images render back to back and all values come to the host in one
+    copy at the end."""
     dev = _device_of(renderer, device)
     H, W = dataset.height_, dataset.width_
     out = {"colors": [], "disparity": [], "first_oct_dis": []}
-    psnrs = []
+    psnrs, scores = [], []
     with _Validate(renderer):
         for idx in dataset.test_set_:
             rays_o, rays_d, _ = dataset.RaysOfCamera(idx)
@@ -130,12 +198,19 @@ def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
             gt = dataset.image_tensors_[idx].reshape(H, W, 3)
             mse = (q.double() - gt.double()).square().mean()
             psnrs.append(20. * torch.log10(1. / torch.sqrt(mse)))
+            sse, ssim_sum = _image_metrics(q, gt.contiguous())
+            scores.append(torch.cat([sse.double(), ssim_sum]))          # SSE < 2^53: exact in float64
             out["colors"].append(q)
             out["disparity"].append(disp.reshape(H, W, 1))
             out["first_oct_dis"].append(first.reshape(H, W, 1))
-    vals = torch.stack(psnrs).tolist() if psnrs else []          # the one host sync
+    rows = torch.cat([torch.stack(psnrs)[:, None], torch.stack(scores)], 1).tolist() if psnrs else []   # the one host sync
+    vals = [r[0] for r in rows]
     out["psnr"] = {int(i): float(v) for i, v in zip(dataset.test_set_, vals)}
     out["mean_psnr"] = sum(vals) / len(vals) if vals else float("nan")
+    out["psnr_8bit"] = {int(i): psnr_8bit(int(r[1]), H * W * 3) for i, r in zip(dataset.test_set_, rows)}
+    out["ssim"] = {int(i): r[2] / _ssim_count(H, W) for i, r in zip(dataset.test_set_, rows)}
+    for k in ("psnr_8bit", "ssim"):
+        out["mean_" + k] = sum(out[k].values()) / len(rows) if rows else float("nan")
     return out
 
 

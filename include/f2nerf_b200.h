@@ -290,6 +290,21 @@ int f2b_gather_pixels(const float* images, const int* cam_indices, const int* ij
                       float* out /* [n,3] */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Image metrics of the reference's evaluation script (scripts/eval.py), which scores the 8-bit PNGs of ExpRunner::TestImages
+ * (ExpRunner.cpp:343-391, Utils::WriteImageTensor, ImageIO.cpp:28-32) with skimage's peak_signal_noise_ratio and rgb_ssim.
+ * pred, gt: one [height, width, 3] fp32 image pair on the device, height, width >= 11.  The 8-bit images are
+ * trunc(clip(pred, 0, 1) * 255) (the writer's cast, which gives quantify's levels back) and rint(clip(gt, 0, 1) * 255) (the
+ * stored byte of a ground truth loaded as u8 / 255.f).  Outputs (device): sse [1] = the sum of squared byte differences over all
+ * height*width*3 values, exact; ssim_sum [1] = the float64 sum of rgb_ssim's map over the (height-10) x (width-10) x 3 valid
+ * region.  taps_host: the 11 normalised Gaussian taps (sigma 1.5) in host memory, read during the call.  work:
+ * F2B_METRICS_WORK_BYTES of 8-byte aligned device scratch.  The reduction order is fixed: the same bits on every run.
+ * ------------------------------------------------------------------------------------------ */
+#define F2B_METRICS_BLOCKS     1024
+#define F2B_METRICS_WORK_BYTES (16 * F2B_METRICS_BLOCKS)
+int f2b_image_metrics(const float* pred, const float* gt, int height, int width, const double* taps_host, void* work,
+                      int64_t* sse, double* ssim_sum, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimizer step (SURVEY §8f N1) — replaces torch::optim::Adam::step for one parameter tensor
  * (built at src/ExpRunner.cpp:54 from Hash3DAnchored::OptimParamGroups, src/Field/Hash3DAnchored.cpp:124-150;
  * stepped at ExpRunner.cpp:136) and, when shadow_f16 != NULL, the fp32->fp16 table copy of the next forward

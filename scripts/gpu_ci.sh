@@ -2,12 +2,13 @@
 # One GPU-box pass: parity tests, reference parity, sanitizer on the end-to-end step, bench.  Logs (small) -> $O (default ci_logs/).
 # Selections are files and node ids, not -k substrings (-k also matches "matches", "prefetched", "unfused" and module names).
 # The tensor-core and fused-kernel tests each run in a process of their own: a faulting kernel must not poison the other tests.
+# So does the trained-checkpoint module (tests/test_gpu_checkpoint.py): it trains ngp_fox with the reference program once.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
      "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
-     tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py)
+     tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
-      --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py)
+      --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py

@@ -4,11 +4,13 @@
 #   reference arm   oracle/_ref/ref_driver      --train   (Totoro97/f2-nerf + tiny-cuda-nn, nothing replaced)
 #   b200 arm        oracle/_ref/ref_driver_b200 --train   (same program, Renderer::Render = f2nerf_b200/shim/B200Renderer.cpp)
 # usage: scripts/train_psnr.sh [end_iter=20000]      -> gpurun_out/train_psnr.json + the two logs
+# ARMS="ref" or ARMS="b200" trains one arm only.  Each arm leaves its experiment directory (checkpoints/latest, test_images)
+# in /tmp/f2b_train_<arm> and its config in /tmp/f2b_train_<arm>.yaml; scripts/eval_trained.py evaluates them on the device.
 set -u
 cd "$(dirname "$0")/.."
 END=${1:-20000}
 mkdir -p gpurun_out
-for arm in ref b200; do
+for arm in ${ARMS:-ref b200}; do
   exp=/tmp/f2b_train_$arm
   rm -rf $exp
   sed -e "s|^base_exp_dir: .*|base_exp_dir: $exp|" -e "s|^  end_iter: .*|  end_iter: $END|" oracle/ref_config_ngp_fox.yaml > /tmp/f2b_train_$arm.yaml
@@ -23,7 +25,10 @@ python - "$END" <<'PY'
 import json, re, sys
 out = {"end_iter": int(sys.argv[1]), "config": "oracle/ref_config_ngp_fox.yaml (confs/wanjinyou.yaml flattened), ngp_fox factor 2, 7 test images"}
 for arm in ("ref", "b200"):
-    log = open(f"gpurun_out/train_{arm}.log", errors="ignore").read()
+    try:
+        log = open(f"gpurun_out/train_{arm}.log", errors="ignore").read()
+    except FileNotFoundError:                                   # an arm left out through ARMS
+        continue
     it = re.findall(r"Iter:\s+(\d+) PSNR: ([\d.]+) NRays:\s+(\d+) OctSamples: ([\d.]+) Samples: ([\d.]+) MeaningfulSamples: ([\d.]+) IPS: ([\d.]+)", log)
     mean = re.findall(r"Mean psnr: ([\d.]+)", log)
     rc = re.findall(r"rc=(\d+) wall_s=([\d.]+)", log)

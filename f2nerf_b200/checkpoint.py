@@ -8,9 +8,12 @@ describe, loaded for evaluation on the device.
 ``load_scene`` rebuilds what ``ExpRunner``'s constructor + ``LoadCheckpoint`` build (ExpRunner.cpp:17-62,188-201) from the
 flat ``runtime_config.yaml`` the reference program reads: the data directory (``dataset.load_dataset``), ``PersSampler``,
 ``Hash3DAnchored``, ``SHShader`` and ``Renderer`` with the checkpoint's states, and the ray-march fineness of the saved
-iteration.  The result renders and evaluates (``eval.TestImages`` / ``RenderPath`` / ``RenderAllImages``).  It does not train:
-the reference's checkpoint holds no edge pool (``PersSampler::States``, PersSampler.cpp:692-701) and the octree is not rebuilt
-here, so a TRAIN-mode ``Renderer.Render`` on a loaded scene raises (empty edge pool) before it draws the TV-loss points.
+iteration.  The result renders and evaluates (``eval.TestImages`` / ``RenderPath`` / ``RenderAllImages``).
+
+By default it does not train: the reference's checkpoint holds no edge pool (``PersSampler::States``, PersSampler.cpp:692-701),
+so a TRAIN-mode ``Renderer.Render`` on a loaded scene raises (empty edge pool) before it draws the TV-loss points.
+``load_scene(..., trainable=True)`` restores what the reference resumes with instead: the edge pool of the initial octree,
+rebuilt from the training cameras (``octree_build``), and the saved iteration's gradient-scaling progress.
 """
 import ctypes
 import ctypes.util
@@ -68,6 +71,17 @@ def ray_march_fineness(iter_step, init_fineness, decay_end_iter):
     return float(_libm.expf(float(x)))
 
 
+def gradient_scaling_progress(iter_step, start, end):
+    """``ExpRunner::UpdateAdaParams``' gradient-scaling progress (ExpRunner.cpp:245-253): max(0, (float(iter) - start) /
+    (end - start + 1e-9f)) in float arithmetic, 1 at or past ``end``.  The TRAIN backward scales the hash-grid gradients
+    of near samples by it (GradientScaling), so a resumed run has to start from the saved iteration's value."""
+    if iter_step >= end:
+        return 1.0
+    f32 = np.float32
+    start, end = int(start), int(end)
+    return float(max(f32(0.), (f32(iter_step) - f32(start)) / (f32(end - start) + f32(1e-9))))
+
+
 class Scene(NamedTuple):
     global_data_pool: GlobalDataPool
     renderer: Renderer
@@ -117,7 +131,29 @@ def check_states(states, cfg, n_images, path="renderer.pt"):
            f"the image count of dataset.data_path = {cfg['dataset']['data_path']} ({n_images} cameras)")
 
 
-def load_scene(config_path, checkpoint_dir=None, device="cuda"):
+def check_initial_octree(tree_nodes, pers_trans, cfg, path="renderer.pt"):
+    """The rebuilt initial octree (TREE_NODE records) against the checkpoint's warps (``pers_trans`` bytes): one valid leaf
+    per warp, and every valid leaf's centre equal, bit for bit, to ``TransInfo.center`` of its ``trans_idx``.  ValueError
+    naming the ``pts_sampler`` keys and the data directory the structure was built from otherwise."""
+    pc, data = cfg["pts_sampler"], cfg["dataset"]["data_path"]
+    built_from = (f"pts_sampler.bbox_levels = {pc['bbox_levels']} / max_level = {pc['max_level']} / split_dist_thres = "
+                  f"{pc['split_dist_thres']} over the training cameras of dataset.data_path = {data}")
+    trans = np.ascontiguousarray(pers_trans).view(np.uint8).reshape(-1, 544)
+    V = trans.shape[0]
+    leaves = tree_nodes[tree_nodes["trans_idx"] >= 0]
+    if len(leaves) != V:
+        raise ValueError(f"{path}: the checkpoint has {V} warps, but the initial octree of {built_from} has {len(leaves)} "
+                         "valid leaves")
+    want = trans[:, 528:540].copy().view(np.uint32)                              # TransInfo.center
+    got = leaves["center"].view(np.uint32)[np.argsort(leaves["trans_idx"])]
+    bad = np.nonzero((want != got).any(-1))[0]
+    if len(bad):
+        raise ValueError(f"{path}: warp {int(bad[0])} is centred at {want[bad[0]].view(np.float32).tolist()}, but the "
+                         f"initial octree of {built_from} puts that leaf at {got[bad[0]].view(np.float32).tolist()} "
+                         f"({len(bad)} of {V} warps differ)")
+
+
+def load_scene(config_path, checkpoint_dir=None, device="cuda", trainable=False):
     """A trained scene from the reference's ``runtime_config.yaml`` and a checkpoint directory (default
     ``<base_exp_dir>/checkpoints/latest``) -> ``Scene(global_data_pool, renderer, dataset, iter_step)``.
 
@@ -128,7 +164,12 @@ def load_scene(config_path, checkpoint_dir=None, device="cuda"):
     checkpoint's primes and biases (no prime draws).  The global data pool is left in VALIDATE mode at the saved iteration's
     ray-march fineness, which is what ``ExpRunner::TestImages`` renders with after training.
 
-    Evaluation only: the checkpoint holds no edge pool, so a TRAIN-mode ``Render`` raises (empty edge pool)."""
+    ``trainable=False``: evaluation only.  The checkpoint holds no edge pool, so a TRAIN-mode ``Render`` raises (empty edge
+    pool).  ``trainable=True``: what the reference's ``is_continue: true`` resumes with (ExpRunner.cpp:56-58).  The edge pool
+    of the initial octree is rebuilt from the training cameras and ``pts_sampler.bbox_levels`` / ``max_level`` /
+    ``split_dist_thres`` (``octree_build.initial_octree``), after the rebuilt valid leaves are checked against the checkpoint's
+    warps (``check_initial_octree``: ValueError on a count or centre mismatch).  The global data pool also gets the saved
+    iteration's gradient-scaling progress.  The scene is still returned in VALIDATE mode; set ``mode_ = TRAIN`` to train."""
     import yaml
     if not os.path.isfile(config_path):
         raise FileNotFoundError(f"load_scene: {config_path} does not exist")
@@ -146,9 +187,15 @@ def load_scene(config_path, checkpoint_dir=None, device="cuda"):
     states = load_states(renderer_pt, dev)
     dataset = load_dataset(dc["data_path"], dc["factor"], dc["bounds_factor"], dev)
     check_states(states, cfg, dataset.n_images_, renderer_pt)
+    edge_pool = None
+    if trainable:
+        from .octree_build import initial_octree
+        tree_nodes, edge_pool = initial_octree(dataset, pc)
+        check_initial_octree(tree_nodes, states[1].cpu().numpy(), cfg, renderer_pt)
+        edge_pool = torch.from_numpy(edge_pool.view(np.uint8).reshape(-1))
 
     gdp = GlobalDataPool()
-    sampler = PersSampler(gdp, states[0], states[1], None, near=float(np.float32(pc["near"])),
+    sampler = PersSampler(gdp, states[0], states[1], edge_pool, near=float(np.float32(pc["near"])),
                           sample_l=float(np.float32(pc["sample_l"])), scale_by_dis=bool(pc["scale_by_dis"]),
                           max_oct_intersect_per_ray=int(pc["max_oct_intersect_per_ray"]), device=dev)
     field = Hash3DAnchored(gdp, log2_table_size=int(fc["log2_table_size"]), mlp_hidden_dim=int(fc["mlp_hidden_dim"]),
@@ -161,5 +208,8 @@ def load_scene(config_path, checkpoint_dir=None, device="cuda"):
     renderer.LoadStates(states)
     gdp.iter_step_ = iter_step
     gdp.ray_march_fineness_ = ray_march_fineness(iter_step, tc["ray_march_init_fineness"], int(tc["ray_march_fineness_decay_end_iter"]))
+    if trainable:
+        gdp.gradient_scaling_progress_ = gradient_scaling_progress(iter_step, tc["gradient_scaling_start"],
+                                                                   tc["gradient_scaling_end"])
     gdp.mode_ = VALIDATE
     return Scene(gdp, renderer, dataset, iter_step)

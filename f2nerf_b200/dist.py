@@ -7,12 +7,15 @@ appearance embedding and octree are replicated; after backward exactly one excha
     overlapping-level quirk) and are never sent;
   * one flattened SUM all-reduce for the two MLP gradients + the appearance-embedding gradient;
   * MAX all-reduce (int32) of the octree votes BEFORE the stat update, so every rank prunes the same
-    nodes (PersSampler.cu:579-603 would otherwise diverge across ranks);
+    nodes (PersSampler.cu:579-603 would otherwise diverge across ranks); a rank whose batch has no sample takes part with
+    neutral votes (Renderer._neutral_votes);
   * OR of the NaN flag, MEAN of the samples-per-ray EMAs that size the next batch (ExpRunner.cpp:86).
 Gradients are averaged (losses are means over the global batch).
 """
 import torch
 import torch.distributed as dist
+
+from .renderer import slab_groups
 
 
 def live_rows(field):
@@ -36,7 +39,8 @@ def install_grad_overlap(renderer):
     previous boundary is final and its SUM all-reduce is issued at once (async, on NCCL's stream, ordered behind the scatter
     stream) while the lower groups still run.  Only the last slab ([0, 5S) of 17S) is exposed.  The 1/world averaging is folded
     into the scatter's gradient multiplier; the backward's last act is to make its stream wait for the slab all-reduces, so
-    the gradient autograd hands to ``.grad`` is already the global average and ``allreduce_grads`` skips the table."""
+    the gradient autograd hands to ``.grad`` is already the global average and ``allreduce_grads`` skips the table.  A rank
+    whose backward did not run (an empty shard) issues the same slab all-reduces from ``allreduce_grads`` instead."""
     world = dist.get_world_size()
     renderer.grad_premul_ = 1.0 / world
     st = dict(hi=None, works=[], table=None)
@@ -62,12 +66,21 @@ def install_grad_overlap(renderer):
 
 def allreduce_grads(renderer):
     """The post-backward exchange step; returns the number of bytes each rank contributed.  Every rank issues the SAME
-    fixed-shape collectives whether or not its own batch produced gradients (a rank whose rays all missed the octree
-    contributes zeros), so ranks can never disagree on the collective sequence."""
+    fixed-shape collectives whether or not its own batch produced gradients (a rank whose rays all missed the octree, or
+    whose shard is empty, contributes zeros), so ranks can never disagree on the collective sequence."""
     world = dist.get_world_size()
     field, shader = renderer.scene_field_, renderer.shader_
     params = (field.mlp_.params_, shader.mlp_.params_, renderer.app_emb_)
     sent = 0
+    hook = getattr(renderer, "grad_slab_hook_", None)
+    if hook is not None and not getattr(renderer, "table_grad_reduced_", False):
+        # overlap installed but no backward of this step called the hook (an empty shard: no graph): issue the same slab
+        # all-reduces the other ranks issued from inside their backward, on a zero contribution
+        if field.feat_pool_.grad is None:
+            field.feat_pool_.grad = torch.zeros_like(field.feat_pool_)
+        for lo, _ in slab_groups():
+            hook(field.feat_pool_.grad, lo, int(field.local_size_))
+        renderer.grad_slab_finish_()
     if getattr(renderer, "table_grad_reduced_", False) and field.feat_pool_.grad is not None:
         renderer.table_grad_reduced_ = False             # averaged slab by slab inside the backward (install_grad_overlap)
         sent += live_rows(field) * 2 * 4

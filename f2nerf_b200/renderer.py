@@ -125,6 +125,8 @@ class Renderer:
         self.sample_result_ = LazySampleResult(slots)
         bg = self._bg(n_rays, dev)
         if n_rays == 0:                                              # an empty batch (Renderer.cpp:83-97); a pending prefetch stays
+            if train:
+                self._neutral_votes(dev)
             z = torch.zeros
             return RenderResult(bg, z((0, 1), device=dev), z((0,), device=dev), None, z((0,), device=dev), None, None)
         S = slots.slot
@@ -215,6 +217,7 @@ class Renderer:
             if n_all <= 0:
                 if train:
                     gdp.meaningful_sampled_pts_per_ray_ *= .9
+                    self._neutral_votes(dev)
                 z = torch.zeros
                 return RenderResult(bg, z((n_rays, 1), device=dev), z((n_rays,), device=dev), None,
                                     torch.full((n_rays,), 512., device=dev), None, None)
@@ -247,6 +250,17 @@ class Renderer:
         if side is not None:
             main.wait_event(votes_done)                           # votes joined before weights0 / alphas0 can be recycled
         return RenderResult(colors, slots.first_oct_dis.clone(), disparity, edge_feats if train else None, depth, weights, new_bounds)
+
+    def _neutral_votes(self, dev):
+        """A TRAIN batch without samples casts no occupancy vote.  Under data parallelism the other ranks' votes are still
+        all-reduced (dist.install_vote_sync), so this rank takes part with neutral ones (-1 votes, no marks, its own visit
+        counts) and applies the synced result: every rank issues the same collectives and keeps the same octree."""
+        sampler = self.pts_sampler_
+        if sampler.vote_allreduce_ is None:
+            return
+        i32 = lambda *sh: torch.empty(sh, dtype=torch.int32, device=dev)
+        f32 = torch.empty((0,), dtype=torch.float32, device=dev)
+        sampler.update_oct_nodes_raw(i32(0, 2), i32(0, 3), f32, f32)
 
     def _fused_forward_ok(self, n_rays):
         """VALIDATE mode takes no gradient, no occupancy votes and no TV-loss edge points: march + ONE kernel

@@ -1,6 +1,7 @@
 """World-size-2 gloo test (CPU) of the data-parallel exchange step in f2nerf_b200/dist.py."""
 import os
 import socket
+from datetime import timedelta
 from types import SimpleNamespace
 
 import numpy as np
@@ -13,18 +14,24 @@ def _free_port():
     s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from f2nerf_b200 import dist as fd
-    from f2nerf_b200.sampler import GlobalDataPool
-    local = 1 << 8
-    pool = local * 16
+def _mock_renderer(rank, local, pool):
     field = SimpleNamespace(feat_pool_=torch.zeros(pool, 2, requires_grad=True), local_size_=local,
                             mlp_=SimpleNamespace(params_=torch.zeros(3072, requires_grad=True)))
     shader = SimpleNamespace(mlp_=SimpleNamespace(params_=torch.zeros(7168, requires_grad=True)))
-    renderer = SimpleNamespace(scene_field_=field, shader_=shader, app_emb_=torch.zeros(5, 16, requires_grad=True),
-                               nonfinite_flag_=torch.tensor([rank == 1, False]))
+    return SimpleNamespace(scene_field_=field, shader_=shader, app_emb_=torch.zeros(5, 16, requires_grad=True),
+                           nonfinite_flag_=torch.tensor([rank == 1, False]))
+
+
+def _worker(rank, world, port, q):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    dist.init_process_group("gloo", rank=rank, world_size=world, timeout=timedelta(seconds=60))
+    from f2nerf_b200 import dist as fd
+    from f2nerf_b200.renderer import slab_groups
+    from f2nerf_b200.sampler import GlobalDataPool
+    local = 1 << 8
+    pool = local * 16
+    renderer = _mock_renderer(rank, local, pool)
+    field, shader = renderer.scene_field_, renderer.shader_
     g = torch.Generator().manual_seed(rank)
     live = fd.live_rows(field)
     assert live == 17 * local // 2
@@ -55,11 +62,29 @@ def _worker(rank, world, port, q):
         renderer.grad_slab_hook_(slab, lo, local)
     renderer.grad_slab_finish_()
     assert renderer.table_grad_reduced_
+    # the overlap installed on both ranks, but rank 1's shard is empty: its backward never runs, so it calls no hook and has
+    # no gradient at all.  allreduce_grads must still issue the slab all-reduces rank 0 issued from inside its backward
+    empty = _mock_renderer(rank, local, pool)
+    fd.install_grad_overlap(empty)
+    ge = torch.Generator().manual_seed(200)
+    own = torch.zeros(pool, 2)
+    if rank == 0:
+        own[:live] = torch.rand(live, 2, generator=ge) * empty.grad_premul_      # the backward's 1/world pre-scaled scatter
+        empty.scene_field_.feat_pool_.grad = own.clone()
+        for lo, _ in slab_groups():
+            empty.grad_slab_hook_(empty.scene_field_.feat_pool_.grad, lo, local)
+        empty.grad_slab_finish_()
+        for p in (empty.scene_field_.mlp_.params_, empty.shader_.mlp_.params_, empty.app_emb_):
+            p.grad = torch.rand(p.shape, generator=ge)
+    e_sent = fd.allreduce_grads(empty)
+    e_got = [empty.scene_field_.feat_pool_.grad, empty.scene_field_.mlp_.params_.grad, empty.shader_.mlp_.params_.grad,
+             empty.app_emb_.grad]
     gdp = GlobalDataPool()
     gdp.sampled_pts_per_ray_ = 100.0 + 50 * rank
     fd.sync_emas(gdp)
     q.put((rank, [t.numpy() for t in mine], [t.numpy() for t in got], renderer.nonfinite_flag_.tolist(), sent,
-           vw.tolist(), va.tolist(), mk.tolist(), vc.tolist(), gdp.sampled_pts_per_ray_, slab0.numpy(), slab.numpy()))
+           vw.tolist(), va.tolist(), mk.tolist(), vc.tolist(), gdp.sampled_pts_per_ray_, slab0.numpy(), slab.numpy(),
+           own.numpy(), [t.numpy() for t in e_got], e_sent, empty.table_grad_reduced_))
     dist.destroy_process_group()
 
 
@@ -68,12 +93,18 @@ def test_allreduce_step_world2():
     q = ctx.Queue()
     port = _free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted([q.get(timeout=120) for _ in range(2)], key=lambda x: x[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    try:
+        for p in procs:
+            p.start()
+        res = sorted([q.get(timeout=120) for _ in range(2)], key=lambda x: x[0])
+        for p in procs:
+            p.join(timeout=60)
+            assert p.exitcode == 0
+    finally:
+        for p in procs:
+            if p.is_alive():
+                p.terminate()
+                p.join(timeout=10)
     (r0, m0, g0, f0, s0, *v0), (r1, m1, g1, f1, s1, *v1) = res
     for a, b, ga, gb in zip(m0, m1, g0, g1):
         np.testing.assert_allclose(ga, (a + b) / 2, rtol=1e-6)           # averaged gradient, identical on both ranks
@@ -87,3 +118,12 @@ def test_allreduce_step_world2():
     np.testing.assert_allclose(v0[6][:live], v0[5][:live] + v1[5][:live], rtol=1e-6)
     np.testing.assert_array_equal(v0[6][:live], v1[6][:live])
     np.testing.assert_array_equal(v0[6][live:], v0[5][live:])
+    # an empty rank under the overlap: same slab all-reduces, so both ranks end with rank 0's pre-scaled contribution (the
+    # average of it and a zero gradient), bit for bit, and report the same bytes sent
+    own0, e0, e1 = v0[7], v0[8], v1[8]
+    assert (own0[:live] != 0).all() and not v1[7].any()
+    np.testing.assert_array_equal(e0[0], own0)
+    for a, b in zip(e0, e1):
+        np.testing.assert_array_equal(a, b)
+    assert v0[9] == v1[9] == s0
+    assert not v0[10] and not v1[10]

@@ -466,19 +466,27 @@ def test_hash_bwd_run_layouts(oracle, hash_params, stride, half):
     check_table(oracle, hp, N(table), pts, v, stride, g, 0.5, f"hash_bwd stride={stride} half={half}")
 
 
-@pytest.mark.parametrize("group", [1, 2, 4, 8])
-def test_hash_bwd_levels_run_layouts(oracle, hash_params, group):
+@pytest.mark.parametrize("stride", [1, 3])
+@pytest.mark.parametrize("half", [False, True])
+@pytest.mark.parametrize("group", [1, 2, 4, 8, "renderer"])
+def test_hash_bwd_levels_run_layouts(oracle, hash_params, group, stride, half):
+    """level groups high to low; "renderer": the data-parallel backward's own groups (renderer.slab_groups), which it scatters
+    with stride-3 anchors and fp16 rows"""
     from f2nerf_b200._lib import call, stream
+    from f2nerf_b200.renderer import slab_groups
     hp = hash_params
     pts, vol, g, _ = layout(oracle, hp)
     n = pts.shape[0]
+    v = vol if stride == 1 else np.stack([vol, vol[::-1], vol], 1).astype(np.int32)
     table = torch.zeros((hp["pool"], 2), dtype=torch.float32, device="cuda")
-    args = (T(hp["prim"]), T(hp["bias"]), hp["V"], hp["local_size"], prefix(pts, np.float32("nan")), prefix(vol, hp["V"] - 1), 1, n,
-            prefix(g, np.float32("nan")), 0, 0.5, table)
-    for lo in reversed(range(0, 16, group)):                       # levels high to low
-        call("f2b_hash_bwd_levels", *args, lo, group, stream())
+    gt = prefix(g.astype(np.float16) if half else g, np.float16("nan") if half else np.float32("nan"))
+    args = (T(hp["prim"]), T(hp["bias"]), hp["V"], hp["local_size"], prefix(pts, np.float32("nan")), prefix(v, hp["V"] - 1), stride,
+            n, gt, int(half), 0.5, table)
+    groups = slab_groups() if group == "renderer" else [(lo, group) for lo in reversed(range(0, 16, group))]
+    for lo, nl in groups:
+        call("f2b_hash_bwd_levels", *args, lo, nl, stream())
     torch.cuda.synchronize()
-    check_table(oracle, hp, N(table), pts, vol, 1, g, 0.5, f"hash_bwd_levels group={group}")
+    check_table(oracle, hp, N(table), pts, v, stride, g, 0.5, f"hash_bwd_levels group={group} stride={stride} half={half}")
 
 
 @pytest.mark.parametrize("stride", [1, 3])

@@ -23,15 +23,22 @@ def build(scene, log2=15, use_app_emb=True, sample_l=1 / 64):
     return gdp, sampler, field, shader, renderer
 
 
-@pytest.mark.parametrize("n_rays,gs_progress,seed,miss", [(192, 1.0, 77, 0), (64, 0.3, 77, 0), (129, 1.0, 11, 7)],
-                         ids=["192-1.0", "64-0.3", "129-1.0-missed"])
-def test_render_train_step_matches_oracle(scene, oracle, n_rays, gs_progress, seed, miss):
+@pytest.mark.parametrize("n_rays,gs_progress,seed,miss,slab", [(192, 1.0, 77, 0, False), (64, 0.3, 77, 0, False),
+                                                                (129, 1.0, 11, 7, False), (129, 1.0, 11, 7, True)],
+                         ids=["192-1.0", "64-0.3", "129-1.0-missed", "129-1.0-missed-slab"])
+def test_render_train_step_matches_oracle(scene, oracle, n_rays, gs_progress, seed, miss, slab):
     """``miss``: every miss-th ray starts far outside the octree and points away (no sample at all); an odd ray count: the 16-lane
-    march packs two rays per warp, so the last warp is half filled."""
+    march packs two rays per warp, so the last warp is half filled.  ``slab``: the data-parallel backward (a slab hook installed,
+    as dist.install_grad_overlap does, here one that only records): unfused MLP backward chain, then level-group scatters."""
     import oracle_pipeline as OP
     from f2nerf_b200 import TRAIN, check_backward_nan, ops, CustomOps
     gdp, sampler, field, shader, renderer = build(scene)
     gdp.mode_, gdp.gradient_scaling_progress_ = TRAIN, gs_progress
+    slab_calls = []
+    if slab:
+        renderer.grad_slab_hook_ = lambda d_table, lo, local_size: slab_calls.append(lo)
+        renderer.grad_slab_finish_ = lambda: slab_calls.append("finish")
+        renderer.grad_premul_ = 1.0
     o, d, dn, cam = make_rays(scene, n_rays, seed=seed)
     if miss:
         o[::miss] = 600.
@@ -57,6 +64,7 @@ def test_render_train_step_matches_oracle(scene, oracle, n_rays, gs_progress, se
     loss = color_loss + 0.01 * var_loss + 0.01 * (res.disparity ** 2).mean() + 0.1 * tv
     loss.backward()
     assert not check_backward_nan(renderer)
+    assert slab_calls == ([12, 8, 4, 0, "finish"] if slab else [])
     cnt = N(res.idx_start_end[:, 1] - res.idx_start_end[:, 0])
     assert cnt.sum() == res.weights.shape[0] and (cnt > 0).any()
     if miss:

@@ -199,8 +199,16 @@ class PersSampler:
         # no record_stream: every tensor the side stream touches stays referenced from the prefetch record / the slots until the
         # consuming Render has made the main stream wait on ``done``, so it cannot be recycled under the march
         self._prefetched = dict(key=(rays_o_raw.data_ptr(), rays_d_raw.data_ptr(), n_rays, rays_o_raw._version, rays_d_raw._version),
-                                slots=slots, done=done, noise_inc=noise_inc, host_totals=host_totals, tree=self.tree_nodes_gpu_.data_ptr(),
+                                slots=slots, done=done, noise_inc=noise_inc, host_totals=host_totals, tree=self._tree_id(),
                                 mode=self.global_data_pool_.mode_, fineness=self.global_data_pool_.ray_march_fineness_)
+
+    def _tree_id(self):
+        """The octree a march ran on: the tensor itself and its version counter, not its address.  ProcOctree and LoadStates
+        replace the tensor (a freed tree's block can come back from the caching allocator for a later one, so an address proves
+        nothing; the record also keeps the marched tree alive until the side stream is done reading it); a host-side in-place
+        write (``copy_``) bumps the version.  The votes' pruning (apply_votes) writes through the raw pointer and bumps nothing:
+        it precedes the prefetched march on its stream.  MarkInvisibleNodes, the other raw-pointer writer, drops the prefetch."""
+        return self.tree_nodes_gpu_, self.tree_nodes_gpu_._version
 
     def take_prefetched(self, rays_o_raw, rays_d_raw):
         """The prefetched march for exactly these ray tensors (and an unchanged octree / mode / fineness), or None."""
@@ -209,7 +217,8 @@ class PersSampler:
             return None
         gdp = self.global_data_pool_
         key = (rays_o_raw.data_ptr(), rays_d_raw.data_ptr(), rays_o_raw.shape[0], rays_o_raw._version, rays_d_raw._version)
-        if (key != pf["key"] or pf["tree"] != self.tree_nodes_gpu_.data_ptr() or pf["mode"] != gdp.mode_
+        tree, version = pf["tree"]
+        if (key != pf["key"] or tree is not self.tree_nodes_gpu_ or version != tree._version or pf["mode"] != gdp.mode_
                 or pf["fineness"] != gdp.ray_march_fineness_ or pf["slots"].generation != getattr(self, "_generation", 0)):
             # (a march in between took the other scratch set and bumped the generation: the prefetched slots are stale by order)
             torch.cuda.current_stream(rays_o_raw.device).wait_event(pf["done"])      # its buffers are released behind the march
@@ -319,6 +328,9 @@ class PersSampler:
         training cameras (the reference keeps them in PersOctree; here the caller passes them)."""
         f = lambda t: torch.as_tensor(t, dtype=torch.float32).to(self.tree_nodes_gpu_.device).contiguous()
         intri, w2c, bounds = f(intri), f(w2c), f(bounds)
+        pf, self._prefetched = getattr(self, "_prefetched", None), None
+        if pf is not None:                                                       # a prefetched march reads the tree written below
+            torch.cuda.current_stream(self.tree_nodes_gpu_.device).wait_event(pf["done"])
         call("f2b_octree_mark_invisible", self.tree_nodes_gpu_, self.n_nodes, intri, w2c, bounds, intri.shape[0], stream())
 
     def maintain(self, cameras=None, compact_freq=1000):

@@ -23,6 +23,50 @@ def build(scene, log2=15, use_app_emb=True, sample_l=1 / 64):
     return gdp, sampler, field, shader, renderer
 
 
+def assert_close_but(a, b, rtol, atol_frac, name, share):
+    """assert_close for all but ``share`` of the elements; those may be up to 5x the bar away.  A density logit whose fp16
+    rounding goes the other way than the oracle's moves its sample's weight by an fp16 ulp of the logit (0.4 % at logits 4..8):
+    over many steps of ~30 k samples a few do."""
+    if share <= 0:
+        return assert_close(a, b, rtol=rtol, atol_frac=atol_frac, name=name)
+    assert_close(a, b, rtol=5 * rtol, atol_frac=5 * atol_frac, name=name)
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    off = np.abs(a - b) > rtol * np.abs(b) + atol_frac * max(np.abs(b).max(), 1e-30)
+    assert off.sum() <= share * off.size, f"{name}: {int(off.sum())} of {off.size} elements past rtol {rtol} / atol_frac {atol_frac}"
+
+
+def check_step_against_oracle(res, sr, loss, ref, g_field, g_shader, g_emb, g_table, flipped_share=0.0):
+    """One TRAIN step (``res`` of Renderer.Render, its SampleResult ``sr``, the loss value and the four gradients) against
+    oracle_pipeline.render_train's ``ref`` on the same rays, noise, parameters and octree.  ``flipped_share``: see
+    assert_close_but (per-sample weights only)."""
+    # integer / index outputs: bit-exact
+    np.testing.assert_array_equal(N(sr.pts_idx_bounds), ref["sample"]["bounds"])
+    np.testing.assert_array_equal(N(sr.pts).view(np.uint32), ref["sample"]["pts"].view(np.uint32))
+    np.testing.assert_array_equal(N(sr.anchors), ref["sample"]["anchors"])
+    assert 0 < ref["n_kept"] <= sr.pts.shape[0]
+    if np.array_equal(N(res.idx_start_end), ref["bounds"]):         # identical keep mask (the usual case)
+        assert_close_but(N(res.weights), ref["weights"], 2e-3, 1e-4, "weights", flipped_share)
+        assert_close(N(res.edge_feats), ref["edge_feats"], rtol=4e-3, atol_frac=2e-3, name="edge_feats")
+    else:                                                           # a threshold-straddling sample: sizes differ by a few
+        assert abs(int(res.idx_start_end[-1, 1]) - ref["n_kept"]) <= 3
+    assert_close(N(res.colors), ref["colors"], rtol=2e-3, atol_frac=2e-3, name="colors")
+    assert_close(N(res.disparity), ref["disparity"], rtol=2e-3, atol_frac=2e-3, name="disparity")
+    assert_close(N(res.depth), ref["depth"], rtol=2e-3, atol_frac=2e-3, name="depth")
+    assert abs(loss - ref["loss"]) <= 2e-5 * abs(ref["loss"])
+    # gradients.  Globally (relative L2 against the oracle's fp32-accumulate chain with the same fp16 rounding points) they
+    # agree to ~1e-5 (cf. tests/test_gpu_headline.py); element-wise a single flipped fp16 rounding shows,
+    # hence the looser per-element bars below
+    rel = lambda a, b: float(np.linalg.norm(np.asarray(a, np.float64) - b) / (np.linalg.norm(b) + 1e-300))
+    for name, mine in (("grad_field_mlp", g_field), ("grad_shader_mlp", g_shader), ("grad_app_emb", g_emb), ("grad_feat_pool", g_table)):
+        assert rel(N(mine), np.asarray(ref[name], np.float64)) <= 1e-3, (name, rel(N(mine), np.asarray(ref[name], np.float64)))
+    assert_close(N(g_field), ref["grad_field_mlp"], rtol=2e-2, atol_frac=1e-2, name="grad field mlp")
+    assert_close(N(g_shader), ref["grad_shader_mlp"], rtol=2e-2, atol_frac=1e-2, name="grad shader mlp")
+    assert_close(N(g_emb), ref["grad_app_emb"], rtol=2e-2, atol_frac=1e-2, name="grad app_emb")
+    g, gr = N(g_table), ref["grad_feat_pool"]
+    assert_close(g, gr, rtol=3e-2, atol_frac=1e-2, name="grad feat_pool")
+    assert np.abs(gr).max() > 0
+
+
 @pytest.mark.parametrize("n_rays,gs_progress,seed,miss,slab", [(192, 1.0, 77, 0, False), (64, 0.3, 77, 0, False),
                                                                 (129, 1.0, 11, 7, False), (129, 1.0, 11, 7, True)],
                          ids=["192-1.0", "64-0.3", "129-1.0-missed", "129-1.0-missed-slab"])
@@ -79,34 +123,9 @@ def test_render_train_step_matches_oracle(scene, oracle, n_rays, gs_progress, se
     ref = OP.render_train(sc, o, N((rays_d / torch.linalg.norm(rays_d, 2, -1, True))), N(noise), N(bg), fld,
                           N(shader.mlp_.params_), N(renderer.app_emb_), cam, (N(e_idx), N(e_coord)), N(gt),
                           scales=ops.hash_level_scales().numpy(), gs_progress=gs_progress)
-    # integer / index outputs: bit-exact
-    sr = renderer.sample_result_
-    np.testing.assert_array_equal(N(sr.pts_idx_bounds), ref["sample"]["bounds"])
-    np.testing.assert_array_equal(N(sr.pts).view(np.uint32), ref["sample"]["pts"].view(np.uint32))
-    np.testing.assert_array_equal(N(sr.anchors), ref["sample"]["anchors"])
-    assert 0 < ref["n_kept"] < sr.pts.shape[0], "early stop must be exercised"
-    if np.array_equal(N(res.idx_start_end), ref["bounds"]):         # identical keep mask (the usual case)
-        assert_close(N(res.weights), ref["weights"], rtol=2e-3, atol_frac=1e-4, name="weights")
-        assert_close(N(res.edge_feats), ref["edge_feats"], rtol=4e-3, atol_frac=2e-3, name="edge_feats")
-    else:                                                           # a threshold-straddling sample: sizes differ by a few
-        assert abs(int(res.idx_start_end[-1, 1]) - ref["n_kept"]) <= 3
-    assert_close(N(res.colors), ref["colors"], rtol=2e-3, atol_frac=2e-3, name="colors")
-    assert_close(N(res.disparity), ref["disparity"], rtol=2e-3, atol_frac=2e-3, name="disparity")
-    assert_close(N(res.depth), ref["depth"], rtol=2e-3, atol_frac=2e-3, name="depth")
-    assert abs(float(loss) - ref["loss"]) <= 2e-5 * abs(ref["loss"])
-    # gradients.  Globally (relative L2 against the oracle's fp32-accumulate chain with the same fp16 rounding points) they
-    # agree to ~1e-5 (cf. tests/test_gpu_headline.py); element-wise a single flipped fp16 rounding shows,
-    # hence the looser per-element bars below
-    rel = lambda a, b: float(np.linalg.norm(np.asarray(a, np.float64) - b) / (np.linalg.norm(b) + 1e-300))
-    for name, mine in (("grad_field_mlp", field.mlp_.params_.grad), ("grad_shader_mlp", shader.mlp_.params_.grad),
-                       ("grad_app_emb", renderer.app_emb_.grad), ("grad_feat_pool", field.feat_pool_.grad)):
-        assert rel(N(mine), np.asarray(ref[name], np.float64)) <= 1e-3, (name, rel(N(mine), np.asarray(ref[name], np.float64)))
-    assert_close(N(field.mlp_.params_.grad), ref["grad_field_mlp"], rtol=2e-2, atol_frac=1e-2, name="grad field mlp")
-    assert_close(N(shader.mlp_.params_.grad), ref["grad_shader_mlp"], rtol=2e-2, atol_frac=1e-2, name="grad shader mlp")
-    assert_close(N(renderer.app_emb_.grad), ref["grad_app_emb"], rtol=2e-2, atol_frac=1e-2, name="grad app_emb")
-    g, gr = N(field.feat_pool_.grad), ref["grad_feat_pool"]
-    assert_close(g, gr, rtol=3e-2, atol_frac=1e-2, name="grad feat_pool")
-    assert np.abs(gr).max() > 0
+    assert ref["n_kept"] < renderer.sample_result_.pts.shape[0], "early stop must be exercised"
+    check_step_against_oracle(res, renderer.sample_result_, float(loss), ref, field.mlp_.params_.grad, shader.mlp_.params_.grad,
+                              renderer.app_emb_.grad, field.feat_pool_.grad)
     # octree statistics moved and match an oracle replay of the votes
     assert (N(sampler.tree_weight_stats_) != stats0).any()
 

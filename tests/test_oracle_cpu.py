@@ -5,6 +5,7 @@ and against known answers recorded from the reference (SURVEY.md §8a probes); t
 against outputs of the reference itself lives in test_golden_ref.py.
 """
 import numpy as np
+import pytest
 import torch
 
 from conftest import make_rays
@@ -257,6 +258,44 @@ def test_octree_proc_invariants(scene, oracle):
                         want = np.array([[(st >> 2) & 1, (st >> 1) & 1, st & 1] for st in range(8)]) * 2 - 1
                         np.testing.assert_array_equal(off, want)
         assert ow.shape[0] == m and oa.shape[0] == m
+
+
+@pytest.mark.parametrize("schedule", ["compact", "milestone", "brute", "milestone+compact", "two-due"])
+def test_train_loop_octree_invariants(scene, oracle, schedule):
+    """The multi-step octree driver (tests/oracle_train_loop.py: votes, subdivision milestones, MarkInvisibleNodes, periodic
+    compaction) over eight iterations on synthetic weights — leaves inside a ball around the origin are occupied, the others
+    empty, statistics start at the pruning threshold.  After every step: links consistent, no dead leaf left by a compaction,
+    split leaves have their 8 octants, visit counts zero after ProcOctree, milestones consumed from the back; every schedule
+    prunes and renumbers, the milestone schedules subdivide."""
+    import oracle_train_loop as TL
+    ms, compact_freq = TL.SCHEDULES[schedule]
+    n = scene["nodes"].size // 64
+    rng = np.random.default_rng(2)
+    st = TL.OctreeState(scene["nodes"], rng.integers(0, 3, n), rng.integers(0, 3, n), ms)
+    cams = TL.scene_cameras(scene["scene"], 6)
+    t0 = TL.tree_view(scene["nodes"])
+    radius = np.median(np.linalg.norm(t0["center"][t0["leaf"] & (t0["trans"] >= 0)], axis=1))
+    counts, kinds, splits = [n], [], 0
+    for it in range(1, TL.N_ITERS + 1):
+        n_rays = (150, 97)[it % 2]
+        o, d, dn, _ = make_rays(scene, n_rays, seed=40 + it)
+        noise = (np.random.default_rng(it).random(1024 + n_rays + 10, dtype=np.float32) + .5).astype(np.float32)
+        s = oracle.sampler(st.nodes, scene["trans"], o, dn, noise, 0.05, 1e8, 1 / 64, True, 1024)
+        assert s["pts"].shape[0] > 0 and s["anchors"][:, 1].max() < st.n_nodes
+        t = TL.tree_view(st.nodes)
+        assert t["leaf"][s["anchors"][:, 1]].all() and (t["trans"][s["anchors"][:, 1]] == s["anchors"][:, 0]).all()
+        occupied = np.linalg.norm(t["center"][s["anchors"][:, 1]], axis=1) < radius
+        w = np.where(occupied, np.float32(.5), np.float32(0))
+        before = list(st.milestones)
+        log = TL.train_step(st, it, s["bounds"], s["anchors"], w, w, cams, compact_freq)
+        TL.check_maintain_log(log, st, before, it, compact_freq)
+        counts.append(st.n_nodes)
+        kinds += [k for k, *_ in log]
+        splits += sum(int(TL.tree_view(a)["leaf"].sum()) > int((TL.tree_view(b)["leaf"] & (TL.tree_view(b)["trans"] >= 0)).sum())
+                      for k, _, b, _, a in log if k == "subdivide")
+    assert st.milestones == [] and len(set(counts)) > 1
+    assert kinds.count("subdivide") == len(ms) and (not ms or splits >= 1)
+    assert min(counts) < n or schedule == "milestone"                # dead leaves were dropped (the milestone schedule grows)
 
 
 def test_img2world_rays_undistorted_closed_form(oracle):

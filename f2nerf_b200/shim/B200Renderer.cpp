@@ -89,6 +89,7 @@ struct ShimProfile {
   }
 };
 ShimProfile g_prof;
+long g_grad_reused = 0, g_grad_fresh = 0;         // table-gradient storage paths taken by the backwards (see RenderFn::backward)
 struct ScopedTimer {
   double* acc; long* cnt; std::chrono::steady_clock::time_point t0;
   ScopedTimer(double* a, long* c) : acc(g_prof.on ? a : nullptr), cnt(c), t0(std::chrono::steady_clock::now()) {}
@@ -237,9 +238,11 @@ public:
     if (wk.d_table_storage && wk.d_table_storage.nbytes() == size_t(table_numel) * 4 && wk.d_table_storage.use_count() == 1) {
       d_table = torch::empty({0}, CUDAFloat).set_(wk.d_table_storage, 0, {table_numel / 2, 2});
       d_table.view({-1}).slice(0, 0, live).zero_();
+      ++g_grad_reused;
     } else {
       d_table = torch::zeros({table_numel / 2, 2}, CUDAFloat);
       wk.d_table_storage = d_table.storage();
+      ++g_grad_fresh;
     }
     const bool emb_on = k.ray_emb_idx.defined();
     Tensor d_app = emb_on ? torch::zeros({ctx->saved_data["n_emb"].toInt(), 16}, CUDAFloat) : Tensor();
@@ -278,6 +281,8 @@ public:
 };
 
 }  // namespace
+
+void f2b_render_grad_storage_counts(long* reused, long* fresh) { *reused = g_grad_reused; *fresh = g_grad_fresh; }
 
 // =================================================================================================================
 RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw, const Tensor& bounds_raw, const Tensor& emb_idx) {

@@ -11,6 +11,16 @@
 //   ref_driver <runtime_config.yaml> <out_dir> <n_rays> [n_time_iters=0] [dump_full_grads=0]
 //   ref_driver --train <runtime_config.yaml>      what the reference's main.cpp does: ExpRunner(conf).Execute() — the
 //                                                 unmodified trainer (train to end_iter, then TestImages -> mean PSNR)
+//   ref_driver --steps <runtime_config.yaml> <out_dir> <n_iters> [fixed_batch=0]
+//       n_iters iterations of the body of ExpRunner::Train (src/ExpRunner.cpp:81-175) from iter_step_ = 0 on the
+//       deterministic parameters below: batch size from the meaningful-samples EMA (:86, or fixed_batch), RandRaysData,
+//       Render, the losses with the config's schedule weights, zero_grad / backward / the backward_nan_ skip / Adam step,
+//       iter_step_++ and UpdateAdaParams (:221-254).  So octree maintenance (compaction, subdivision milestones) runs
+//       inside Render on the iterations the config names.  It deviates from the trainer in two ways: both torch
+//       generators are reseeded (kStepSeed + k) at the start of iteration k, so that every iteration can be replayed from
+//       its dumped state alone; and after each iteration a small probe is drawn from each generator and dumped — equal
+//       probes mean the iteration consumed the same draws.  Per iteration, <out_dir>/it<k>/ holds the state before the
+//       step, the Render outputs, the loss, the gradients, the octree after the step and the probes.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -56,28 +66,29 @@ static void dump(const std::string& name, const Tensor& t_in) {
 }
 static void dump_scalar(const std::string& name, float v) { dump(name, torch::full({1}, v, CPUFloat)); }
 
-int main(int argc, char** argv) {
-  if (argc >= 3 && std::string(argv[1]) == "--train") {     // main.cpp:6-13 verbatim in behaviour
-    torch::manual_seed(2022);
-    auto exp_runner = std::make_unique<ExpRunner>(argv[2]);
-    exp_runner->Execute();
-    return 0;
-  }
-  if (argc < 4) { std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads]\n"); return 1; }
-  const std::string conf_path = argv[1];
-  g_out = argv[2];
-  const int n_rays = std::atoi(argv[3]);
-  const int n_time = argc > 4 ? std::atoi(argv[4]) : 0;
-  const int full_grads = argc > 5 ? std::atoi(argv[5]) : 0;
-  fs::create_directories(g_out);
+// The reference's objects as ExpRunner::ExpRunner builds them, with the deterministic parameters below and, in
+// ref_driver_b200, this library's drop-in installed.
+struct Scene {
+  std::unique_ptr<GlobalDataPool> gdp;
+  std::unique_ptr<Dataset> dataset;
+  std::unique_ptr<Renderer> renderer;
+  PersSampler* sampler = nullptr;
+  Hash3DAnchored* field = nullptr;
+  SHShader* shader = nullptr;
+};
 
+static Scene make_scene(const std::string& conf_path, bool fixed_lr) {
+  Scene sc;
   torch::manual_seed(2022);   // main.cpp:8
-  auto gdp = std::make_unique<GlobalDataPool>(conf_path);
+  sc.gdp = std::make_unique<GlobalDataPool>(conf_path);
+  GlobalDataPool* gdp = sc.gdp.get();
   gdp->base_exp_dir_ = gdp->config_["base_exp_dir"].as<std::string>();
   fs::create_directories(gdp->base_exp_dir_);
-  gdp->learning_rate_ = 1e-2f;
-  auto dataset = std::make_unique<Dataset>(gdp.get());
-  auto renderer = std::make_unique<Renderer>(gdp.get(), dataset->n_images_);
+  if (fixed_lr) gdp->learning_rate_ = 1e-2f;
+  sc.dataset = std::make_unique<Dataset>(gdp);
+  sc.renderer = std::make_unique<Renderer>(gdp, sc.dataset->n_images_);
+  auto& dataset = sc.dataset;
+  auto& renderer = sc.renderer;
   auto* sampler = dynamic_cast<PersSampler*>(renderer->pts_sampler_.get());
   auto* field = dynamic_cast<Hash3DAnchored*>(renderer->scene_field_.get());
   auto* shader = dynamic_cast<SHShader*>(renderer->shader_.get());
@@ -102,12 +113,19 @@ int main(int argc, char** argv) {
   const bool shim_ops = shim_env && std::string(shim_env) == "ops";
   if (shim_ops) {
     f2b_render_use_reference(true);
-    auto b_sampler = std::make_unique<B200Sampler>(gdp.get());
+    auto b_sampler = std::make_unique<B200Sampler>(gdp);
     b_sampler->pers_octree_ = std::move(sampler->pers_octree_);          // the very same octree / warps / edge pool
-    auto b_field = std::make_unique<B200HashField>(gdp.get());
+    auto b_field = std::make_unique<B200HashField>(gdp);
     b_field->LoadStates(field->States(), 0);
-    auto b_shader = std::make_unique<B200Shader>(gdp.get());
+    auto b_shader = std::make_unique<B200Shader>(gdp);
     b_shader->LoadStates(shader->States(), 0);
+    // Renderer::OptimParamGroups / States / LoadStates walk the sub-pipes the constructor registered (Renderer.cpp:28-35,
+    // Pipe.cpp): point them at the replacements, or they would reach the destroyed originals
+    for (auto& p : renderer->sub_pipes_) {
+      if (p == sampler) p = b_sampler.get();
+      else if (p == field) p = b_field.get();
+      else if (p == shader) p = b_shader.get();
+    }
     renderer->pts_sampler_ = std::move(b_sampler);
     renderer->scene_field_ = std::move(b_field);
     renderer->shader_ = std::move(b_shader);
@@ -121,8 +139,12 @@ int main(int argc, char** argv) {
     std::printf("ref_driver_b200: Renderer::Render replaced by the fused B200 host\n");
   }
 #endif
+  sc.sampler = sampler; sc.field = field; sc.shader = shader;
+  return sc;
+}
 
-  // ---- scene blobs & scalars --------------------------------------------------------------------
+static void dump_scene(const Scene& sc, int n_rays) {
+  auto* sampler = sc.sampler; auto* field = sc.field; auto* shader = sc.shader;
   dump("tree_nodes", sampler->pers_octree_->tree_nodes_gpu_);
   dump("pers_trans", sampler->pers_octree_->pers_trans_gpu_);
   dump("edge_pool", sampler->pers_octree_->edge_pool_gpu_);
@@ -131,14 +153,47 @@ int main(int argc, char** argv) {
   dump("bias_pool", field->bias_pool_);
   dump("field_mlp_params", field->mlp_->params_);
   dump("shader_mlp_params", shader->mlp_->params_);
-  dump("app_emb", renderer->app_emb_);
-  {
-    Tensor sc = torch::zeros({8}, CPUFloat);
-    sc[0] = sampler->global_near_; sc[1] = sampler->sample_l_; sc[2] = sampler->scale_by_dis_ ? 1.f : 0.f;
-    sc[3] = float(sampler->max_oct_intersect_per_ray_); sc[4] = float(field->n_volumes_);
-    sc[5] = float(field->pool_size_); sc[6] = float(dataset->n_images_); sc[7] = float(n_rays);
-    dump("scalars", sc);
+  dump("app_emb", sc.renderer->app_emb_);
+  Tensor s = torch::zeros({8}, CPUFloat);
+  s[0] = sampler->global_near_; s[1] = sampler->sample_l_; s[2] = sampler->scale_by_dis_ ? 1.f : 0.f;
+  s[3] = float(sampler->max_oct_intersect_per_ray_); s[4] = float(field->n_volumes_);
+  s[5] = float(field->pool_size_); s[6] = float(sc.dataset->n_images_); s[7] = float(n_rays);
+  dump("scalars", s);
+}
+
+static int run_steps(const std::string& conf_path, const std::string& out_root, int n_iters, int fixed_batch);
+
+int main(int argc, char** argv) {
+  if (argc >= 3 && std::string(argv[1]) == "--train") {     // main.cpp:6-13 verbatim in behaviour
+    torch::manual_seed(2022);
+    auto exp_runner = std::make_unique<ExpRunner>(argv[2]);
+    exp_runner->Execute();
+    return 0;
   }
+  if (argc >= 5 && std::string(argv[1]) == "--steps")
+    return run_steps(argv[2], argv[3], std::atoi(argv[4]), argc > 5 ? std::atoi(argv[5]) : 0);
+  if (argc < 4) {
+    std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads]\n"
+                         "       ref_driver --steps <config.yaml> <out_dir> <n_iters> [fixed_batch]\n");
+    return 1;
+  }
+  const std::string conf_path = argv[1];
+  g_out = argv[2];
+  const int n_rays = std::atoi(argv[3]);
+  const int n_time = argc > 4 ? std::atoi(argv[4]) : 0;
+  const int full_grads = argc > 5 ? std::atoi(argv[5]) : 0;
+  fs::create_directories(g_out);
+
+  Scene sc = make_scene(conf_path, true);
+  GlobalDataPool* gdp = sc.gdp.get();
+  auto& dataset = sc.dataset;
+  auto& renderer = sc.renderer;
+  auto* sampler = sc.sampler;
+  auto* field = sc.field;
+  auto* shader = sc.shader;
+
+  // ---- scene blobs & scalars --------------------------------------------------------------------
+  dump_scene(sc, n_rays);
 
   // ---- rays ---------------------------------------------------------------------------------------
   torch::manual_seed(2023);
@@ -332,5 +387,161 @@ int main(int argc, char** argv) {
     dump("oct_nodes_final", oct.tree_nodes_gpu_); dump("oct_w_final", oct.tree_weight_stats_); dump("oct_a_final", oct.tree_alpha_stats_);
   }
   std::printf("ref_driver: done, dumps in %s\n", g_out.c_str());
+  return 0;
+}
+
+// ==================================================================================================== --steps ===
+static const int64_t kStepSeed = 31000;
+
+static void dump_octree(const std::string& prefix, PersSampler* sampler) {
+  auto& oct = *sampler->pers_octree_;
+  dump(prefix + "tree_nodes", oct.tree_nodes_gpu_);
+  dump(prefix + "weight_stats", oct.tree_weight_stats_); dump(prefix + "alpha_stats", oct.tree_alpha_stats_);
+  dump(prefix + "visit_cnt", oct.tree_visit_cnt_);
+  // [count, the remaining milestones as the sampler holds them: reversed, the next one last (PersSampler.cpp:674)]
+  const auto& ms = sampler->sub_div_milestones_;
+  Tensor t = torch::zeros({int64_t(ms.size()) + 1}, CPUInt);
+  t[0] = int(ms.size());
+  for (size_t i = 0; i < ms.size(); i++) t[i + 1] = ms[i];
+  dump(prefix + "milestones", t);
+}
+
+static int run_steps(const std::string& conf_path, const std::string& out_root, int n_iters, int fixed_batch) {
+  Scene sc = make_scene(conf_path, false);
+  GlobalDataPool* gdp = sc.gdp.get();
+  Dataset* dataset = sc.dataset.get();
+  Renderer* renderer = sc.renderer.get();
+  auto* sampler = sc.sampler; auto* field = sc.field; auto* shader = sc.shader;
+  const auto& tc = gdp->config_["train"];                                                  // ExpRunner.cpp:28-45
+  const int pts_batch_size = tc["pts_batch_size"].as<int>(), end_iter = tc["end_iter"].as<int>();
+  const float learning_rate = tc["learning_rate"].as<float>(), learning_rate_alpha = tc["learning_rate_alpha"].as<float>();
+  const int warm_up_end_iter = tc["learning_rate_warm_up_end_iter"].as<int>();
+  const float init_fineness = tc["ray_march_init_fineness"].as<float>();
+  const int fineness_decay_end_iter = tc["ray_march_fineness_decay_end_iter"].as<int>();
+  const float tv_loss_weight = tc["tv_loss_weight"].as<float>(), disp_loss_weight = tc["disp_loss_weight"].as<float>();
+  const float var_loss_weight_max = tc["var_loss_weight"].as<float>();
+  const int var_loss_start = tc["var_loss_start"].as<int>(), var_loss_end = tc["var_loss_end"].as<int>();
+  const int gs_start = tc["gradient_scaling_start"].as<int>(), gs_end = tc["gradient_scaling_end"].as<int>();
+  torch::optim::Adam optimizer(renderer->OptimParamGroups());                                // :54
+  int iter_step = 0;
+  auto update_ada_params = [&]() {                                                          // :221-254
+    if (iter_step >= fineness_decay_end_iter) {
+      gdp->ray_march_fineness_ = 1.f;
+    } else {
+      float progress = float(iter_step) / float(fineness_decay_end_iter);
+      gdp->ray_march_fineness_ = std::exp(std::log(1.f) * progress + std::log(init_fineness) * (1.f - progress));
+    }
+    float lr_factor;
+    if (iter_step >= warm_up_end_iter) {
+      float progress = float(iter_step - warm_up_end_iter) / float(end_iter - warm_up_end_iter);
+      lr_factor = (1.f - learning_rate_alpha) * (std::cos(progress * float(M_PI)) * .5f + .5f) + learning_rate_alpha;
+    } else {
+      lr_factor = float(iter_step) / float(warm_up_end_iter);
+    }
+    for (auto& g : optimizer.param_groups()) g.options().set_lr(learning_rate * lr_factor);
+    float progress = 1.f;
+    if (iter_step < gs_end) progress = std::max(0.f, (float(iter_step) - gs_start) / (gs_end - gs_start + 1e-9f));
+    gdp->gradient_scaling_progress_ = progress;
+  };
+
+  gdp->mode_ = RunningMode::TRAIN;                                                          // :66
+  update_ada_params();                                                                      // :76
+  gdp->iter_step_ = iter_step;                                                              // :80
+  g_out = out_root;
+  fs::create_directories(g_out);
+  dump_scene(sc, fixed_batch);
+  {
+    auto& oct = *sampler->pers_octree_;                  // the cameras MarkInvisibleNodes tests against
+    dump("oct_intri", oct.intri_.reshape({-1, 9})); dump("oct_w2c", oct.w2c_.reshape({-1, 12})); dump("oct_bound", oct.bound_);
+    dump("ds_poses", dataset->poses_.reshape({-1, 12})); dump("ds_intri", dataset->intri_.reshape({-1, 9}));
+    dump("ds_dist_params", dataset->dist_params_); dump("ds_bounds", dataset->bounds_);
+    Tensor hw = torch::zeros({2}, CPUFloat); hw[0] = float(dataset->height_); hw[1] = float(dataset->width_);
+    dump("ds_hw", hw);
+    dump("ds_train_set", torch::from_blob(dataset->train_set_.data(), {int(dataset->train_set_.size())}, CPUInt).clone());
+    Tensor run = torch::zeros({4}, CPUFloat);
+    run[0] = float(sampler->compact_freq_); run[1] = float(pts_batch_size); run[2] = float(kStepSeed); run[3] = float(n_iters);
+    dump("run", run);
+  }
+
+  for (int k = 0; k < n_iters; k++) {
+    g_out = out_root + "/it" + std::to_string(k);
+    fs::create_directories(g_out);
+    gdp->backward_nan_ = false;                                                             // :82
+    torch::manual_seed(kStepSeed + k);                                                      // harness: replayable iterations
+    const int n_rays = fixed_batch > 0 ? fixed_batch
+                                       : int(pts_batch_size / gdp->meaningful_sampled_pts_per_ray_) >> 4 << 4;    // :86
+    float var_loss_weight = 0.f;                                                            // :108-114
+    if (iter_step > var_loss_end) var_loss_weight = var_loss_weight_max;
+    else if (iter_step > var_loss_start)
+      var_loss_weight = float(iter_step - var_loss_start) / float(var_loss_end - var_loss_start) * var_loss_weight_max;
+
+    // ---- the state the step starts from
+    dump("feat_pool", field->feat_pool_); dump("field_mlp_params", field->mlp_->params_);
+    dump("shader_mlp_params", shader->mlp_->params_); dump("app_emb", renderer->app_emb_);
+    dump_octree("", sampler);
+    const int64_t nodes_before = sampler->pers_octree_->tree_nodes_gpu_.numel() / 64;
+    {
+      Tensor st = torch::zeros({12}, CPUFloat);
+      st[0] = float(gdp->iter_step_); st[1] = float(n_rays); st[2] = gdp->ray_march_fineness_; st[3] = gdp->gradient_scaling_progress_;
+      st[4] = field->mlp_->loss_scale_; st[5] = shader->mlp_->loss_scale_; st[6] = gdp->sampled_oct_per_ray_;
+      st[7] = gdp->sampled_pts_per_ray_; st[8] = gdp->meaningful_sampled_pts_per_ray_; st[9] = var_loss_weight;
+      st[10] = disp_loss_weight; st[11] = tv_loss_weight;
+      dump("state", st);
+    }
+
+    // ---- the step
+    auto [train_rays, gt_colors, emb_idx] = dataset->RandRaysData(n_rays, DATA_TRAIN_SET);   // :87
+    dump("rays_o", train_rays.origins); dump("rays_d", train_rays.dirs); dump("gt_colors", gt_colors); dump("emb_idx", emb_idx);
+    auto r = renderer->Render(train_rays.origins, train_rays.dirs, train_rays.bounds, emb_idx);   // :93
+    if (k == 0) {
+      const auto& s = renderer->sample_result_;
+      dump("sample_pts", s.pts); dump("sample_dt", s.dt); dump("sample_t", s.t); dump("sample_bounds", s.pts_idx_bounds);
+      dump("sample_anchors", s.anchors.index({Slc(), Slc(0, 2)}).contiguous());
+    }
+    Tensor pred_colors = r.colors.index({Slc(0, n_rays)});                                 // :94-118
+    Tensor color_loss = torch::sqrt((pred_colors - gt_colors).square() + 1e-4f).mean();
+    Tensor disparity_loss = r.disparity.square().mean();
+    Tensor tv_loss = (r.edge_feats.index({Slc(), 0}) - r.edge_feats.index({Slc(), 1})).square().mean();
+    Tensor var_loss = (CustomOps::WeightVar(r.weights, r.idx_start_end) + 1e-2).sqrt().mean();
+    Tensor loss = color_loss + var_loss * var_loss_weight + disparity_loss * disp_loss_weight + tv_loss * tv_loss_weight;
+    dump("colors", pred_colors); dump("disparity", r.disparity); dump("depth", r.depth); dump("weights", r.weights);
+    dump("idx_start_end", r.idx_start_end); dump("edge_feats", r.edge_feats); dump("first_oct_dis", r.first_oct_dis);
+    dump("loss", loss.reshape({1}));
+    bool stepped = false;
+    if (loss.requires_grad()) {                                                             // :128-138
+      optimizer.zero_grad();
+      loss.backward();
+      dump("grad_field_mlp", field->mlp_->params_.grad()); dump("grad_shader_mlp", shader->mlp_->params_.grad());
+      if (renderer->app_emb_.grad().defined()) dump("grad_app_emb", renderer->app_emb_.grad());
+      Tensor g = field->feat_pool_.grad().reshape({-1});
+      Tensor nz = torch::nonzero(g).reshape({-1});
+      dump("grad_feat_pool_nz_idx", nz.to(torch::kInt32)); dump("grad_feat_pool_nz_val", g.index({nz}));
+      if (!gdp->backward_nan_) { optimizer.step(); stepped = true; }
+    }
+    const bool nan_skip = gdp->backward_nan_;                                               // :131-134: `continue`
+    if (!nan_skip) {
+      iter_step++;                                                                          // :142-143
+      gdp->iter_step_ = iter_step;
+      update_ada_params();                                                                  // :175
+    }
+
+    // ---- after the step: the octree (maintained inside Render), the EMAs, the two generators
+    dump_octree("after_", sampler);
+    long reused = 0, fresh = 0;
+#ifdef F2B_WITH_SHIM
+    f2b_render_grad_storage_counts(&reused, &fresh);
+#endif
+    Tensor af = torch::zeros({8}, CPUFloat);
+    af[0] = float(gdp->iter_step_); af[1] = gdp->sampled_oct_per_ray_; af[2] = gdp->sampled_pts_per_ray_;
+    af[3] = gdp->meaningful_sampled_pts_per_ray_; af[4] = nan_skip ? 1.f : 0.f; af[5] = float(reused); af[6] = float(fresh);
+    af[7] = stepped ? 1.f : 0.f;
+    dump("after", af);
+    dump("probe_cpu", torch::rand({4}, CPUFloat));
+    dump("probe_cuda", torch::rand({4}, CUDAFloat));
+    std::printf("{\"step\": %d, \"iter_step\": %d, \"n_rays\": %d, \"loss\": %.6f, \"nodes\": [%lld, %lld], \"backward_nan\": %d, "
+                "\"grad_storage\": {\"reused\": %ld, \"fresh\": %ld}}\n", k, int(gdp->iter_step_), n_rays, loss.item<float>(),
+                (long long) nodes_before, (long long) (sampler->pers_octree_->tree_nodes_gpu_.numel() / 64), int(nan_skip), reused, fresh);
+  }
+  std::printf("ref_driver: done, %d steps in %s\n", n_iters, out_root.c_str());
   return 0;
 }

@@ -5,14 +5,15 @@
 # So does the trained-checkpoint module (tests/test_gpu_checkpoint.py): it trains ngp_fox with the reference program once.
 # And the training-with-octree-maintenance module (tests/test_gpu_train_maintenance.py): eight fused TRAIN steps per case.
 # And the C++-host training-steps module (tests/test_gpu_cpp_host_steps.py): it runs the reference program for ten iterations per arm.
+# And the float64-autograd gradient module (tests/test_gpu_grad_autograd.py): 48 TRAIN steps, each with a float64 twin on the device.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
      "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
      tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py tests/test_gpu_train_maintenance.py
-     tests/test_gpu_cpp_host_steps.py)
+     tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
       --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
-      --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py)
+      --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py --ignore=tests/test_gpu_grad_autograd.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py

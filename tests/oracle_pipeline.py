@@ -20,7 +20,9 @@ def render_train(sc, rays_o, rays_dn, noise, bg, field, shader_params, app_emb=N
                  diagnostics=False):
     """sc: dict(nodes, trans, edges, near, sample_l, scale_by_dis, max_hits)
     field: dict(table16 [pool,2] f16, prim, bias, V, local_size, mlp_params f32)
-    edge: (edge_idx [n], edge_coord [n,2]) or None.  Returns dict of forward outputs (+ grads)."""
+    edge: (edge_idx [n], edge_coord [n,2]) or None.  Returns dict of forward outputs (+ grads).
+    loss_w: weights of the colour, variance, disparity and TV terms (ExpRunner.cpp:116-118), optionally a fifth one of a
+    squared-depth term (mean depth^2) that takes the d_depth path of the composite backward."""
     out = {}
     s = O.sampler(sc["nodes"], sc["trans"], rays_o, rays_dn, noise, sc["near"], 1e8, sc["sample_l"], sc["scale_by_dis"],
                   sc["max_hits"])
@@ -58,29 +60,31 @@ def render_train(sc, rays_o, rays_dn, noise, bg, field, shader_params, app_emb=N
     colors, disp, depth, weights = O.composite_fwd(scene_feat[:n_kept], 16, rgb, dt, t, nb, bg)
     edge_feats = scene_feat[n_kept:].reshape(-1, 2, 16)
     out.update(colors=colors, disparity=disp, depth=depth, weights=weights, edge_feats=edge_feats, scene_feat=scene_feat,
-               rgb=rgb, pts=pts)
+               rgb=rgb, pts=pts, feat16=feat16, mlp_in=mlp_in, raw=raw, q_pts=q_pts, q_vol=q_vol, dt=dt, t=t, dirs=dirs)
     if gt_colors is None:
         return out
     # losses (ExpRunner.cpp:94-118)
-    wc, wv, wd, wt = loss_w
+    wc, wv, wd, wt = loss_w[:4]
+    wz = loss_w[4] if len(loss_w) > 4 else 0.0
     diff = colors - gt_colors
     color_loss = np.sqrt(diff * diff + 1e-4).mean()
     var, _ = O.weight_var(weights, nb)
     var_loss = np.sqrt(var + 1e-2).mean()
     disp_loss = (disp * disp).mean()
     tv = ((edge_feats[:, 0] - edge_feats[:, 1]) ** 2).mean() if n_edge else 0.0
-    out["loss"] = wc * color_loss + wv * var_loss + wd * disp_loss + wt * tv
+    out["loss"] = wc * color_loss + wv * var_loss + wd * disp_loss + wt * tv + wz * (depth * depth).mean()
     if not backward:
         return out
     d_colors = (wc * diff / np.sqrt(diff * diff + 1e-4) / diff.size).astype(np.float32)
     d_var = (wv * 0.5 / np.sqrt(var + 1e-2) / R).astype(np.float32)
     _, d_weights = O.weight_var(weights, nb, d_var)
     d_disp = (wd * 2 * disp / R).astype(np.float32)
+    d_depth = (wz * 2 * depth / R).astype(np.float32) if wz else None
     d_scene = np.zeros((scene_feat.shape[0], 16), np.float32)
     if n_edge:
         de = (wt * 2 * (edge_feats[:, 0] - edge_feats[:, 1]) / (edge_feats.shape[0] * 16)).astype(np.float32)
         d_scene[n_kept:] = np.stack([de, -de], 1).reshape(-1, 16)
-    d_logit, d_rgb = O.composite_bwd(scene_feat[:n_kept], 16, rgb, dt, t, nb, bg, d_colors, d_disp, None, d_weights, gs_progress)
+    d_logit, d_rgb = O.composite_bwd(scene_feat[:n_kept], 16, rgb, dt, t, nb, bg, d_colors, d_disp, d_depth, d_weights, gs_progress)
     d_scene[:n_kept, 0] = d_logit
     # shader backward
     o3 = raw[:, :3].astype(np.float32)

@@ -4,9 +4,11 @@
 // Why: the step would otherwise keep the GPU idle behind the one host sync of
 // Renderer::Render — a Python host needs ~130 foreign calls / allocator calls to enqueue the second half of the step, and
 // the short kernels right after the sync finish faster than it can launch them.  The sequences are fixed, so they live here:
-// one foreign call per phase, the kernels back to back.  No new arithmetic: every launch goes through the entry points
-// declared earlier in the header (same kernels, same order, same streams as f2nerf_b200/renderer.py used to issue one by one);
-// the only kernels of this file are the gradient un-scaling + finiteness flags that replace ~10 ATen passes.
+// one foreign call per phase, the kernels back to back.  This file is the one place that says which kernels make up a TRAIN
+// step, in what order and with what arguments: both hosts — the Python one (f2nerf_b200/renderer.py) and the C++ one
+// (f2nerf_b200/shim/B200Renderer.cpp) — fill `f2b_render` and call these sequences.  No new arithmetic: every launch goes
+// through the entry points declared earlier in the header; the only kernels of this file are the gradient un-scaling +
+// finiteness flags that replace ~10 ATen passes.
 #include "common.cuh"
 
 namespace f2b {

@@ -9,11 +9,13 @@
 // -DRender=RenderReference (its own body stays callable under that name, see RenderReferenceThunk.cpp), this file
 // is compiled without the macro.  Setting F2B_RENDER=reference at run time routes every call back to the reference body.
 //
-// Same pipeline as the Python host mirror (f2nerf_b200/renderer.py), kernel for kernel, through the flat C ABI
-// (include/f2nerf_b200.h): one-pass march into per-ray slots -> early-stop field pass on the slots -> per-ray
-// survivor counts -> ONE host sync -> compaction (samples + their encoded features) -> fused field-MLP / shader-input
-// epilogue -> shader MLP + colour activation -> composite; ONE autograd node carries the whole backward
-// (composite+activation bwd -> shader MLP bwd -> input-assembly bwd -> field MLP bwd -> hash scatter).
+// Which kernels make up a TRAIN step, in what order and with what arguments, is decided in one place: the launch sequences
+// of csrc/render.cu (f2b_render_phase1 / _phase2_fwd / _bwd / _grad_finalize, include/f2nerf_b200.h), which the Python
+// host (f2nerf_b200/renderer.py) calls too.  This file fills their argument block, `f2b_render`, once per call and keeps
+// what only a host can do: the one-pass march into per-ray slots (issued here, because the VALIDATE branch's fused
+// forward needs the slots too), the torch RNG draws, the ONE host sync behind phase 1, the GlobalDataPool EMAs, the
+// octree votes and maintenance, and ONE autograd node that carries the whole backward and reads the per-MLP non-finite
+// flags back for the loss-scale back-off.
 // RNG: the same torch draws in the same order as the reference (noise, background, edge samples) and the Philox
 // offset advanced by what the reference's torch::rand MLP-output buffers (TCNNWP.cpp:143) and GradientScaling's
 // rand_like (CustomOps.cu:154) would have consumed, so a seeded run stays on the reference's random stream.
@@ -56,7 +58,6 @@ void f2b_render_use_reference(bool on) { g_use_reference = on; }
 
 namespace {
 
-constexpr int kSlot = 1024;            // MAX_SAMPLE_PER_RAY (PersSampler.h:9)
 constexpr int kEdgePts = 8192;         // Renderer.cpp:155
 const auto kHalf = torch::TensorOptions().dtype(torch::kFloat16).device(torch::kCUDA);
 const auto kByte = torch::TensorOptions().dtype(torch::kUInt8).device(torch::kCUDA);
@@ -122,7 +123,7 @@ struct Work {
   c10::optional<c10::cuda::CUDAStream> side_votes, side_scatter;
   void ensure(int64_t n_rays, int64_t table_numel) {
     if (n_rays > cap_rays) {
-      const int64_t n = n_rays * kSlot;
+      const int64_t n = n_rays * F2B_MAX_SAMPLE_PER_RAY;
       s_pts = torch::empty({n, 3}, CUDAFloat); s_dt = torch::empty({n}, CUDAFloat); s_t = torch::empty({n}, CUDAFloat);
       s_anchors = torch::empty({n, 2}, CUDAInt);
       logit_s = torch::empty({n}, CUDAFloat); feat_s = torch::empty({n, 32}, kHalf);
@@ -145,17 +146,15 @@ void stream_wait(const c10::cuda::CUDAStream& waiter, const c10::cuda::CUDAStrea
   ev.block(waiter);
 }
 
-// What the second half of Render hands to its autograd node (plain struct; lives in the node through a registry slot).
+// What Render hands to its autograd node: the call's argument block of the launch sequences next to the tensors its pointers
+// refer to (plain struct; lives in the node through a registry slot).
 struct Pack {
   Renderer* renderer = nullptr;
   Hash3DAnchored* field = nullptr;
   SHShader* shader = nullptr;
-  Tensor pts, dirs, dt, t, anchors, bounds, bg, feat16, e_pts, e_anc, pt_emb_idx, ray_emb_idx;
-  int64_t n_kept = 0, n_edge = 0;
+  f2b_render ra{};
+  std::vector<Tensor> keepalive;
   bool grad_on = false;
-  float gs_progress = 1.f;
-  // saved by forward
-  Tensor fparams16, sparams16, logit, mlp_in, raw, rgb;
 };
 std::mutex g_pack_mu;
 std::unordered_map<int64_t, std::shared_ptr<Pack>> g_packs;
@@ -167,34 +166,14 @@ public:
                                int64_t pack_id) {
     std::shared_ptr<Pack> pk;
     { std::lock_guard<std::mutex> l(g_pack_mu); pk = g_packs.at(pack_id); }
-    Pack& k = *pk;
-    const int64_t n_kept = k.n_kept, n_q = k.feat16.size(0);
-    k.fparams16 = torch::empty({field_params.numel()}, kHalf);
-    k.sparams16 = torch::empty({shader_params.numel()}, kHalf);
-    F2B_CHECK(f2b_cast_f32_to_f16(field_params.data_ptr<float>(), P(k.fparams16), field_params.numel(), 1.f, cur_stream()));
-    F2B_CHECK(f2b_cast_f32_to_f16(shader_params.data_ptr<float>(), P(k.sparams16), shader_params.numel(), 1.f, cur_stream()));
-    const bool emb_on = k.pt_emb_idx.defined();
-    k.logit = torch::empty({n_kept}, CUDAFloat);
-    k.mlp_in = torch::empty({n_kept, 32}, kHalf);
-    F2B_CHECK(f2b_field_shade_fwd(P(k.feat16), P(k.fparams16), PF(k.dirs), emb_on ? app_emb.data_ptr<float>() : nullptr,
-                                  emb_on ? PI(k.pt_emb_idx) : nullptr, (int) n_kept, PF(k.logit), P(k.mlp_in), nullptr,
-                                  cur_stream()));
-    Tensor edge32 = torch::empty({n_q - n_kept, 16}, CUDAFloat);
-    if (n_q > n_kept) {
-      F2B_CHECK(f2b_mlp_fwd_f32((char*) P(k.feat16) + n_kept * 64, P(k.fparams16), 0, (int) (n_q - n_kept), PF(edge32), nullptr,
-                                nullptr, cur_stream()));
-    }
-    k.raw = torch::empty({n_kept, 16}, kHalf);
-    k.rgb = torch::empty({n_kept, 3}, CUDAFloat);
-    F2B_CHECK(f2b_shader_mlp_rgb_fwd(P(k.mlp_in), P(k.sparams16), (int) n_kept, P(k.raw), PF(k.rgb), nullptr, cur_stream()));
-    const int n_rays = k.bounds.size(0);
-    Tensor colors = torch::empty({n_rays, 3}, CUDAFloat), disp = torch::empty({n_rays}, CUDAFloat),
-           depth = torch::empty({n_rays}, CUDAFloat), weights = torch::empty({n_kept}, CUDAFloat);
-    F2B_CHECK(f2b_composite_fwd(PF(k.logit), 1, PF(k.rgb), PF(k.dt), PF(k.t), PI(k.bounds), PF(k.bg), n_rays, PF(colors),
-                                PF(disp), PF(depth), PF(weights), cur_stream()));
+    f2b_render& ra = pk->ra;
+    Tensor colors = torch::empty({ra.n_rays, 3}, CUDAFloat), disp = torch::empty({ra.n_rays}, CUDAFloat),
+           depth = torch::empty({ra.n_rays}, CUDAFloat), weights = torch::empty({ra.n_kept}, CUDAFloat),
+           edge32 = torch::empty({2 * int64_t(ra.n_edge_pairs), 16}, CUDAFloat);
+    ra.colors = PF(colors); ra.disparity = PF(disp); ra.depth = PF(depth); ra.weights = PF(weights); ra.edge32 = PF(edge32);
+    F2B_CHECK(f2b_render_phase2_fwd(&ra));
     ctx->saved_data["pack"] = pack_id;
     ctx->saved_data["table_numel"] = feat_pool.numel();
-    ctx->saved_data["n_emb"] = app_emb.size(0);
     return {colors, disp, depth, weights, edge32.reshape({-1, 2, 16})};
   }
 
@@ -211,71 +190,53 @@ public:
     }
     Pack& k = *pk;
     CHECK(k.grad_on) << "Renderer::Render backward: forward ran without grad (VALIDATE mode / NoGradGuard)";
-    const int64_t n_kept = k.n_kept, n_q = k.feat16.size(0);
-    const int n_rays = k.bounds.size(0);
+    f2b_render& ra = k.ra;
     Hash3DAnchored* field = k.field;
     SHShader* shader = k.shader;
-    Tensor d_colors = g[0].defined() ? g[0].contiguous() : torch::zeros({n_rays, 3}, CUDAFloat);
+    Tensor d_colors = g[0].defined() ? g[0].contiguous() : torch::zeros({ra.n_rays, 3}, CUDAFloat);
     Tensor d_disp = g[1].defined() ? g[1].contiguous() : Tensor();
     Tensor d_depth = g[2].defined() ? g[2].contiguous() : Tensor();
     Tensor d_weights = g[3].defined() ? g[3].contiguous() : Tensor();
-    Tensor d_edge = g[4];
-    if (k.gs_progress < 1.f) { burn_rand(n_kept * 3); burn_rand(n_kept); }       // GradientScaling::backward's rand_like
+    Tensor d_edge = g[4].defined() ? g[4].reshape({-1, 16}).contiguous() : Tensor();
+    if (ra.gs_progress < 1.f) { burn_rand(ra.n_kept * 3); burn_rand(ra.n_kept); }  // GradientScaling::backward's rand_like
     const float s_scale = shader->mlp_->loss_scale_, f_scale = field->mlp_->loss_scale_;
-    Tensor d_logit = torch::empty({n_kept}, CUDAFloat);
-    Tensor d_raw = torch::empty({n_kept, 16}, kHalf);
-    Tensor d_edge16 = torch::empty({n_q - n_kept, 16}, kHalf);      // the edge points' field dL/dout rows (the rays' stay on chip)
-    Tensor ticket = torch::empty({1}, CUDAInt);
-    Tensor d_sparams = torch::zeros({k.sparams16.numel()}, CUDAFloat), d_fparams = torch::zeros({k.fparams16.numel()}, CUDAFloat);
+    Tensor d_logit = torch::empty({ra.n_kept}, CUDAFloat);
+    Tensor d_raw = torch::empty({ra.n_kept, 16}, kHalf);
+    Tensor d_edge16 = torch::empty({2 * int64_t(ra.n_edge_pairs), 16}, kHalf);   // the edge points' field dL/dout rows (the rays' stay on chip)
+    Tensor ticket = torch::empty({1}, CUDAInt), nonfinite = torch::empty({2}, CUDAInt);
+    Tensor d_sparams = torch::empty({ra.n_shader_params}, CUDAFloat), d_fparams = torch::empty({ra.n_field_params}, CUDAFloat);
     const int64_t table_numel = ctx->saved_data["table_numel"].toInt();
-    const int local_size = ((field->pool_size_ / N_LEVELS) >> 4) << 4;
-    const int64_t live = std::min<int64_t>(table_numel, int64_t(N_LEVELS + 1) * local_size);     // halves [0, 17 S) are ever addressed
-    // Only floats [0, 17 S) of the gradient are ever written, so its storage is kept across steps and only that live prefix is
-    // zero-filled per backward — unless a tensor on last step's gradient is still alive (a trainer that keeps .grad): then a fresh,
-    // fully zeroed one.  Each backward hands autograd a NEW tensor on the storage, so it becomes .grad without a copy.
+    const int64_t live = std::min<int64_t>(table_numel, int64_t(N_LEVELS + 1) * ra.local_size);  // halves [0, 17 S) are ever addressed
+    // Only floats [0, 17 S) of the gradient are ever written, so its storage is kept across steps and f2b_render_bwd zero-fills only
+    // that live prefix — unless a tensor on last step's gradient is still alive (a trainer that keeps .grad): then a fresh one,
+    // zero-filled as a whole.  Each backward hands autograd a NEW tensor on the storage, so it becomes .grad without a copy.
     Work& wk = work_of(k.renderer);
     Tensor d_table;
     if (wk.d_table_storage && wk.d_table_storage.nbytes() == size_t(table_numel) * 4 && wk.d_table_storage.use_count() == 1) {
       d_table = torch::empty({0}, CUDAFloat).set_(wk.d_table_storage, 0, {table_numel / 2, 2});
-      d_table.view({-1}).slice(0, 0, live).zero_();
+      ra.table_numel = live;
       ++g_grad_reused;
     } else {
-      d_table = torch::zeros({table_numel / 2, 2}, CUDAFloat);
+      d_table = torch::empty({table_numel / 2, 2}, CUDAFloat);
       wk.d_table_storage = d_table.storage();
+      ra.table_numel = table_numel;
       ++g_grad_fresh;
     }
-    const bool emb_on = k.ray_emb_idx.defined();
-    Tensor d_app = emb_on ? torch::zeros({ctx->saved_data["n_emb"].toInt(), 16}, CUDAFloat) : Tensor();
-    if (n_q > n_kept) {
-      if (d_edge.defined()) d_edge16.copy_((d_edge.reshape({-1, 16}) * f_scale).to(torch::kFloat16));
-      else d_edge16.zero_();
-    }
-    F2B_CHECK(f2b_composite_act_bwd(PF(k.logit), 1, PF(k.rgb), PF(k.dt), PF(k.t), PI(k.bounds), PF(k.bg), n_rays, PF(d_colors),
-                                    PF(d_disp), PF(d_depth), PF(d_weights), k.gs_progress, P(k.raw), s_scale, PF(d_logit), 1,
-                                    P(d_raw), cur_stream()));
-    // as f2b_render_bwd issues them: the ray samples' shader-MLP, input-assembly and field-MLP backward with their hash scatter in
-    // one kernel (activations rebuilt from the input rows), then the TV-loss edge points' field-MLP backward + scatter
-    F2B_CHECK(f2b_shade_field_bwd_scatter(P(d_raw), P(k.mlp_in), P(k.sparams16), PF(d_logit), emb_on ? PI(k.pt_emb_idx) : nullptr,
-                                          1.f / s_scale, f_scale, P(k.feat16), P(k.fparams16), (int) n_kept, PF(k.pts), PI(k.anchors), 3,
-                                          field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_,
-                                          local_size, 1.f / f_scale, PF(d_sparams), PF(d_fparams), PF(d_table), PF(d_app), PI(ticket),
-                                          nullptr, nullptr, nullptr, cur_stream()));
-    if (n_q > n_kept) {
-      F2B_CHECK(f2b_field_bwd_scatter(P(d_edge16), (char*) P(k.feat16) + n_kept * 64, P(k.fparams16),
-                                      (int) (n_q - n_kept), PF(k.e_pts), PI(k.e_anc), 1, field->prim_pool_.data_ptr<int>(),
-                                      field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size, 1.f / f_scale, PF(d_fparams),
-                                      PF(d_table), nullptr, cur_stream()));
-    }
-    d_sparams = d_sparams / s_scale;
-    d_fparams = d_fparams / f_scale;
-    // NaN back-off of TCNNWPFunction::backward (TCNNWP.cpp:231-240), per MLP, dL/dparams and dL/dinput (through what the input
-    // gradients feed: d_app / the table gradient).  ExpRunner reads backward_nan_ right after loss.backward(): one host sync.
-    Tensor ok_s = torch::isfinite(d_sparams).all();
-    if (emb_on) ok_s = ok_s & torch::isfinite(d_app).all();
-    Tensor ok_f = torch::isfinite(d_fparams).all() & torch::isfinite(d_table.view({-1}).slice(0, 0, live)).all();
-    Tensor flags = torch::stack({ok_s, ok_f}).to(torch::kCPU);
-    if (!flags[0].item<bool>()) { shader->global_data_pool_->backward_nan_ = true; shader->mlp_->loss_scale_ = std::max(s_scale / 2.f, 1.f); }
-    if (!flags[1].item<bool>()) { field->global_data_pool_->backward_nan_ = true; field->mlp_->loss_scale_ = std::max(f_scale / 2.f, 1.f); }
+    const bool emb_on = ra.ray_emb_idx != nullptr;
+    Tensor d_app = emb_on ? torch::empty({ra.n_emb, 16}, CUDAFloat) : Tensor();
+    ra.d_colors = PF(d_colors); ra.d_disparity = PF(d_disp); ra.d_depth = PF(d_depth); ra.d_weights = PF(d_weights); ra.d_edge = PF(d_edge);
+    ra.shader_loss_scale = s_scale; ra.field_loss_scale = f_scale; ra.table_grad_mul = 1.f / f_scale;
+    ra.d_logit = PF(d_logit); ra.d_raw = P(d_raw); ra.d_scene16 = P(d_edge16);
+    ra.d_sparams = PF(d_sparams); ra.d_fparams = PF(d_fparams); ra.d_table = PF(d_table); ra.table_live = live; ra.d_app = PF(d_app);
+    ra.nonfinite = PI(nonfinite); ra.tile_ticket = PI(ticket);
+    ra.stream = cur_stream();
+    F2B_CHECK(f2b_render_bwd(&ra));
+    F2B_CHECK(f2b_render_grad_finalize(&ra));
+    // NaN back-off of TCNNWPFunction::backward (TCNNWP.cpp:231-240), per MLP, on the flags f2b_render_grad_finalize raised (dL/dparams,
+    // and dL/dinput through d_app / the table gradient).  ExpRunner reads backward_nan_ right after loss.backward(): one host sync.
+    Tensor flags = nonfinite.to(torch::kCPU);
+    if (flags[0].item<int>()) { shader->global_data_pool_->backward_nan_ = true; shader->mlp_->loss_scale_ = std::max(s_scale / 2.f, 1.f); }
+    if (flags[1].item<int>()) { field->global_data_pool_->backward_nan_ = true; field->mlp_->loss_scale_ = std::max(f_scale / 2.f, 1.f); }
     return {d_table, d_fparams, d_sparams, emb_on ? d_app : Tensor(), Tensor()};
   }
 };
@@ -302,12 +263,12 @@ RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw
   const bool caller_grad = torch::GradMode::is_enabled();                       // ExpRunner's validation paths run under NoGradGuard
   torch::NoGradGuard no_grad;                                                    // everything up to the autograd node is grad-free
 
-  // ---- phase 1: march -> early-stop field pass -> survivor counts, all in the march's slot layout ----------------------
+  // ---- march -> phase 1 (early-stop field pass -> survivor counts), all in the march's slot layout --------------------
   Tensor rays_o = rays_o_raw.contiguous();
   Tensor rays_d = (rays_d_raw / torch::linalg_norm(rays_d_raw, 2, -1, true)).contiguous();
   Tensor noise;                                                                  // PersSampler.cu:373-381
-  if (gdp->mode_ == RunningMode::VALIDATE) noise = torch::ones({kSlot + n_rays + 10}, CUDAFloat);
-  else noise = ((torch::rand({kSlot + n_rays + 10}, CUDAFloat) - .5f) + 1.f).contiguous();
+  if (gdp->mode_ == RunningMode::VALIDATE) noise = torch::ones({F2B_MAX_SAMPLE_PER_RAY + n_rays + 10}, CUDAFloat);
+  else noise = ((torch::rand({F2B_MAX_SAMPLE_PER_RAY + n_rays + 10}, CUDAFloat) - .5f) + 1.f).contiguous();
   noise.mul_(gdp->ray_march_fineness_);
   Tensor bg;                                                                     // Renderer.cpp:67-81
   if (bg_color_type_ == BGColorType::white) bg = torch::ones({n_rays, 3}, CUDAFloat);
@@ -321,8 +282,7 @@ RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw
   const int64_t live = std::min<int64_t>(field->feat_pool_.numel(), int64_t(N_LEVELS + 1) * local_size);
   // fp16 shadow of the live prefix of the table (the reference re-casts all of it on every AnchoredQuery, Hash3DAnchored.cu:186)
   F2B_CHECK(f2b_table_to_half(field->feat_pool_.data_ptr<float>(), P(w.table16), live, cur_stream()));
-  Tensor fparams16 = torch::empty({field->mlp_->params_.numel()}, kHalf);
-  F2B_CHECK(f2b_cast_f32_to_f16(field->mlp_->params_.data_ptr<float>(), P(fparams16), fparams16.numel(), 1.f, cur_stream()));
+  Tensor fparams16 = torch::empty({field->mlp_->params_.numel()}, kHalf), sparams16 = torch::empty({shader->mlp_->params_.numel()}, kHalf);
   Tensor counts = torch::empty({n_rays}, CUDAInt), chunk_bounds = torch::empty({n_rays, 2}, CUDAInt);
   Tensor slot_bounds = torch::empty({n_rays, 2}, CUDAInt), first_oct_dis = torch::empty({n_rays, 1}, CUDAFloat);
   Tensor heads = torch::empty({3}, CUDAInt);                                    // [n_kept, n_all, n_all_oct]
@@ -331,18 +291,18 @@ RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw
                               sampler->global_near_, 1e8f, sampler->sample_l_, sampler->scale_by_dis_ ? 1 : 0,
                               sampler->max_oct_intersect_per_ray_, /*count_all_hits=*/0, PF(w.s_pts), PF(w.s_dt), PF(w.s_t), PI(w.s_anchors),
                               PI(counts), PI(chunk_bounds), PI(heads) + 1, PF(first_oct_dis), cur_stream()));
-  F2B_CHECK(f2b_slot_bounds(PI(counts), n_rays, kSlot, 0, PI(slot_bounds), cur_stream()));
+  F2B_CHECK(f2b_slot_bounds(PI(counts), n_rays, F2B_MAX_SAMPLE_PER_RAY, 0, PI(slot_bounds), cur_stream()));
   if (!train && fused_forward()) {
     // VALIDATE (ExpRunner::RenderWholeImage / TestImages under NoGradGuard): no gradient, no occupancy votes, no TV-loss edge points.
     // Everything behind the march is ONE kernel walking each ray front to back — encode -> field MLP -> early stop -> SH + shader MLP
-    // -> composite — that stops at the first opaque sample (csrc/fused_fwd.cu); values bit-identical to the operator sequence below.
-    Tensor sparams16 = torch::empty({shader->mlp_->params_.numel()}, kHalf);
+    // -> composite — that stops at the first opaque sample (csrc/fused_fwd.cu); values bit-identical to the launch sequences below.
+    F2B_CHECK(f2b_cast_f32_to_f16(field->mlp_->params_.data_ptr<float>(), P(fparams16), fparams16.numel(), 1.f, cur_stream()));
     F2B_CHECK(f2b_cast_f32_to_f16(shader->mlp_->params_.data_ptr<float>(), P(sparams16), sparams16.numel(), 1.f, cur_stream()));
     Tensor colors = torch::empty({n_rays, 3}, CUDAFloat), disp = torch::empty({n_rays}, CUDAFloat), depth = torch::empty({n_rays}, CUDAFloat);
     Tensor kept = torch::empty({n_rays}, CUDAInt), ticket = torch::empty({1}, CUDAInt);
     F2B_CHECK(f2b_render_fwd_fused(P(w.table16), field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_,
                                    local_size, P(fparams16), P(sparams16), PF(w.s_pts), PF(w.s_dt), PF(w.s_t), PI(w.s_anchors), PI(counts),
-                                   PF(rays_d), PF(bg), n_rays, kSlot, PI(heads) + 1, PI(ticket), PF(colors), PF(disp), PF(depth), PI(kept),
+                                   PF(rays_d), PF(bg), n_rays, F2B_MAX_SAMPLE_PER_RAY, PI(heads) + 1, PI(ticket), PF(colors), PF(disp), PF(depth), PI(kept),
                                    PF(w.w0), cur_stream()));
     sample_result_ = SampleResultFlex();
     sample_result_.first_oct_dis = first_oct_dis;
@@ -356,17 +316,34 @@ RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw
     sample_result_.pts = torch::empty({n_all, 0}, CUDAFloat);
     if (n_all > 0) { burn_mlp_output(n_all); burn_mlp_output(n_kept); burn_mlp_output(n_kept); }   // the three TCNNWP::Query outputs (rng parity)
     Tensor weights = torch::empty({n_kept}, CUDAFloat);
-    if (n_kept > 0) F2B_CHECK(f2b_gather_kept_weights(PF(w.w0), PI(new_bounds), n_rays, kSlot, PF(weights), cur_stream()));
+    if (n_kept > 0) F2B_CHECK(f2b_gather_kept_weights(PF(w.w0), PI(new_bounds), n_rays, F2B_MAX_SAMPLE_PER_RAY, PF(weights), cur_stream()));
     if (n_all <= 0) return {bg, torch::zeros({n_rays, 1}, CUDAFloat), torch::zeros({n_rays}, CUDAFloat), Tensor(), torch::full({n_rays}, 512.f, CUDAFloat), Tensor(), Tensor()};
     return {colors, first_oct_dis, disp, Tensor(), depth, weights, new_bounds};
   }
-  F2B_CHECK(f2b_field_fwd_slots(P(w.table16), field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_,
-                                local_size, P(fparams16), PF(w.s_pts), PI(w.s_anchors), 2, PI(counts), n_rays, kSlot, 1, PF(w.logit_s),
-                                P(w.feat_s), cur_stream()));
-  F2B_CHECK(f2b_early_stop_rays(PF(w.logit_s), 1, PF(w.s_dt), PI(slot_bounds), n_rays, PF(w.w0), PF(w.a0), w.keep.data_ptr<uint8_t>(),
-                                PI(w.kept_counts), cur_stream()));
+  // TRAIN (and VALIDATE under F2B_FUSED_FORWARD=0): the launch sequences of csrc/render.cu on one argument block, filled as
+  // f2nerf_b200/renderer.py fills it.  The slots are marched above, so phase 1 starts at the field-parameter cast.
   Tensor new_bounds = torch::empty({n_rays, 2}, CUDAInt);
-  F2B_CHECK(f2b_count_scan(PI(w.kept_counts), n_rays, PI(new_bounds), PI(heads), cur_stream()));
+  auto pk = std::make_shared<Pack>();
+  Pack& k = *pk;
+  k.renderer = this; k.field = field; k.shader = shader;
+  f2b_render& ra = k.ra;
+  ra.tree_nodes = P(oct.tree_nodes_gpu_); ra.n_nodes = n_nodes; ra.trans = P(oct.pers_trans_gpu_); ra.n_trans = n_trans;
+  ra.edge_pool = P(oct.edge_pool_gpu_);
+  ra.near_t = sampler->global_near_; ra.far_t = 1e8f; ra.sample_l = sampler->sample_l_; ra.scale_by_dis = sampler->scale_by_dis_ ? 1 : 0;
+  ra.max_hits = sampler->max_oct_intersect_per_ray_; ra.count_all_hits = 0;
+  ra.table16 = P(w.table16); ra.prim = field->prim_pool_.data_ptr<int>(); ra.bias = field->bias_pool_.data_ptr<float>();
+  ra.n_volumes = field->n_volumes_; ra.local_size = local_size;
+  ra.field_params = field->mlp_->params_.data_ptr<float>(); ra.n_field_params = fparams16.numel();
+  ra.shader_params = shader->mlp_->params_.data_ptr<float>(); ra.n_shader_params = sparams16.numel();
+  ra.fparams16 = P(fparams16); ra.sparams16 = P(sparams16);
+  ra.n_rays = n_rays; ra.rays_o = PF(rays_o); ra.rays_d = PF(rays_d); ra.noise = PF(noise); ra.bg = PF(bg);
+  ra.skip_march = 1;
+  ra.s_pts = PF(w.s_pts); ra.s_dt = PF(w.s_dt); ra.s_t = PF(w.s_t); ra.s_anchors = PI(w.s_anchors); ra.counts = PI(counts);
+  ra.chunk_bounds = PI(chunk_bounds); ra.slot_bounds = PI(slot_bounds); ra.first_oct_dis = PF(first_oct_dis); ra.totals = PI(heads) + 1;
+  ra.logit_s = PF(w.logit_s); ra.feat_s = P(w.feat_s); ra.w0 = PF(w.w0); ra.a0 = PF(w.a0); ra.keep = w.keep.data_ptr<uint8_t>();
+  ra.kept_counts = PI(w.kept_counts); ra.new_bounds = PI(new_bounds); ra.total_kept = PI(heads);
+  ra.stream = cur_stream();
+  F2B_CHECK(f2b_render_phase1(&ra));
   Tensor heads_cpu = heads.to(torch::kCPU);                                      // THE host sync of the step
   const int64_t n_kept = heads_cpu[0].item<int>(), n_all = heads_cpu[1].item<int>(), n_all_oct = heads_cpu[2].item<int>();
   if (gdp->mode_ != RunningMode::VALIDATE)                                       // PersSampler.cu:378-379
@@ -427,37 +404,34 @@ RenderResult Renderer::Render(const Tensor& rays_o_raw, const Tensor& rays_d_raw
     gdp->meaningful_sampled_pts_per_ray_ = gdp->meaningful_sampled_pts_per_ray_ * .9f + (float(n_kept) / float(n_rays)) * .1f;
   }
 
-  // ---- phase 2 inputs: compaction of the survivors (samples + their encoded features), TV-loss edge points ------------
-  auto pk = std::make_shared<Pack>();
-  Pack& k = *pk;
-  k.renderer = this; k.field = field; k.shader = shader;
-  const int64_t n_edge = train ? 2 * kEdgePts : 0;
-  k.n_kept = n_kept; k.n_edge = n_edge;
-  k.feat16 = torch::empty({n_kept + n_edge, 32}, kHalf);
-  k.pts = torch::empty({n_kept, 3}, CUDAFloat); k.dirs = torch::empty({n_kept, 3}, CUDAFloat);
-  k.dt = torch::empty({n_kept}, CUDAFloat); k.t = torch::empty({n_kept}, CUDAFloat); k.anchors = torch::empty({n_kept, 3}, CUDAInt);
-  k.bounds = new_bounds; k.bg = bg;
-  F2B_CHECK(f2b_compact_slots(w.keep.data_ptr<uint8_t>(), PI(slot_bounds), PI(new_bounds), n_rays, PF(rays_d), PF(w.s_pts), PF(w.s_dt),
-                              PF(w.s_t), PI(w.s_anchors), P(w.feat_s), PF(k.pts), PF(k.dirs), PF(k.dt), PF(k.t), PI(k.anchors), P(k.feat16),
-                              cur_stream()));
+  // ---- phase 2: buffers of the survivors and the TV-loss edge points; the autograd node enqueues f2b_render_phase2_fwd ------
+  const int n_pairs = train ? kEdgePts : 0;
+  const int64_t n_edge = 2 * int64_t(n_pairs);
+  Tensor pts = torch::empty({n_kept, 3}, CUDAFloat), dirs = torch::empty({n_kept, 3}, CUDAFloat), dt = torch::empty({n_kept}, CUDAFloat),
+         t = torch::empty({n_kept}, CUDAFloat), anchors = torch::empty({n_kept, 3}, CUDAInt), feat_q = torch::empty({n_kept + n_edge, 32}, kHalf),
+         logit = torch::empty({n_kept}, CUDAFloat), mlp_in = torch::empty({n_kept, 32}, kHalf), raw = torch::empty({n_kept, 16}, kHalf),
+         rgb = torch::empty({n_kept, 3}, CUDAFloat);
+  ra.n_kept = n_kept; ra.n_edge_pairs = n_pairs;
+  ra.pts = PF(pts); ra.dirs = PF(dirs); ra.dt = PF(dt); ra.t = PF(t); ra.anchors = PI(anchors); ra.feat_q = P(feat_q);
+  ra.logit = PF(logit); ra.mlp_in = P(mlp_in); ra.raw = P(raw); ra.rgb = PF(rgb);
+  Tensor edge_idx, edge_coord, e_pts, e_anc, ray_emb_idx, pt_emb_idx;
   if (train) {
     const int n_edges = oct.edge_pool_.size();
-    Tensor edge_idx = torch::randint(0, n_edges, {kEdgePts}, CUDAInt).contiguous();                 // PersSampler.cu:456-457
-    Tensor edge_coord = (torch::rand({kEdgePts, 2}, CUDAFloat) * 2.f - 1.f).contiguous();
-    k.e_pts = torch::empty({kEdgePts * 2, 3}, CUDAFloat); k.e_anc = torch::empty({kEdgePts * 2}, CUDAInt);
-    F2B_CHECK(f2b_edge_samples(P(oct.edge_pool_gpu_), P(oct.pers_trans_gpu_), PI(edge_idx), PF(edge_coord), kEdgePts, PF(k.e_pts), PI(k.e_anc),
-                               cur_stream()));
-    F2B_CHECK(f2b_hash_fwd(P(w.table16), field->prim_pool_.data_ptr<int>(), field->bias_pool_.data_ptr<float>(), field->n_volumes_, local_size,
-                           PF(k.e_pts), PI(k.e_anc), 1, (int) n_edge, (char*) P(k.feat16) + n_kept * 64, cur_stream()));
+    edge_idx = torch::randint(0, n_edges, {n_pairs}, CUDAInt).contiguous();                          // PersSampler.cu:456-457
+    edge_coord = (torch::rand({n_pairs, 2}, CUDAFloat) * 2.f - 1.f).contiguous();
+    e_pts = torch::empty({n_edge, 3}, CUDAFloat); e_anc = torch::empty({n_edge}, CUDAInt);
+    ra.edge_idx = PI(edge_idx); ra.edge_coord = PF(edge_coord); ra.e_pts = PF(e_pts); ra.e_anc = PI(e_anc);
   }
   burn_mlp_output(n_kept + n_edge);                                              // second AnchoredQuery (Renderer.cpp:165/172) ...
   burn_mlp_output(n_kept);                                                       // ... and the shader MLP (SHShader.cpp:27)
   if (train && use_app_emb_) {
-    k.ray_emb_idx = emb_idx.to(torch::kInt32).contiguous();
-    k.pt_emb_idx = torch::empty({n_kept}, CUDAInt);
-    F2B_CHECK(f2b_scatter_idx(PI(new_bounds), PI(k.ray_emb_idx), n_rays, PI(k.pt_emb_idx), cur_stream()));
+    ray_emb_idx = emb_idx.to(torch::kInt32).contiguous();
+    pt_emb_idx = torch::empty({n_kept}, CUDAInt);
+    ra.app_emb = app_emb_.data_ptr<float>(); ra.n_emb = app_emb_.size(0); ra.ray_emb_idx = PI(ray_emb_idx); ra.pt_emb_idx = PI(pt_emb_idx);
   }
-  k.gs_progress = gdp->gradient_scaling_progress_;
+  ra.gs_progress = gdp->gradient_scaling_progress_;
+  k.keepalive = {rays_o, rays_d, noise, bg, counts, chunk_bounds, slot_bounds, first_oct_dis, heads, new_bounds, fparams16, sparams16,
+                 pts, dirs, dt, t, anchors, feat_q, logit, mlp_in, raw, rgb, edge_idx, edge_coord, e_pts, e_anc, ray_emb_idx, pt_emb_idx};
   k.grad_on = caller_grad && train;
   int64_t id;
   {

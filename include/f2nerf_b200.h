@@ -381,13 +381,14 @@ int f2b_weight_var_bwd(const float* weights, const int* idx_start_end, int n_out
                        float* dl_dw, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Renderer::Render (src/Renderer/Renderer.cpp:52-213) as THREE launch sequences — what the host mirrors call per batch.
+ * Renderer::Render (src/Renderer/Renderer.cpp:52-213) as THREE launch sequences — what both hosts call per TRAIN batch: the
+ * Python host (f2nerf_b200/renderer.py) and the C++ host inside the reference's program (f2nerf_b200/shim/B200Renderer.cpp).
  * Each entry point enqueues the fixed kernel sequence of one phase of the fused pipeline (the very kernels declared above,
  * same order, same streams) in ONE call, so that a scripting-language host pays one foreign call per phase instead of one
- * per kernel; nothing is allocated, every buffer (and the two streams) comes from the caller in `f2b_render`.  Fields a
- * phase does not use may be left NULL / 0.  The host keeps what only it can do: the torch RNG draws (noise, background,
- * edge indices / coordinates), the ONE host sync between phase 1 and phase 2 (n_kept sizes the survivors' buffers),
- * the GlobalDataPool EMAs and the autograd plumbing.
+ * per kernel, and which kernels make up a step is written down once; nothing is allocated, every buffer (and the two streams)
+ * comes from the caller in `f2b_render`.  Fields a phase does not use may be left NULL / 0.  The host keeps what only it can
+ * do: the torch RNG draws (noise, background, edge indices / coordinates), the ONE host sync between phase 1 and phase 2
+ * (n_kept sizes the survivors' buffers), the GlobalDataPool EMAs, the octree votes and maintenance, and the autograd plumbing.
  *   f2b_render_phase1      [march + slot bounds unless skip_march] -> field-parameter cast -> early-stop field pass on the
  *                          slots -> per-ray early stop -> survivor count scan                    (Renderer.cpp:52-126)
  *   f2b_render_phase2_fwd  compaction -> [TRAIN: edge points + their encode] -> point->camera index -> parameter casts ->

@@ -17,6 +17,11 @@ b. The fused host and the operator shim (F2B_SHIM=ops) against the unmodified pr
 c. Each case asserts that it covered what it is for: compaction at iteration 0 and renumbering later, leaves split on each
    milestone (one of them a compaction iteration too), the batch size falling at least once, gradient-scaling progress
    crossing 1, and the C++ host's table-gradient storage reused across steps.
+d. The non-finite back-off, on a copy of the config with an infinite TV-loss weight (three iterations, fixed batch): the TV
+   term makes the edge points' dL/dout non-finite, which reaches the field MLP only.  So under TCNNWP.cpp:231-240 every
+   iteration sets backward_nan_ (no Adam step, iter_step_ stays 0) and halves the field loss scale, 128 -> 64 -> 32, while
+   the shader's stays 128 — in the unmodified program, on the C++ host (the flags of its gradient-finalize kernels) and on
+   the Python host (check_backward_nan) replaying iteration 0 from the C++ run's state.
 """
 import json
 import os
@@ -50,26 +55,28 @@ def _load_dir(d):
     return {f[:-4]: np.load(os.path.join(d, f)) for f in os.listdir(d) if f.endswith(".npy")}
 
 
-def _run(kind, fixed_batch):
-    """``ref_driver --steps`` of one arm: "ref" (unmodified), "fused" (the C++ host) or "ops" (the operator shim)"""
-    key = (kind, fixed_batch)
+def _run(kind, fixed_batch, config=CONFIG, n_iters=N_ITERS):
+    """``ref_driver --steps`` of one arm: "ref" (unmodified), "fused" (the C++ host) or "ops" (the operator shim), on ``config``
+    (its paths are relative to the repository root, where the program runs)"""
+    key = (kind, fixed_batch, config, n_iters)
     if key in _runs:
         return _runs[key]
     binary = REF if kind == "ref" else B200
     if not os.path.exists(binary):
         pytest.skip(f"{binary} not built (oracle/Makefile.ref)")
-    out = os.path.join(tempfile.gettempdir(), f"f2b_cpp_host_steps_{kind}_{fixed_batch}")
+    tag = f"{kind}_{fixed_batch}" + ("" if config == CONFIG else "_" + os.path.splitext(os.path.basename(config))[0])
+    out = os.path.join(tempfile.gettempdir(), f"f2b_cpp_host_steps_{tag}")
     shutil.rmtree(out, ignore_errors=True)
     env = {k: v for k, v in os.environ.items() if k not in ("F2B_SHIM", "F2B_RENDER")}
     if kind == "ops":
         env["F2B_SHIM"] = "ops"
-    r = subprocess.run([binary, "--steps", CONFIG, out, str(N_ITERS), str(fixed_batch)], cwd=ROOT, capture_output=True, text=True,
+    r = subprocess.run([binary, "--steps", config, out, str(n_iters), str(fixed_batch)], cwd=ROOT, capture_output=True, text=True,
                        timeout=900, env=env)
-    open(diag_path(f"cpp_host_steps_{kind}_{fixed_batch}.log"), "w").write(r.stdout[-20000:] + "\n--- stderr ---\n" + r.stderr[-20000:])
+    open(diag_path(f"cpp_host_steps_{tag}.log"), "w").write(r.stdout[-20000:] + "\n--- stderr ---\n" + r.stderr[-20000:])
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
     if kind != "ref":
         assert ("replaced by the B200 subclasses" if kind == "ops" else "replaced by the fused B200 host") in r.stdout
-    run = dict(root=_load_dir(out), its=[_load_dir(os.path.join(out, f"it{k}")) for k in range(N_ITERS)])
+    run = dict(root=_load_dir(out), its=[_load_dir(os.path.join(out, f"it{k}")) for k in range(n_iters)])
     shutil.rmtree(out, ignore_errors=True)
     _runs[key] = run
     return run
@@ -95,10 +102,18 @@ def bits(a):
     return a.view(np.uint32) if a.dtype == np.float32 else a
 
 
+def ray_generator(root):
+    from f2nerf_b200 import RayGenerator
+    h, w = int(root["ds_hw"][0]), int(root["ds_hw"][1])
+    return RayGenerator(root["ds_poses"].reshape(-1, 3, 4), root["ds_intri"].reshape(-1, 3, 3), root["ds_dist_params"], root["ds_bounds"],
+                        images=None, height=h, width=w, train_set=root["ds_train_set"].tolist())
+
+
 def python_step(root, it, k, gen):
-    """Render + loss + backward of iteration k on the Python host, from the C++ run's dumped starting state"""
+    """Render + loss + backward of iteration k on the Python host, from the C++ run's dumped starting state (the caller then
+    reads the non-finite flags: check_nonfinite)"""
     from test_ref_parity import build_from_ref
-    from f2nerf_b200 import TRAIN, CustomOps, check_backward_nan
+    from f2nerf_b200 import TRAIN, CustomOps
     st = it["state"]
     gdp, sampler, field, shader, renderer = build_from_ref(root)
     field.feat_pool_.data.copy_(T(it["feat_pool"]))
@@ -127,8 +142,13 @@ def python_step(root, it, k, gen):
     loss = (torch.sqrt((r.colors - gt) ** 2 + 1e-4).mean() + torch.sqrt(CustomOps.WeightVar(r.weights, r.idx_start_end) + 1e-2).mean() * w_var
             + (r.disparity ** 2).mean() * w_disp + ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean() * w_tv)
     loss.backward()
-    assert not check_backward_nan(renderer) and it["after"][4] == 0
     return (gdp, sampler, field, shader, renderer), r, loss.detach()
+
+
+def check_nonfinite(renderer, it, nonfinite):
+    """The Python host's non-finite back-off (check_backward_nan) fired iff ``nonfinite``, as the C++ run's backward_nan_ did"""
+    from f2nerf_b200 import check_backward_nan
+    assert check_backward_nan(renderer) == nonfinite and it["after"][4] == int(nonfinite)
 
 
 def rel_l2(a, b):
@@ -141,6 +161,7 @@ def replay(root, it, k, gen):
     compact_freq = int(root["run"][0])
     st = it["state"]
     (gdp, sampler, field, shader, renderer), r, loss = python_step(root, it, k, gen)
+    check_nonfinite(renderer, it, False)
     n_rays = int(st[1])
     voted_visits = N(sampler.tree_visit_cnt_)
     sampler.maintain((root["oct_intri"].reshape(-1, 3, 3), root["oct_w2c"].reshape(-1, 3, 4), root["oct_bound"]), compact_freq)
@@ -162,6 +183,7 @@ def replay(root, it, k, gen):
         # iteration once more on the Python host measures that noise, and the C++ host may differ by no more than a few times it
         # (a stale or wrongly zeroed gradient storage differs by O(1)).
         objs2, _, _ = python_step(root, it, k, gen)
+        check_nonfinite(objs2[4], it, False)
         noise = rel_l2(N(objs2[2].feat_pool_.grad), N(field.feat_pool_.grad))
     for name, v in rel.items():
         bar = max(1e-5, 4 * noise) if (name == "feat_pool" and noise is not None) else 1e-5
@@ -183,12 +205,9 @@ def replay(root, it, k, gen):
 
 def test_fused_cpp_host_equals_python_host_each_iteration():
     """a. and c. of the module text"""
-    from f2nerf_b200 import RayGenerator
     run = _run("fused", 0)
     root = run["root"]
-    h, w = int(root["ds_hw"][0]), int(root["ds_hw"][1])
-    gen = RayGenerator(root["ds_poses"].reshape(-1, 3, 4), root["ds_intri"].reshape(-1, 3, 3), root["ds_dist_params"], root["ds_bounds"],
-                       images=None, height=h, width=w, train_set=root["ds_train_set"].tolist())
+    gen = ray_generator(root)
     recs = []
     try:
         for k, it in enumerate(run["its"]):
@@ -234,3 +253,27 @@ def test_hosts_against_unmodified_program(kind):
     assert max(m["loss_rel"] for m in margins) <= LOSS_REL_BAR, margins
     assert sum(m["maintenance"] for m in margins) >= 4, margins
     assert max(m["nodes_rel"] for m in margins if m["maintenance"]) <= NODES_REL_BAR, margins
+
+
+def test_nonfinite_backward_backs_off_the_field_loss_scale(tmp_path):
+    """d. of the module text"""
+    text = open(CONFIG).read()
+    assert "  tv_loss_weight: 0.1\n" in text
+    config = str(tmp_path / "ref_config_ngp_fox_steps_tv_inf.yaml")
+    open(config, "w").write(text.replace("  tv_loss_weight: 0.1\n", "  tv_loss_weight: .inf\n"))
+    seqs = {}
+    for kind in ("ref", "fused"):
+        its = _run(kind, FIXED_BATCH, config, 3)["its"]
+        assert all(np.isinf(it["state"][11]) for it in its), kind                  # the case covered what it is for
+        # per iteration: iter_step before / after, backward_nan_ skip, Adam step taken, field / shader loss scale
+        seqs[kind] = [(int(it["state"][0]), int(it["after"][0]), int(it["after"][4]), int(it["after"][7]), float(it["state"][4]),
+                       float(it["state"][5])) for it in its]
+        assert seqs[kind] == [(0, 0, 1, 0, 128., 128.), (0, 0, 1, 0, 64., 128.), (0, 0, 1, 0, 32., 128.)], (kind, seqs[kind])
+    assert seqs["fused"] == seqs["ref"]
+    # the Python host from the C++ run's state at iteration 0: the same flags, the same two loss scales afterwards
+    run = _run("fused", FIXED_BATCH, config, 3)
+    (gdp, _, field, shader, renderer), _, _ = python_step(run["root"], run["its"][0], 0, ray_generator(run["root"]))
+    check_nonfinite(renderer, run["its"][0], True)
+    assert gdp.backward_nan_
+    assert (field.mlp_.loss_scale_, shader.mlp_.loss_scale_) == tuple(run["its"][1]["state"][4:6].tolist()), (
+        field.mlp_.loss_scale_, shader.mlp_.loss_scale_)

@@ -12,12 +12,12 @@ OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp
      tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py tests/test_gpu_train_maintenance.py
      tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
-      --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
+      --ignore=tests/test_gpu_mlp_fwd_reference.py --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
       --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py --ignore=tests/test_gpu_grad_autograd.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py
-  echo tests/test_ref_parity.py
+  echo tests/test_gpu_mlp_fwd_reference.py; echo tests/test_ref_parity.py
   exit 0
 fi
 O=${O:-ci_logs}
@@ -36,6 +36,9 @@ echo "--- tests/test_gpu_bwd_reference.py"; tail -n 40 $O/pytest_bwd_reference.l
 # the slot-layout forward kernels and the fused forward renderer against the CPU oracle (planned ray lengths and early stops)
 timeout 900 python -m pytest tests/test_gpu_fwd_reference.py -m gpu -q -p no:cacheprovider --durations=10 > $O/pytest_fwd_reference.log 2>&1
 echo "--- tests/test_gpu_fwd_reference.py"; tail -n 40 $O/pytest_fwd_reference.log | cut -c1-250
+# the packed tensor-core forwards, their epilogues and the casts against float64 / ATen references (tensor-core kernels: own process)
+timeout 900 python -m pytest tests/test_gpu_mlp_fwd_reference.py -m gpu -q -p no:cacheprovider --durations=10 > $O/pytest_mlp_fwd_reference.log 2>&1
+echo "--- tests/test_gpu_mlp_fwd_reference.py"; tail -n 40 $O/pytest_mlp_fwd_reference.log | cut -c1-250
 timeout 600 python -m pytest tests/test_ref_parity.py -m gpu -q -p no:cacheprovider > $O/pytest_ref.log 2>&1
 tail -n 60 $O/pytest_ref.log
 if [ "${SANITIZE:-0}" = "1" ]; then

@@ -225,7 +225,8 @@ def field_forward(field, table16, params16, points, anchors, anchor_stride, save
 
 
 def field_backward(field, params16, points, anchors, anchor_stride, feat16, hidden, d_out_f32):
-    """dL/d out [n,16] fp32 -> (dL/d feat_pool fp32 [pool,2], dL/d mlp params fp32)."""
+    """dL/d out [n,16] fp32 -> (dL/d feat_pool fp32 [pool,2], dL/d mlp params fp32, whether dL/d params and the MLP's
+    dL/d input rows are all finite)."""
     scale = field.mlp_.loss_scale_
     d16 = ops.cast_f32_to_f16(d_out_f32, scale)
     dfeat16, dparams = ops.mlp_bwd(d16, feat16, hidden, params16, field.mlp_.n_hidden_matmuls, need_din=True)
@@ -233,7 +234,8 @@ def field_backward(field, params16, points, anchors, anchor_stride, feat16, hidd
     ops.hash_bwd(field.prim_pool_, field.bias_pool_, field.n_volumes_, field.local_size_, points, anchors, anchor_stride, dfeat16,
                  1.0 / scale, grad_table)
     dparams = dparams / scale
-    return grad_table, dparams
+    finite = bool(torch.isfinite(dfeat16).all() & torch.isfinite(dparams).all())
+    return grad_table, dparams, finite
 
 
 class _FieldFunction(torch.autograd.Function):
@@ -252,8 +254,10 @@ class _FieldFunction(torch.autograd.Function):
     def backward(ctx, g):
         field = ctx.field
         params16, points, anchors, feat16, hidden = ctx.saved
-        grad_table, dparams = field_backward(field, params16, points, anchors, 1, feat16, hidden, g.contiguous())
-        if not torch.isfinite(dparams).all():
+        grad_table, dparams, finite = field_backward(field, params16, points, anchors, 1, feat16, hidden, g.contiguous())
+        # TCNNWP.cpp:231-240: a non-finite dL/dinput (the fp16 dL/dfeat rows, which overflow before the fp32 dL/dparams
+        # do) backs off like a non-finite dL/dparams
+        if not finite:
             field.global_data_pool_.backward_nan_ = True
             field.mlp_.loss_scale_ = max(field.mlp_.loss_scale_ / 2.0, 1.0)
         return grad_table, dparams, None, None, None

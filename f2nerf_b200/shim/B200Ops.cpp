@@ -124,7 +124,8 @@ public:
                            points.data_ptr<float>(), anchors.data_ptr<int>(), 1, n, dfeat16.data_ptr(), 1, 1.f / scale,
                            dtable.data_ptr<float>(), cur_stream()));
     dparams = dparams / scale;
-    if (!torch::all(torch::isfinite(dparams)).item<bool>()) {            // TCNNWP.cpp:231-240
+    // TCNNWP.cpp:231-240: dL/dinput (the fp16 dL/dfeat rows, which overflow before the fp32 dL/dparams do) or dL/dparams
+    if (!torch::all(torch::isfinite(dfeat16)).item<bool>() || !torch::all(torch::isfinite(dparams)).item<bool>()) {
       f->global_data_pool_->backward_nan_ = true;
       f->mlp_->loss_scale_ = std::max(f->mlp_->loss_scale_ / 2.f, 1.f);
     }
@@ -171,7 +172,7 @@ public:
                           dparams.data_ptr<float>(), cur_stream()));
     F2B_CHECK(f2b_cast_f16_to_f32(din16.data_ptr(), din.data_ptr<float>(), din.numel(), 1.f / scale, cur_stream()));
     dparams = dparams / scale;
-    if (!torch::all(torch::isfinite(dparams)).item<bool>()) {
+    if (!torch::all(torch::isfinite(din)).item<bool>() || !torch::all(torch::isfinite(dparams)).item<bool>()) {   // as FieldFn
       s->global_data_pool_->backward_nan_ = true;
       s->mlp_->loss_scale_ = std::max(s->mlp_->loss_scale_ / 2.f, 1.f);
     }

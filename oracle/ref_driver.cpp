@@ -21,6 +21,16 @@
 //       its dumped state alone; and after each iteration a small probe is drawn from each generator and dumped — equal
 //       probes mean the iteration consumed the same draws.  Per iteration, <out_dir>/it<k>/ holds the state before the
 //       step, the Render outputs, the loss, the gradients, the octree after the step and the probes.
+//   ref_driver --ops <runtime_config.yaml> <in_dir> <out_dir>
+//       the two MLP operators alone, on inputs a test wrote: Hash3DAnchored::AnchoredQuery and SHShader::Query, each followed
+//       by (out * g).sum().backward().  In ref_driver these are the reference's own (tiny-cuda-nn); in ref_driver_b200 always
+//       this library's operator subclasses, whatever F2B_SHIM says.  Every subdirectory <case> of in_dir holding points.npy is
+//       one case, run in name order on the one scene; a case reads <in_dir>/<case>/<name>.npy, or <in_dir>/<name>.npy when it
+//       has none: feat_pool [pool,2], field_params, shader_params, loss_scales [2] (field, shader), points [n,3],
+//       anchors [n] i32, d_out [n,16], feats [n,16], dirs [n,3], d_rgb [n,3].  The generators are seeded right before each
+//       operator.  <out_dir>/<case>/ gets the outputs, the gradients (the table's as nonzero index / value), the flags
+//       [backward_nan_, field loss scale, shader loss scale] after each operator's backward and a 4-value torch::rand probe of
+//       the CUDA generator after each operator; <out_dir> itself gets the scene blobs.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -77,7 +87,7 @@ struct Scene {
   SHShader* shader = nullptr;
 };
 
-static Scene make_scene(const std::string& conf_path, bool fixed_lr) {
+static Scene make_scene(const std::string& conf_path, bool fixed_lr, bool ops_level = false) {
   Scene sc;
   torch::manual_seed(2022);   // main.cpp:8
   sc.gdp = std::make_unique<GlobalDataPool>(conf_path);
@@ -108,9 +118,10 @@ static Scene make_scene(const std::string& conf_path, bool fixed_lr) {
   // (f2nerf_b200/shim/B200Renderer.cpp) working on the reference's own operator objects.  F2B_SHIM=ops: the operator-level
   // drop-in — the reference's OWN Renderer::Render / autograd / loss drive this library's subclasses (INTEGRATION.md): same octree
   // object, same parameters.  Either way every dump below is directly comparable with the pure-reference run of
-  // oracle/_ref/ref_driver.  Never built into ref_driver (the reference arm stays unmodified).
+  // oracle/_ref/ref_driver.  Never built into ref_driver (the reference arm stays unmodified).  ``ops_level`` (--ops) installs
+  // the operator subclasses whatever F2B_SHIM says.
   const char* shim_env = std::getenv("F2B_SHIM");
-  const bool shim_ops = shim_env && std::string(shim_env) == "ops";
+  const bool shim_ops = ops_level || (shim_env && std::string(shim_env) == "ops");
   if (shim_ops) {
     f2b_render_use_reference(true);
     auto b_sampler = std::make_unique<B200Sampler>(gdp);
@@ -162,8 +173,10 @@ static void dump_scene(const Scene& sc, int n_rays) {
 }
 
 static int run_steps(const std::string& conf_path, const std::string& out_root, int n_iters, int fixed_batch);
+static int run_ops(const std::string& conf_path, const std::string& in_dir, const std::string& out_root);
 
 int main(int argc, char** argv) {
+  if (argc >= 5 && std::string(argv[1]) == "--ops") return run_ops(argv[2], argv[3], argv[4]);
   if (argc >= 3 && std::string(argv[1]) == "--train") {     // main.cpp:6-13 verbatim in behaviour
     torch::manual_seed(2022);
     auto exp_runner = std::make_unique<ExpRunner>(argv[2]);
@@ -174,7 +187,8 @@ int main(int argc, char** argv) {
     return run_steps(argv[2], argv[3], std::atoi(argv[4]), argc > 5 ? std::atoi(argv[5]) : 0);
   if (argc < 4) {
     std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads]\n"
-                         "       ref_driver --steps <config.yaml> <out_dir> <n_iters> [fixed_batch]\n");
+                         "       ref_driver --steps <config.yaml> <out_dir> <n_iters> [fixed_batch]\n"
+                         "       ref_driver --ops <config.yaml> <in_dir> <out_dir>\n");
     return 1;
   }
   const std::string conf_path = argv[1];
@@ -543,5 +557,81 @@ static int run_steps(const std::string& conf_path, const std::string& out_root, 
                 (long long) nodes_before, (long long) (sampler->pers_octree_->tree_nodes_gpu_.numel() / 64), int(nan_skip), reused, fresh);
   }
   std::printf("ref_driver: done, %d steps in %s\n", n_iters, out_root.c_str());
+  return 0;
+}
+
+// ====================================================================================================== --ops ===
+static const int64_t kOpsSeed = 52000;
+
+static int run_ops(const std::string& conf_path, const std::string& in_dir, const std::string& out_root) {
+  Scene sc = make_scene(conf_path, true, /*ops_level=*/true);
+  GlobalDataPool* gdp = sc.gdp.get();
+  auto* field = sc.field; auto* shader = sc.shader;
+  gdp->mode_ = RunningMode::TRAIN;
+  g_out = out_root;
+  fs::create_directories(g_out);
+  dump_scene(sc, 0);
+  std::vector<std::string> cases;
+  for (const auto& e : fs::directory_iterator(in_dir))
+    if (fs::is_directory(e.path()) && fs::exists(e.path() / "points.npy")) cases.push_back(e.path().filename().string());
+  std::sort(cases.begin(), cases.end());
+  const auto opts_of = [](bool is_int) { return is_int ? CPUInt : CPUFloat; };
+
+  for (const auto& c : cases) {
+    const auto in = [&](const std::string& name, bool is_int = false) {
+      std::string p = in_dir + "/" + c + "/" + name + ".npy";
+      if (!fs::exists(p)) p = in_dir + "/" + name + ".npy";
+      cnpy::NpyArray a = cnpy::npy_load(p);
+      CHECK(a.word_size == 4 && !a.fortran_order) << p;
+      std::vector<int64_t> shape(a.shape.begin(), a.shape.end());
+      return torch::from_blob(a.data<char>(), shape, opts_of(is_int)).clone().to(torch::kCUDA).contiguous();
+    };
+    g_out = out_root + "/" + c;
+    fs::create_directories(g_out);
+    field->feat_pool_.data().copy_(in("feat_pool"));
+    field->mlp_->params_.data().copy_(in("field_params"));
+    shader->mlp_->params_.data().copy_(in("shader_params"));
+    Tensor scales = in("loss_scales").to(torch::kCPU);
+    field->mlp_->loss_scale_ = scales[0].item<float>();
+    shader->mlp_->loss_scale_ = scales[1].item<float>();
+    field->feat_pool_.mutable_grad() = Tensor(); field->mlp_->params_.mutable_grad() = Tensor();
+    shader->mlp_->params_.mutable_grad() = Tensor();
+    const auto flags = [&]() {
+      Tensor f = torch::zeros({3}, CPUFloat);
+      f[0] = gdp->backward_nan_ ? 1.f : 0.f; f[1] = field->mlp_->loss_scale_; f[2] = shader->mlp_->loss_scale_;
+      return f;
+    };
+
+    // field: hash encode + field MLP
+    gdp->backward_nan_ = false;
+    torch::manual_seed(kOpsSeed);
+    Tensor out = field->AnchoredQuery(in("points"), in("anchors", true));
+    (out * in("d_out")).sum().backward();
+    dump("field_out", out);
+    Tensor g = field->feat_pool_.grad().reshape({-1});
+    Tensor nz = torch::nonzero(g).reshape({-1});
+    dump("field_grad_table_nz_idx", nz.to(torch::kInt32)); dump("field_grad_table_nz_val", g.index({nz}));
+    dump("field_grad_params", field->mlp_->params_.grad());
+    Tensor ff = flags();
+    dump("field_flags", ff);
+    dump("field_probe", torch::rand({4}, CUDAFloat));
+
+    // shader: SH encode + shader MLP + colour activation
+    gdp->backward_nan_ = false;
+    torch::manual_seed(kOpsSeed + 1);
+    Tensor feats = in("feats").requires_grad_(true);
+    Tensor rgb = shader->Query(feats, in("dirs"));
+    (rgb * in("d_rgb")).sum().backward();
+    dump("rgb", rgb);
+    dump("shader_grad_params", shader->mlp_->params_.grad());
+    dump("feats_grad", feats.grad());
+    Tensor sf = flags();
+    dump("shader_flags", sf);
+    dump("shader_probe", torch::rand({4}, CUDAFloat));
+    std::printf("{\"ops_case\": \"%s\", \"n\": %d, \"field_flags\": [%g, %g, %g], \"shader_flags\": [%g, %g, %g]}\n", c.c_str(),
+                int(out.size(0)), ff[0].item<float>(), ff[1].item<float>(), ff[2].item<float>(), sf[0].item<float>(),
+                sf[1].item<float>(), sf[2].item<float>());
+  }
+  std::printf("ref_driver: done, %d operator cases in %s\n", int(cases.size()), out_root.c_str());
   return 0;
 }

@@ -53,6 +53,11 @@ SIGNATURES = {
     "f2b_mlp_fwd": [_P, _P, c_int, c_int, _P, _P, _P],
     "f2b_mlp_fwd_f32": [_P, _P, c_int, c_int, _P, _P, _P, _P],
     "f2b_mlp_bwd": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
+    "f2b_locate_points": [_P, c_int, _P, _P, c_int, _P, _P, _P],
+    "f2b_query_logit_points": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_float, _P, _P],
+    "f2b_query_logit_grid": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _P],
+    "f2b_iso_count": [_P, c_int, c_int, c_int, c_float, c_float, c_int, c_int, _P, _P, _P, _P],
+    "f2b_iso_emit": [_P, c_int, c_int, c_int, c_float, c_float, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P],
     "f2b_field_shade_fwd": [_P, _P, _P, _P, _P, c_int, _P, _P, _P, _P],
     "f2b_shader_mlp_rgb_fwd": [_P, _P, c_int, _P, _P, _P, _P],
     "f2b_mlp_bwd2": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],

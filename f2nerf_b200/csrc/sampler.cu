@@ -21,6 +21,7 @@
 //  * DFS stack lives in shared memory (packed node<<4|cursor, one private copy per lane so no
 //    intra-group ordering is assumed), not 192 B/thread of local memory.
 #include "common.cuh"
+#include "locate.cuh"
 #include "scan.cuh"
 
 namespace f2b {
@@ -321,28 +322,7 @@ sampler_gather_kernel(const float* __restrict__ rays_d, const int* __restrict__ 
   for (int i = lane; i < n; i += 32) { dt[beg + i] = s_dt[src + i]; t[beg + i] = s_t[src + i]; }
 }
 
-// ---- edge samples (PersSampler.cu:436-452) ----------------------------------------------------
-__device__ __forceinline__ void warp_point(const TransInfo* __restrict__ T, float X, float Y, float Z,
-                                           float out[3]) {
-  float v[12];
-#pragma unroll
-  for (int i = 0; i < 12; i++) {
-    const float* a = T->w2xz[i];
-    const float xz0 = fadd(ffma(X, a[0], fmul(Y, a[1])), ffma(Z, a[2], a[3]));
-    const float xz1 = fadd(ffma(X, a[4], fmul(Y, a[5])), ffma(Z, a[6], a[7]));
-    v[i] = fdiv(xz0, xz1);
-  }
-#pragma unroll
-  for (int r = 0; r < 3; r++) {
-    const float* w = T->weight[r];
-    float g[4];
-#pragma unroll
-    for (int s = 0; s < 4; s++)
-      g[s] = ffma(w[3 * s], v[3 * s], ffma(w[3 * s + 1], v[3 * s + 1], fmul(w[3 * s + 2], v[3 * s + 2])));
-    out[r] = fadd(fadd(g[0], g[1]), fadd(g[2], g[3]));
-  }
-}
-
+// ---- edge samples (PersSampler.cu:436-452; warp_point in locate.cuh) ----------------------------
 __global__ void edge_samples_kernel(int n_pts, const EdgePool* __restrict__ edge_pool,
                                     const TransInfo* __restrict__ trans,
                                     const int* __restrict__ edge_idx,

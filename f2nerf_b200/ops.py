@@ -170,6 +170,56 @@ def cast_f16_to_f32(x, scale=1.0):
     return out
 
 
+# ------------------------------------------------------------------ geometry --------------------
+def _host3(v):
+    import ctypes
+    return (ctypes.c_float * 3)(*[float(x) for x in v])
+
+
+def locate_points(tree_nodes, trans, pts):
+    """-> (warped [n,3] f32, anchors [n,2] i32 = (trans_idx, leaf node), (-1, -1) where no leaf holds the point)."""
+    _chk(pts, F32, "locate_points: pts")
+    n = pts.shape[0]
+    warped = dev_empty((n, 3), F32, pts)
+    anchors = dev_empty((n, 2), I32, pts)
+    call("f2b_locate_points", tree_nodes, tree_nodes.numel() // 64, trans, pts, n, warped, anchors, stream())
+    return warped, anchors
+
+
+def query_logit_points(tree_nodes, trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, pts, empty_logit):
+    _chk(pts, F32, "query_logit_points: pts")
+    n = pts.shape[0]
+    out = dev_empty((n,), F32, pts)
+    call("f2b_query_logit_points", tree_nodes, tree_nodes.numel() // 64, trans, table_f16, prim_pool, bias_pool, int(n_volumes),
+         int(local_size), params_f16, pts, n, float(empty_logit), out, stream())
+    return out
+
+
+def query_logit_grid(tree_nodes, trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, origin, voxel, nx, ny,
+                     z0, nz, empty_logit, out):
+    """Logits of lattice layers [z0, z0 + nz) into ``out`` ([nz, ny, nx] f32, contiguous)."""
+    o3, v3 = _host3(origin), _host3(voxel)
+    import ctypes
+    call("f2b_query_logit_grid", tree_nodes, tree_nodes.numel() // 64, trans, table_f16, prim_pool, bias_pool, int(n_volumes),
+         int(local_size), params_f16, ctypes.addressof(o3), ctypes.addressof(v3), int(nx), int(ny), int(z0), int(nz),
+         float(empty_logit), out, stream())
+    return out
+
+
+def iso_count(logit, level, empty_logit, ez0, ez1, edge_mask, vert_counts, tri_counts):
+    nz, ny, nx = logit.shape
+    call("f2b_iso_count", logit, nx, ny, nz, float(level), float(empty_logit), int(ez0), int(ez1), edge_mask, vert_counts,
+         tri_counts, stream())
+
+
+def iso_emit(logit, level, empty_logit, origin, voxel, ez0, ez1, vert_base, edge_mask, vert_bounds, tri_bounds, verts, faces):
+    import ctypes
+    nz, ny, nx = logit.shape
+    o3, v3 = _host3(origin), _host3(voxel)
+    call("f2b_iso_emit", logit, nx, ny, nz, float(level), float(empty_logit), ctypes.addressof(o3), ctypes.addressof(v3), int(ez0),
+         int(ez1), int(vert_base), edge_mask, vert_bounds, tri_bounds, verts, faces, stream())
+
+
 # ------------------------------------------------------------------ shader ----------------------
 def sh_encode(dirs, degree=4):
     n = dirs.shape[0]

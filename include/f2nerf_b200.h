@@ -170,6 +170,43 @@ int f2b_field_fwd_slots(const void* table_f16, const int* prim_pool, const float
                         int vol_stride, const int* ray_counts, int n_rays, int slot_size, int logit_only,
                         float* out_f32, void* feat_save_f16, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Geometry — no reference counterpart (the reference renders images only).  A trained scene's density at arbitrary
+ * world points of the normalised scene frame and its isosurface; DESIGN.md §3i.
+ * ------------------------------------------------------------------------------------------ */
+/* Point location: the leaf holding each point (root-down walk, one child per level; every node is the half-open cube
+ * [c - s/2, c + s/2), so a point on a splitting plane goes to the upper child) and the point warped by that leaf's
+ * TransInfo in the march's roundings.  anchors [n,2] = (trans_idx, leaf node) as the march's s_anchors; (-1, -1) and
+ * warped (0, 0, 0) where the point is outside the root cube, in a dead child slot or in a leaf with trans_idx < 0. */
+int f2b_locate_points(const void* tree_nodes, int n_nodes, const void* trans, const float* pts /* [n,3] */, int n_pts,
+                      float* warped /* [n,3] */, int* anchors /* [n,2] */, void* stream);
+/* Density logit (field output channel 0) of located world points: f2b_locate_points + the f2b_field_fwd kernel, with the
+ * located rows bit-identical to f2b_field_fwd(logit_only = 1) on (warped, trans_idx) and empty_logit on the others. */
+int f2b_query_logit_points(const void* tree_nodes, int n_nodes, const void* trans, const void* table_f16,
+                           const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                           const void* mlp_params_f16, const float* pts /* [n,3] */, int n_pts, float empty_logit,
+                           float* logit /* [n] */, void* stream);
+/* The same on the lattice point (x, y, z) = origin + voxel * (i, j, k) (fp32: fadd(origin, fmul(voxel, float(i))) per axis)
+ * for i < nx, j < ny, k in [z0, z0 + nz), generated in the kernel; logit[(k - z0) * nx * ny + j * nx + i].
+ * origin3 / voxel3: host arrays of 3 floats. */
+int f2b_query_logit_grid(const void* tree_nodes, int n_nodes, const void* trans, const void* table_f16,
+                         const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                         const void* mlp_params_f16, const float* origin3, const float* voxel3, int nx, int ny, int z0,
+                         int nz, float empty_logit, float* logit, void* stream);
+/* Isosurface {logit = level} of an nx x ny x nz logit lattice (x fastest) by marching tetrahedra on the Kuhn split of each
+ * cell, lattice points outside the lattice reading empty_logit (<= level), for the cells of extended z-layers [ez0, ez1)
+ * (0 <= ez0 < ez1 <= nz + 1; extended layer e holds lattice layer e - 1, see geometry.cu).  Pass 1 writes, per owner
+ * point of extended layers [ez0, min(ez1 + 1, nz + 1)) ((nx+1)(ny+1) per layer), the 7-bit mask of its crossing edges
+ * and their count, and per cell of [ez0, ez1) its triangle count.  f2b_count_scan of both counts gives vert_bounds /
+ * tri_bounds; pass 2 writes the slab's vertices (slab-local index vert_bounds[p] + rank of the direction) as
+ * origin + voxel * (index + t * dir), t = (level - f_a) / (f_b - f_a), and its triangles (outward, towards lower logits)
+ * as global vertex ids, vert_base + slab-local id.  origin3 / voxel3: host arrays of 3 floats. */
+int f2b_iso_count(const float* logit, int nx, int ny, int nz, float level, float empty_logit, int ez0, int ez1,
+                  uint8_t* edge_mask, int* vert_counts, int* tri_counts, void* stream);
+int f2b_iso_emit(const float* logit, int nx, int ny, int nz, float level, float empty_logit, const float* origin3,
+                 const float* voxel3, int ez0, int ez1, int vert_base, const uint8_t* edge_mask, const int* vert_bounds,
+                 const int* tri_bounds, float* verts, int* faces, void* stream);
+
 /* Field MLP on already-encoded features with the shading-feature assembly fused into its epilogue (the fp32 [P,16]
  * scene_feat tensor, `ones_like`/`cat`/ScatterAdd of Renderer.cpp:179-187 and the SH encode + cast of SHShader.cpp:23-26
  * never materialise): logit[p] = out[p,0]; mlp_in[p] = fp16([1, out[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])). */

@@ -3,11 +3,14 @@
 reference (oracle/_ref/ref_driver, built by oracle/Makefile.ref) on an H100:
 
     python oracle/make_golden.py OUT_DIR              # writes OUT_DIR/ref_ngp_fox{,_512}_{run,rays,adam}.npz
-    mv OUT_DIR/ref_ngp_fox_*.npz tests/golden/
+    python oracle/make_golden.py OUT_DIR --config free  # writes OUT_DIR/ref_free_512_{run,rays}.npz
+    mv OUT_DIR/ref_*.npz tests/golden/
 
 ref_ngp_fox_*: an 8-ray batch with every per-sample tensor.  ref_ngp_fox_512_*: the 512-ray batch tests/test_ref_parity.py's
 ``live`` cases run the reference on, stored for when its binary is not built: every per-ray tensor, and the per-sample tensors
-of SAMPLE_RAYS seeded rays (``sample_rays``; their segments concatenated in ray order).
+of SAMPLE_RAYS seeded rays (``sample_rays``; their segments concatenated in ray order).  ``--config free``: the same 512-ray
+batch under oracle/ref_config_free.yaml at the fineness and gradient-scaling progress of its iteration 0 (FREE_RUN), for
+tests/test_gpu_ref_configs.py; no optimizer sample (the optimizer step does not depend on the config).
 
 The fixture (tests/workloads.py:load_golden merges the two files, each kept under 1 MB: the scene and parameters in the first,
 the ray batch's dumps in the second) holds the reference's own ngp_fox octree / warp blobs, a small seeded ray batch and every
@@ -17,6 +20,7 @@ tests/test_golden_ref.py pins oracle/f2_oracle.c against it on the CPU.  tests/g
 is the scene part of an earlier run of this script, kept so that the benchmark's inputs stay fixed.  The 64 MB hash table is not stored:
 both sides regenerate it from the CPU generator seed 1234 (see ref_driver.cpp).
 """
+import argparse
 import os
 import subprocess
 import sys
@@ -42,16 +46,27 @@ def segments(a, bounds, rays):
     return np.concatenate([a[b:e] for b, e in bounds[rays]]) if len(rays) else a[:0]
 
 
+# ref_driver's trailing [fineness, gs_progress] per config: what ExpRunner::UpdateAdaParams gives ref_config_free.yaml at
+# iteration 0 (ray_march_init_fineness 4, no gradient scaling)
+FREE_RUN = ("4", "1")
+
+
 def main():
-    dst_dir = sys.argv[1]
-    dump(dst_dir, "ref_ngp_fox", 8, None)
-    dump(dst_dir, "ref_ngp_fox_512", 512, SAMPLE_RAYS)
+    ap = argparse.ArgumentParser()
+    ap.add_argument("dst_dir")
+    ap.add_argument("--config", choices=("ngp_fox", "free"), default="ngp_fox")
+    a = ap.parse_args()
+    if a.config == "ngp_fox":
+        dump(a.dst_dir, "ref_ngp_fox", 8, None)
+        dump(a.dst_dir, "ref_ngp_fox_512", 512, SAMPLE_RAYS)
+    else:
+        dump(a.dst_dir, "ref_free_512", 512, SAMPLE_RAYS, "ref_config_free.yaml", FREE_RUN, with_adam=False)
 
 
-def dump(dst_dir, prefix, n_rays, sample_rays):
+def dump(dst_dir, prefix, n_rays, sample_rays, config="ref_config_ngp_fox.yaml", run_args=(), with_adam=True):
     drv = os.path.join(ROOT, "oracle", "_ref", "ref_driver")
     out = "/tmp/f2b_golden_dump"
-    r = subprocess.run([drv, os.path.join(ROOT, "oracle", "ref_config_ngp_fox.yaml"), out, str(n_rays), "0", "1"], cwd=ROOT,
+    r = subprocess.run([drv, os.path.join(ROOT, "oracle", config), out, str(n_rays), "0", "1", *run_args], cwd=ROOT,
                        capture_output=True, text=True, timeout=900)
     if r.returncode != 0:
         print(r.stdout[-2000:], r.stderr[-4000:])
@@ -63,12 +78,14 @@ def dump(dst_dir, prefix, n_rays, sample_rays):
             "train_noise", "train_bg", "train_edge_idx", "train_edge_coord", "train_pts", "train_dt", "train_t", "train_anchors",
             "train_bounds", "train_colors", "train_disparity", "train_depth", "train_weights", "train_idx_start_end",
             "train_first_oct_dis", "train_tree_nodes_after", "train_weight_stats_after", "train_alpha_stats_after",
-            "train_visit_cnt_after", "train_loss", "grad_field_mlp", "grad_shader_mlp", "grad_app_emb",
+            "train_visit_cnt_after", "train_loss", "grad_field_mlp", "grad_shader_mlp",
             "edge_idx", "edge_coord", "edge_pts", "edge_anchors", "train_edge_feats",
             "ds_poses", "ds_intri", "ds_dist_params", "ray_ij", "ds_hw", "ds_bounds", "ds_train_set", "ray_bounds",
             "oct_intri", "oct_w2c", "oct_bound", "backward_nan",
             "oct_nodes_in", "oct_w_in", "oct_a_in", "oct_visit_in", "oct_nodes_sub", "oct_w_sub", "oct_a_sub",
             "oct_nodes_invis", "oct_nodes_final", "oct_w_final", "oct_a_final"]
+    if os.path.exists(os.path.join(out, "grad_app_emb.npy")):          # not dumped when the config has no embedding
+        keep.append("grad_app_emb")
     data = {k: np.load(os.path.join(out, k + ".npy")) for k in keep}
     if sample_rays:
         rays = np.sort(np.random.default_rng(2).choice(n_rays, sample_rays, replace=False))
@@ -107,8 +124,8 @@ def dump(dst_dir, prefix, n_rays, sample_rays):
     data["train_edge_coord"] = data["train_edge_coord"].astype(np.float32)
     os.makedirs(dst_dir, exist_ok=True)
     scene = {k: v for k, v in data.items() if k.startswith(SCENE)}
-    for name, part in ((prefix + "_run.npz", scene), (prefix + "_rays.npz", {k: v for k, v in data.items() if k not in scene}),
-                       (prefix + "_adam.npz", adam)):
+    parts = [(prefix + "_run.npz", scene), (prefix + "_rays.npz", {k: v for k, v in data.items() if k not in scene})]
+    for name, part in parts + ([(prefix + "_adam.npz", adam)] if with_adam else []):
         dst = os.path.join(dst_dir, name)
         np.savez_compressed(dst, **part)
         print("wrote", dst, os.path.getsize(dst) / 1e6, "MB")

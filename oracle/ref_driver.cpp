@@ -8,7 +8,11 @@
 // inputs and dumps every boundary tensor as .npy, (3) times Render + backward with CUDA events.
 // The dumps pin oracle/f2_oracle.c and the CUDA kernels (tests/golden/, tests/test_ref_parity.py).
 //
-//   ref_driver <runtime_config.yaml> <out_dir> <n_rays> [n_time_iters=0] [dump_full_grads=0]
+//   ref_driver <runtime_config.yaml> <out_dir> <n_rays> [n_time_iters=0] [dump_full_grads=0] [fineness=1] [gs_progress=0.25]
+//       the seeded VALIDATE and TRAIN batches run at ray-march fineness `fineness` and gradient-scaling progress `gs_progress`
+//       (ExpRunner::UpdateAdaParams' values at iteration 0 of the free configs are 4 and 1); `scalars` records them with
+//       use_app_emb: [near, sample_l, scale_by_dis, max_hits, n_volumes, pool_size, n_images, n_rays, use_app_emb, fineness,
+//       gs_progress].  Readers take a vector of the first 8 only as use_app_emb 1, fineness 1, progress 0.25.
 //   ref_driver --train <runtime_config.yaml>      what the reference's main.cpp does: ExpRunner(conf).Execute() — the
 //                                                 unmodified trainer (train to end_iter, then TestImages -> mean PSNR)
 //   ref_driver --steps <runtime_config.yaml> <out_dir> <n_iters> [fixed_batch=0]
@@ -20,7 +24,8 @@
 //       generators are reseeded (kStepSeed + k) at the start of iteration k, so that every iteration can be replayed from
 //       its dumped state alone; and after each iteration a small probe is drawn from each generator and dumped — equal
 //       probes mean the iteration consumed the same draws.  Per iteration, <out_dir>/it<k>/ holds the state before the
-//       step, the Render outputs, the loss, the gradients, the octree after the step and the probes.
+//       step, the Render outputs, the loss, the gradients (d_weights: dL/dweights as the loss hands it to Render's backward,
+//       the var-loss term through the reference's WeightVar), the octree after the step and the probes.
 //   ref_driver --ops <runtime_config.yaml> <in_dir> <out_dir>
 //       the two MLP operators alone, on inputs a test wrote: Hash3DAnchored::AnchoredQuery and SHShader::Query, each followed
 //       by (out * g).sum().backward().  In ref_driver these are the reference's own (tiny-cuda-nn); in ref_driver_b200 always
@@ -165,10 +170,12 @@ static void dump_scene(const Scene& sc, int n_rays) {
   dump("field_mlp_params", field->mlp_->params_);
   dump("shader_mlp_params", shader->mlp_->params_);
   dump("app_emb", sc.renderer->app_emb_);
-  Tensor s = torch::zeros({8}, CPUFloat);
+  Tensor s = torch::zeros({11}, CPUFloat);
   s[0] = sampler->global_near_; s[1] = sampler->sample_l_; s[2] = sampler->scale_by_dis_ ? 1.f : 0.f;
   s[3] = float(sampler->max_oct_intersect_per_ray_); s[4] = float(field->n_volumes_);
   s[5] = float(field->pool_size_); s[6] = float(sc.dataset->n_images_); s[7] = float(n_rays);
+  s[8] = sc.renderer->use_app_emb_ ? 1.f : 0.f;
+  s[9] = sc.gdp->ray_march_fineness_; s[10] = sc.gdp->gradient_scaling_progress_;
   dump("scalars", s);
 }
 
@@ -186,7 +193,7 @@ int main(int argc, char** argv) {
   if (argc >= 5 && std::string(argv[1]) == "--steps")
     return run_steps(argv[2], argv[3], std::atoi(argv[4]), argc > 5 ? std::atoi(argv[5]) : 0);
   if (argc < 4) {
-    std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads]\n"
+    std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads] [fineness] [gs_progress]\n"
                          "       ref_driver --steps <config.yaml> <out_dir> <n_iters> [fixed_batch]\n"
                          "       ref_driver --ops <config.yaml> <in_dir> <out_dir>\n");
     return 1;
@@ -196,6 +203,8 @@ int main(int argc, char** argv) {
   const int n_rays = std::atoi(argv[3]);
   const int n_time = argc > 4 ? std::atoi(argv[4]) : 0;
   const int full_grads = argc > 5 ? std::atoi(argv[5]) : 0;
+  const float fineness = argc > 6 ? std::strtof(argv[6], nullptr) : 1.f;
+  const float gs_progress = argc > 7 ? std::strtof(argv[7], nullptr) : 0.25f;   // < 1 exercises GradientScaling
   fs::create_directories(g_out);
 
   Scene sc = make_scene(conf_path, true);
@@ -206,7 +215,9 @@ int main(int argc, char** argv) {
   auto* field = sc.field;
   auto* shader = sc.shader;
 
-  // ---- scene blobs & scalars --------------------------------------------------------------------
+  // ---- scene blobs & scalars (the fineness and progress both seeded batches run at are part of them) ----------------
+  gdp->ray_march_fineness_ = fineness;
+  gdp->gradient_scaling_progress_ = gs_progress;
   dump_scene(sc, n_rays);
 
   // ---- rays ---------------------------------------------------------------------------------------
@@ -244,8 +255,6 @@ int main(int argc, char** argv) {
 
   // ---- sampler, VALIDATE mode (noise == 1) --------------------------------------------------------
   gdp->iter_step_ = 1;
-  gdp->ray_march_fineness_ = 1.f;
-  gdp->gradient_scaling_progress_ = 0.25f;   // exercise GradientScaling
   gdp->mode_ = RunningMode::VALIDATE;
   {
     torch::NoGradGuard ng;
@@ -524,7 +533,9 @@ static int run_steps(const std::string& conf_path, const std::string& out_root, 
     bool stepped = false;
     if (loss.requires_grad()) {                                                             // :128-138
       optimizer.zero_grad();
+      if (r.weights.requires_grad()) r.weights.retain_grad();
       loss.backward();
+      if (r.weights.grad().defined()) dump("d_weights", r.weights.grad());
       dump("grad_field_mlp", field->mlp_->params_.grad()); dump("grad_shader_mlp", shader->mlp_->params_.grad());
       if (renderer->app_emb_.grad().defined()) dump("grad_app_emb", renderer->app_emb_.grad());
       Tensor g = field->feat_pool_.grad().reshape({-1});

@@ -8,6 +8,7 @@
 # And the float64-autograd gradient module (tests/test_gpu_grad_autograd.py): 48 TRAIN steps, each with a float64 twin on the device.
 # And the C++ operator module (tests/test_gpu_cpp_ops_reference.py): it runs both reference binaries over 16 operator cases.
 # And the geometry module (tests/test_gpu_geometry.py): the tensor-core point query, and a 300-iteration ngp_fox training.
+# And the reference-configs module (tests/test_gpu_ref_configs.py): both reference binaries, three arms on free, big20 and big22.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
      "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
@@ -16,11 +17,11 @@ OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
       --ignore=tests/test_gpu_mlp_fwd_reference.py --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
       --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py --ignore=tests/test_gpu_grad_autograd.py
-      --ignore=tests/test_gpu_cpp_ops_reference.py --ignore=tests/test_gpu_geometry.py)
+      --ignore=tests/test_gpu_cpp_ops_reference.py --ignore=tests/test_gpu_geometry.py --ignore=tests/test_gpu_ref_configs.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py
-  echo tests/test_gpu_mlp_fwd_reference.py; echo tests/test_ref_parity.py
+  echo tests/test_gpu_mlp_fwd_reference.py; echo tests/test_ref_parity.py; echo tests/test_gpu_ref_configs.py
   exit 0
 fi
 O=${O:-ci_logs}
@@ -44,6 +45,10 @@ timeout 900 python -m pytest tests/test_gpu_mlp_fwd_reference.py -m gpu -q -p no
 echo "--- tests/test_gpu_mlp_fwd_reference.py"; tail -n 40 $O/pytest_mlp_fwd_reference.log | cut -c1-250
 timeout 600 python -m pytest tests/test_ref_parity.py -m gpu -q -p no:cacheprovider > $O/pytest_ref.log 2>&1
 tail -n 60 $O/pytest_ref.log
+# the free / big20 / big22 configs against the reference program in three arms (nine reference-program runs); -rs lists skips
+timeout 1800 python -m pytest tests/test_gpu_ref_configs.py -m gpu -q -rs -p no:cacheprovider --durations=10 > $O/pytest_ref_configs.log 2>&1
+echo "--- tests/test_gpu_ref_configs.py"; tail -n 40 $O/pytest_ref_configs.log | cut -c1-250
+cp "$(python -c 'import tempfile; print(tempfile.gettempdir())')"/f2b_test_diag/refcfg_*.json "$O"/ 2>/dev/null   # measured margins
 if [ "${SANITIZE:-0}" = "1" ]; then
   timeout 900 compute-sanitizer --tool memcheck --print-limit 8 python -m pytest "tests/test_gpu_render.py::test_render_train_step_matches_oracle" -q -x -p no:cacheprovider -k "64" > $O/sanitizer.log 2>&1
   grep -E "Invalid|at 0x|by thread|Address|in /|\.cu:|=========     at|ERROR SUMMARY" $O/sanitizer.log | head -40

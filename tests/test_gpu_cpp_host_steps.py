@@ -3,10 +3,14 @@
 oracle/ref_config_ngp_fox_steps.yaml — compaction every 3 iterations from iteration 0, subdivision milestones at 4 and 6,
 gradient-scaling progress ramping through 1, a ramping var-loss weight, the batch size from the meaningful-samples EMA —
 and dumps every iteration's starting state, outputs, loss, gradients, octree afterwards and a probe of both generators.
+a. and b. also run on oracle/ref_config_free_steps.yaml, the same schedule on the free settings (no appearance embedding,
+scale_by_dis off, near 0.05, fineness decaying 4 -> 1, no gradient scaling): there no host may give the embedding a gradient.
 
 a. The fused C++ host (f2nerf_b200/shim/B200Renderer.cpp) against the Python host, iteration by iteration.  Each iteration
    is replayed from the C++ run's dumped state (so atomic-order gradient differences do not accumulate) through Render,
-   the same loss, backward and PersSampler.maintain.  Bit-identical: the probes, the batch size, every deterministic output,
+   the same loss, backward and PersSampler.maintain.  The backward takes the C++ run's dL/dweights, so both hosts start it
+   from the same upstream gradient; the Python loss's own dL/dweights (f2b_weight_var) is compared with it separately
+   (python_step).  Bit-identical: the probes, the batch size, every deterministic output,
    and after the step the tree, its statistics and visit counts and the remaining milestones; the loss to 1e-6, the
    gradients to fp32 summation order, the EMAs to fp32 rounding (the Python host keeps them in double).  On the
    maintenance iterations this also holds the reference's own host ProcOctree / MarkInvisibleNodes, which the C++ host runs
@@ -42,6 +46,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = os.path.join(ROOT, "oracle", "_ref", "ref_driver")
 B200 = os.path.join(ROOT, "oracle", "_ref", "ref_driver_b200")
 CONFIG = os.path.join(ROOT, "oracle", "ref_config_ngp_fox_steps.yaml")
+# the same schedule on the free settings: no appearance embedding, scale_by_dis off, near 0.05, fineness 4 -> 1, no gradient scaling
+FREE_CONFIG = os.path.join(ROOT, "oracle", "ref_config_free_steps.yaml")
 N_ITERS = 10
 FIXED_BATCH = 256
 # b.: bars a few times above what an H100 SXM run measures (written to cpp_host_steps_margins_<arm>.json under
@@ -111,7 +117,14 @@ def ray_generator(root):
 
 def python_step(root, it, k, gen):
     """Render + loss + backward of iteration k on the Python host, from the C++ run's dumped starting state (the caller then
-    reads the non-finite flags: check_nonfinite)"""
+    reads the non-finite flags: check_nonfinite) -> (objects, RenderResult, loss, relative L2 of the Python loss's dL/dweights
+    against the C++ run's).
+
+    The backward takes the C++ run's own dL/dweights (``d_weights``) in place of the var-loss term's: that term goes through
+    WeightVar, which the C++ run's loss computes with the reference's kernel (CustomOps.cu:38-66, one thread summing a ray's
+    samples in order) and the Python host with f2b_weight_var (a warp reduction).  The two sums round differently in fp32, and
+    its ~1e-5 relative difference reaches the table gradient through the fp16 rounding of dL/dfeat, so it would hide what the
+    hosts themselves do; the WeightVars are compared on their own through the returned figure."""
     from test_ref_parity import build_from_ref
     from f2nerf_b200 import TRAIN, CustomOps
     st = it["state"]
@@ -139,10 +152,15 @@ def python_step(root, it, k, gen):
     gt = T(it["gt_colors"])
     r = renderer.Render(ro, rd, None, cam)
     w_var, w_disp, w_tv = (float(x) for x in st[9:12])
-    loss = (torch.sqrt((r.colors - gt) ** 2 + 1e-4).mean() + torch.sqrt(CustomOps.WeightVar(r.weights, r.idx_start_end) + 1e-2).mean() * w_var
-            + (r.disparity ** 2).mean() * w_disp + ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean() * w_tv)
-    loss.backward()
-    return (gdp, sampler, field, shader, renderer), r, loss.detach()
+    var_term = torch.sqrt(CustomOps.WeightVar(r.weights, r.idx_start_end) + 1e-2).mean() * w_var
+    rest = (torch.sqrt((r.colors - gt) ** 2 + 1e-4).mean() + (r.disparity ** 2).mean() * w_disp
+            + ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean() * w_tv)
+    loss = rest + var_term
+    d_weights, = torch.autograd.grad(var_term, r.weights, retain_graph=True)
+    want = T(it["d_weights"])
+    dw_rel = float(torch.linalg.norm((d_weights - want).double()) / max(float(torch.linalg.norm(want.double())), 1e-30))
+    (rest + (r.weights * want).sum()).backward()
+    return (gdp, sampler, field, shader, renderer), r, loss.detach(), dw_rel
 
 
 def check_nonfinite(renderer, it, nonfinite):
@@ -160,8 +178,12 @@ def replay(root, it, k, gen):
     """Iteration k through the Python host, checked against the C++ host's dumps -> summary of the iteration"""
     compact_freq = int(root["run"][0])
     st = it["state"]
-    (gdp, sampler, field, shader, renderer), r, loss = python_step(root, it, k, gen)
+    (gdp, sampler, field, shader, renderer), r, loss, dw_rel = python_step(root, it, k, gen)
     check_nonfinite(renderer, it, False)
+    # f2b_weight_var's dL/dweights against the reference's WeightVar: fp32 summation order only, the module's gradient bar.
+    # Measured on an H100 80GB HBM3 at 700 W: at most 1.9e-6 over both steps configs.
+    assert dw_rel <= 1e-5, f"dL/dweights, iteration {k}: relative L2 {dw_rel:.3g}"
+    use_app_emb = renderer.use_app_emb_                 # build_from_ref takes it from the run's scalars
     n_rays = int(st[1])
     voted_visits = N(sampler.tree_visit_cnt_)
     sampler.maintain((root["oct_intri"].reshape(-1, 3, 3), root["oct_w2c"].reshape(-1, 3, 4), root["oct_bound"]), compact_freq)
@@ -174,15 +196,19 @@ def replay(root, it, k, gen):
     assert abs(float(loss) - float(it["loss"][0])) <= 1e-6 * abs(float(it["loss"][0])), (k, float(loss), float(it["loss"][0]))
     g_table = np.zeros(it["feat_pool"].size, np.float32)
     g_table[it["grad_feat_pool_nz_idx"]] = it["grad_feat_pool_nz_val"]
-    rel = {name: rel_l2(N(g), want) for name, g, want in (
-        ("field_mlp", field.mlp_.params_.grad, it["grad_field_mlp"]), ("shader_mlp", shader.mlp_.params_.grad, it["grad_shader_mlp"]),
-        ("app_emb", renderer.app_emb_.grad, it["grad_app_emb"]), ("feat_pool", field.feat_pool_.grad, g_table))}
+    groups = [("field_mlp", field.mlp_.params_.grad, it["grad_field_mlp"]), ("shader_mlp", shader.mlp_.params_.grad, it["grad_shader_mlp"]),
+              ("feat_pool", field.feat_pool_.grad, g_table)]
+    if use_app_emb:
+        groups.append(("app_emb", renderer.app_emb_.grad, it["grad_app_emb"]))
+    else:                                               # the embedding takes no part: neither host gives it a gradient
+        assert "grad_app_emb" not in it and renderer.app_emb_.grad is None, f"embedding gradient, iteration {k}"
+    rel = {name: rel_l2(N(g), want) for name, g, want in groups}
     noise = None
     if rel["feat_pool"] > 1e-5:
         # The table gradient is summed with fp32 atomics in no fixed order, so two runs of the same host differ too: the same
         # iteration once more on the Python host measures that noise, and the C++ host may differ by no more than a few times it
         # (a stale or wrongly zeroed gradient storage differs by O(1)).
-        objs2, _, _ = python_step(root, it, k, gen)
+        objs2, _, _, _ = python_step(root, it, k, gen)
         check_nonfinite(objs2[4], it, False)
         noise = rel_l2(N(objs2[2].feat_pool_.grad), N(field.feat_pool_.grad))
     for name, v in rel.items():
@@ -200,12 +226,27 @@ def replay(root, it, k, gen):
                 nodes_after=it["after_tree_nodes"].size // 64, leaves_before=valid_leaves(it["tree_nodes"]),
                 leaves_after=valid_leaves(it["after_tree_nodes"]), voted_visits=int(voted_visits.sum()),
                 visits_after=int(it["after_visit_cnt"].sum()), grad_reused=int(it["after"][5]), grad_fresh=int(it["after"][6]),
-                grad_rel_l2=rel, table_grad_self_noise=noise)
+                grad_rel_l2=rel, table_grad_self_noise=noise, d_weights_rel_l2=dw_rel)
 
 
 def test_fused_cpp_host_equals_python_host_each_iteration():
     """a. and c. of the module text"""
-    run = _run("fused", 0)
+    recs = replay_run(CONFIG, "cpp_host_steps_fused_vs_python.json")
+    gs = [r["gs_progress"] for r in recs]
+    assert gs[0] < 1 and gs[-1] >= 1 and any(0 < g < 1 for g in gs), gs
+
+
+def test_fused_cpp_host_equals_python_host_each_iteration_free():
+    """a. and c. of the module text on the free settings: no embedding gradient in either host, fineness 4 decaying"""
+    recs = replay_run(FREE_CONFIG, "cpp_host_steps_free_fused_vs_python.json")
+    assert all(r["gs_progress"] == 1 for r in recs), [r["gs_progress"] for r in recs]
+    fin = [r["fineness"] for r in recs]
+    assert fin[0] == 4 and all(b < a for a, b in zip(fin, fin[1:])) and fin[-1] > 1, fin
+
+
+def replay_run(config, diag_name):
+    """a. and the schedule coverage of c. common to both steps configs -> per-iteration records"""
+    run = _run("fused", 0, config)
     root = run["root"]
     gen = ray_generator(root)
     recs = []
@@ -213,7 +254,7 @@ def test_fused_cpp_host_equals_python_host_each_iteration():
         for k, it in enumerate(run["its"]):
             recs.append(replay(root, it, k, gen))
     finally:
-        json.dump(recs, open(diag_path("cpp_host_steps_fused_vs_python.json"), "w"), indent=1)
+        json.dump(recs, open(diag_path(diag_name), "w"), indent=1)
     # c. what the run covered
     assert [r["iter_step"] for r in recs] == list(range(N_ITERS))
     r0 = recs[0]
@@ -225,15 +266,27 @@ def test_fused_cpp_host_equals_python_host_each_iteration():
     assert any(r["compaction"] for r in split), "no milestone on a compaction iteration"
     n = [r["n_rays"] for r in recs]
     assert any(b < a for a, b in zip(n, n[1:])) and len(set(n)) > 2, n
-    gs = [r["gs_progress"] for r in recs]
-    assert gs[0] < 1 and gs[-1] >= 1 and any(0 < g < 1 for g in gs), gs
     assert recs[0]["grad_fresh"] == 1 and recs[-1]["grad_reused"] >= 1, (recs[0], recs[-1])
+    return recs
 
 
 @pytest.mark.parametrize("kind", ["fused", "ops"])
 def test_hosts_against_unmodified_program(kind):
     """b. of the module text"""
-    ref, mine = _run("ref", FIXED_BATCH), _run(kind, FIXED_BATCH)
+    hosts_against_unmodified_program(kind, CONFIG, f"cpp_host_steps_margins_{kind}.json")
+
+
+@pytest.mark.parametrize("kind", ["fused", "ops"])
+def test_hosts_against_unmodified_program_free(kind):
+    """b. of the module text on the free settings"""
+    ref = hosts_against_unmodified_program(kind, FREE_CONFIG, f"cpp_host_steps_free_margins_{kind}.json")
+    assert all("grad_app_emb" not in it for it in ref["its"])
+
+
+def hosts_against_unmodified_program(kind, config, diag_name):
+    ref, mine = _run("ref", FIXED_BATCH, config), _run(kind, FIXED_BATCH, config)
+    for it in mine["its"]:
+        assert ("grad_app_emb" in it) == ("grad_app_emb" in ref["its"][0]), "the arms disagree on the embedding gradient"
     a0, b0 = ref["its"][0], mine["its"][0]
     for name in ("rays_o", "rays_d", "emb_idx", "sample_bounds", "sample_anchors", "sample_pts", "sample_dt", "sample_t", "first_oct_dis"):
         np.testing.assert_array_equal(bits(b0[name]), bits(a0[name]), err_msg=f"{name}, iteration 0")
@@ -249,10 +302,11 @@ def test_hosts_against_unmodified_program(kind):
                  or milestones(a["after_milestones"]) != milestones(a["milestones"]))
         margins.append(dict(iteration=k, loss_ref=la, loss=lb, loss_rel=abs(lb - la) / abs(la), maintenance=bool(maint),
                             nodes_ref=int(na), nodes=int(nb), nodes_rel=abs(nb - na) / na))
-    json.dump(margins, open(diag_path(f"cpp_host_steps_margins_{kind}.json"), "w"), indent=1)
+    json.dump(margins, open(diag_path(diag_name), "w"), indent=1)
     assert max(m["loss_rel"] for m in margins) <= LOSS_REL_BAR, margins
     assert sum(m["maintenance"] for m in margins) >= 4, margins
     assert max(m["nodes_rel"] for m in margins if m["maintenance"]) <= NODES_REL_BAR, margins
+    return ref
 
 
 def test_nonfinite_backward_backs_off_the_field_loss_scale(tmp_path):
@@ -272,7 +326,7 @@ def test_nonfinite_backward_backs_off_the_field_loss_scale(tmp_path):
     assert seqs["fused"] == seqs["ref"]
     # the Python host from the C++ run's state at iteration 0: the same flags, the same two loss scales afterwards
     run = _run("fused", FIXED_BATCH, config, 3)
-    (gdp, _, field, shader, renderer), _, _ = python_step(run["root"], run["its"][0], 0, ray_generator(run["root"]))
+    (gdp, _, field, shader, renderer), _, _, _ = python_step(run["root"], run["its"][0], 0, ray_generator(run["root"]))
     check_nonfinite(renderer, run["its"][0], True)
     assert gdp.backward_nan_
     assert (field.mlp_.loss_scale_, shader.mlp_.loss_scale_) == tuple(run["its"][1]["state"][4:6].tolist()), (

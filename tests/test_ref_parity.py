@@ -59,6 +59,21 @@ def n_rays_of(ref):
     return int(ref["scalars"][7])
 
 
+def margin_path(ref, name):
+    """Where a check on ``ref`` writes its measured margins: diag_path(name), prefixed by ref["_tag"] for a run of another
+    config (tests/test_gpu_ref_configs.py)"""
+    return diag_path(name if "_tag" not in ref else f"{ref['_tag']}_{name}")
+
+
+def run_settings(ref):
+    """(use_app_emb, ray-march fineness, gradient-scaling progress) the reference's seeded batches ran with.  A scalars vector of
+    8 entries predates them: the wanjinyou settings ref_driver then hard-coded (embedding on, fineness 1, progress 0.25)."""
+    sc = ref["scalars"]
+    if sc.size < 11:
+        return True, 1.0, 0.25
+    return bool(sc[8]), float(sc[9]), float(sc[10])
+
+
 def stored_rows(ref, a, bounds_key):
     """Our per-sample tensor ``a`` restricted to the rays whose samples ``ref`` holds: all rays, unless it stores the
     segments of ``sample_rays`` only ([begin, end) row ranges per ray in ``ref[bounds_key]``, concatenated in ray order)."""
@@ -71,7 +86,9 @@ def build_from_ref(ref):
     from f2nerf_b200 import GlobalDataPool, Hash3DAnchored, PersSampler, Renderer, SHShader
     sc = ref["scalars"]
     near, sample_l, scale_by_dis, max_hits, V, pool, n_img = float(sc[0]), float(sc[1]), bool(sc[2]), int(sc[3]), int(sc[4]), int(sc[5]), int(sc[6])
+    use_app_emb, fineness, _ = run_settings(ref)
     gdp = GlobalDataPool()
+    gdp.ray_march_fineness_ = fineness                            # VALIDATE noise is fineness too (PersSampler.cu:373-381)
     sampler = PersSampler(gdp, ref["tree_nodes"], ref["pers_trans"], ref["edge_pool"], near=near, sample_l=sample_l,
                           scale_by_dis=scale_by_dis, max_oct_intersect_per_ray=max_hits)
     assert gdp.n_volumes_ == V
@@ -82,7 +99,7 @@ def build_from_ref(ref):
     field.mlp_.params_.data.copy_(T(ref["field_mlp_params"]))
     shader = SHShader(gdp)
     shader.mlp_.params_.data.copy_(T(ref["shader_mlp_params"]))
-    renderer = Renderer(gdp, sampler, field, shader, n_images=n_img, use_app_emb=True)
+    renderer = Renderer(gdp, sampler, field, shader, n_images=n_img, use_app_emb=use_app_emb)
     renderer.app_emb_.data.copy_((torch.rand((n_img, 16), generator=g) * .2 - .1).cuda())
     np.testing.assert_array_equal(N(renderer.app_emb_), ref["app_emb"])
     return gdp, sampler, field, shader, renderer
@@ -133,8 +150,11 @@ def test_render_validate_vs_reference(ref):
     mine, theirs = N(r.idx_start_end), ref["val_idx_start_end"]
     cnt_m, cnt_t = mine[:, 1] - mine[:, 0], theirs[:, 1] - theirs[:, 0]
     frac_rays_same = (cnt_m == cnt_t).mean()
+    col_err, depth_rel = np.abs(N(r.colors) - ref["val_colors"]), np.abs(N(r.depth) - ref["val_depth"]) / (np.abs(ref["val_depth"]) + 1e-3)
     json.dump(dict(frac_rays_same_count=float(frac_rays_same), max_count_diff=int(np.abs(cnt_m - cnt_t).max()),
-                   kept_mine=int(cnt_m.sum()), kept_ref=int(cnt_t.sum())), open(diag_path("ref_validate_mask.json"), "w"))
+                   kept_mine=int(cnt_m.sum()), kept_ref=int(cnt_t.sum()), colors_max=float(col_err.max()),
+                   colors_median=float(np.median(col_err)), depth_rel_median=float(np.median(depth_rel))),
+              open(margin_path(ref, "ref_validate_mask.json"), "w"))
     # the T > 1e-4 crossing sits downstream of the fp16 MLP: tcnn's fp16-accumulate noise shifts it by a few samples
     assert frac_rays_same >= 0.9 and abs(int(cnt_m.sum()) - int(cnt_t.sum())) <= 2e-3 * cnt_t.sum(), (frac_rays_same, cnt_m.sum(), cnt_t.sum())
     assert np.abs(N(r.colors) - ref["val_colors"]).max() <= 0.03
@@ -152,7 +172,7 @@ def test_edge_samples_vs_reference(ref):
     np.testing.assert_array_equal(N(idx), ref["edge_anchors"])
     diff = np.abs(N(pts).astype(np.float64) - ref["edge_pts"].astype(np.float64))
     json.dump(dict(max_abs=float(diff.max()), frac_bit_exact=float((N(pts).view(np.uint32) == ref["edge_pts"].view(np.uint32)).mean())),
-              open(diag_path("ref_edge_samples.json"), "w"))
+              open(margin_path(ref, "ref_edge_samples.json"), "w"))
     np.testing.assert_array_equal(N(pts).view(np.uint32), ref["edge_pts"].view(np.uint32))       # bit-exact
     torch.manual_seed(4242)                                       # same Philox stream => identical draws through our mirror
     e_pts, e_idx = sampler.GetEdgeSamples(8192)
@@ -165,7 +185,8 @@ def test_render_train_vs_reference(ref):
     """Seeded TRAIN-mode step: same torch RNG draws, octree votes bit-exact, gradients close."""
     from f2nerf_b200 import TRAIN, CustomOps, check_backward_nan
     gdp, sampler, field, shader, renderer = build_from_ref(ref)
-    gdp.mode_, gdp.iter_step_, gdp.ray_march_fineness_, gdp.gradient_scaling_progress_ = TRAIN, 1, 1.0, 0.25
+    use_app_emb, fineness, gs_progress = run_settings(ref)
+    gdp.mode_, gdp.iter_step_, gdp.ray_march_fineness_, gdp.gradient_scaling_progress_ = TRAIN, 1, fineness, gs_progress
     rays_o, rays_d, emb_idx, gt = T(ref["rays_o"]), T(ref["rays_d"]), T(ref["emb_idx"]), T(ref["gt_colors"])
     torch.manual_seed(777)
     noise = sampler.make_noise(n_rays_of(ref), rays_o.device)
@@ -191,7 +212,11 @@ def test_render_train_vs_reference(ref):
     assert not check_backward_nan(renderer) and ref["backward_nan"][0] == 0
     assert abs(float(loss) - float(ref["train_loss"][0])) <= 5e-3 * abs(float(ref["train_loss"][0]))
     assert np.abs(N(r.colors) - ref["train_colors"]).max() <= 0.03
-    summary = {}
+    summary = dict(loss_rel=abs(float(loss) - float(ref["train_loss"][0])) / abs(float(ref["train_loss"][0])),
+                   colors_max=float(np.abs(N(r.colors) - ref["train_colors"]).max()),
+                   stats_flip_frac={k: float((N(m) != ref[k]).mean()) for m, k in (
+                       (sampler.tree_weight_stats_, "train_weight_stats_after"), (sampler.tree_alpha_stats_, "train_alpha_stats_after"),
+                       (sampler.tree_visit_cnt_, "train_visit_cnt_after"), (sampler.tree_nodes_gpu_, "train_tree_nodes_after"))})
     if "train_edge_feats" in ref:                     # same Philox draws => same edge points => same features (fp16 MLP noise)
         from f2nerf_b200 import ops as _ops
         from f2nerf_b200.field import field_forward
@@ -210,18 +235,24 @@ def test_render_train_vs_reference(ref):
                                      frac_rows_close=float(row_close.mean()), frac_rows_close_a=float(row_close[:, 0].mean()),
                                      frac_rows_close_b=float(row_close[:, 1].mean()),
                                      per_channel_cos=[cs(ef_m[..., k], ef_t[..., k]) for k in range(16)])
-        json.dump(summary, open(diag_path("ref_edge_feats.json"), "w"), indent=1)
+        json.dump(summary, open(margin_path(ref, "ref_edge_feats.json"), "w"), indent=1)
         # identical edge points (RNG-stream parity incl. the reference's torch::rand output buffers): fp16 MLP noise only
         assert summary["edge_feats"]["cos_ours_ref"] >= 0.999 and summary["edge_feats"]["frac_rows_close"] >= 0.97, summary["edge_feats"]
     if "grad_feat_pool" in ref:
         table_pair = (field.feat_pool_.grad.reshape(-1), ref["grad_feat_pool"])
-    else:                                             # committed fixture: a seeded 2^18-element subsample of the live prefix
+    elif "grad_feat_pool_sub_idx" in ref:             # committed fixture: a seeded 2^18-element subsample of the live prefix
         sub = torch.from_numpy(ref["grad_feat_pool_sub_idx"]).long().cuda()
         table_pair = (field.feat_pool_.grad.reshape(-1)[sub], ref["grad_feat_pool_sub_val"])
-    for name, mine, theirs in (("field_mlp", field.mlp_.params_.grad, ref["grad_field_mlp"]),
-                               ("shader_mlp", shader.mlp_.params_.grad, ref["grad_shader_mlp"]),
-                               ("app_emb", renderer.app_emb_.grad, ref["grad_app_emb"]),
-                               ("feat_pool",) + table_pair):
+    else:                                             # a run without the dense table gradient: the reference's non-zero entries
+        nz = torch.from_numpy(ref["grad_feat_pool_nz_idx"]).long().cuda()
+        table_pair = (field.feat_pool_.grad.reshape(-1)[nz], ref["grad_feat_pool_nz_val"])
+    groups = [("field_mlp", field.mlp_.params_.grad, ref["grad_field_mlp"]), ("shader_mlp", shader.mlp_.params_.grad, ref["grad_shader_mlp"])]
+    if use_app_emb:
+        groups.append(("app_emb", renderer.app_emb_.grad, ref["grad_app_emb"]))
+    else:                                             # the embedding takes no part in the step: the reference leaves it undefined
+        assert "grad_app_emb" not in ref
+        assert renderer.app_emb_.grad is None or not renderer.app_emb_.grad.any()
+    for name, mine, theirs in groups + [("feat_pool",) + table_pair]:
         a, b = N(mine).astype(np.float64).reshape(-1), theirs.astype(np.float64).reshape(-1)
         cos = float((a * b).sum() / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-30))
         rel = float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
@@ -229,10 +260,15 @@ def test_render_train_vs_reference(ref):
     if "grad_feat_pool" not in ref:
         S = field.local_size_
         mine_flat = field.feat_pool_.grad.reshape(-1).double()
+        if "grad_feat_pool_slab_norm" in ref:
+            ref_norms = ref["grad_feat_pool_slab_norm"].astype(np.float64)
+        else:
+            nz_idx, nz_val = ref["grad_feat_pool_nz_idx"], ref["grad_feat_pool_nz_val"].astype(np.float64)
+            ref_norms = np.array([np.linalg.norm(nz_val[(nz_idx >= l * S) & (nz_idx < (l + 1) * S)]) for l in range(17)])
         norms = np.array([float(torch.linalg.norm(mine_flat[l * S:(l + 1) * S])) for l in range(17)])
-        summary["slab_norm_ratio"] = (norms / np.maximum(ref["grad_feat_pool_slab_norm"].astype(np.float64), 1e-30)).tolist()
-        json.dump(summary, open(diag_path("golden_grad_parity.json"), "w"), indent=1)
-        for name in ("field_mlp", "shader_mlp", "app_emb"):
+        summary["slab_norm_ratio"] = (norms / np.maximum(ref_norms, 1e-30)).tolist()
+        json.dump(summary, open(margin_path(ref, "golden_grad_parity.json"), "w"), indent=1)
+        for name, _, _ in groups:
             assert summary[name]["cos"] >= 0.98 and summary[name]["rel_l2"] <= 0.2, (name, summary[name])
         assert summary["feat_pool"]["cos"] >= 0.97, summary
         assert all(0.8 <= r <= 1.25 for r in summary["slab_norm_ratio"] if np.isfinite(r)), summary["slab_norm_ratio"]
@@ -247,8 +283,8 @@ def test_render_train_vs_reference(ref):
     fld = dict(table16=N(field.table_f16()), prim=N(field.prim_pool_), bias=N(field.bias_pool_), V=field.n_volumes_,
                local_size=field.local_size_, mlp_params=ref["field_mlp_params"])
     orc = OP.render_train(sc, ref["rays_o"], ref["rays_d_normed"], ref["train_noise"], ref["train_bg"], fld, ref["shader_mlp_params"],
-                          ref["app_emb"], ref["emb_idx"], (ref["train_edge_idx"], ref["train_edge_coord"]), ref["gt_colors"],
-                          scales=ops.hash_level_scales().numpy(), gs_progress=0.25, diagnostics=True)
+                          ref["app_emb"] if use_app_emb else None, ref["emb_idx"], (ref["train_edge_idx"], ref["train_edge_coord"]),
+                          ref["gt_colors"], scales=ops.hash_level_scales().numpy(), gs_progress=gs_progress, diagnostics=True)
     def cosd(x, y):
         x, y = np.asarray(x, np.float64).reshape(-1), np.asarray(y, np.float64).reshape(-1)
         return float((x * y).sum() / (np.linalg.norm(x) * np.linalg.norm(y) + 1e-30))
@@ -271,8 +307,8 @@ def test_render_train_vs_reference(ref):
                           norm_ref=float(np.linalg.norm(gref[sl])), norm_ours=float(np.linalg.norm(mine_flat[sl])),
                           nnz_ref=int((gref[sl] != 0).sum()), nnz_ours=int((mine_flat[sl] != 0).sum())))
     summary["feat_pool_slabs"] = slabs
-    json.dump(summary, open(diag_path("ref_grad_parity.json"), "w"), indent=1)
-    for name in ("field_mlp", "shader_mlp", "app_emb"):
+    json.dump(summary, open(margin_path(ref, "ref_grad_parity.json"), "w"), indent=1)
+    for name, _, _ in groups:
         assert summary[name]["cos"] >= 0.98 and summary[name]["rel_l2"] <= 0.2, (name, summary[name])
     assert summary["feat_pool_ours_vs_oracle_exact"] >= 0.995, summary
     # Ours equals the exact sum (oracle, double accumulation) to 1e-9; what is left against the reference is its own

@@ -13,6 +13,7 @@ bit for bit on every deterministic output: the two are the same kernel sequence.
 """
 import json
 import os
+import shutil
 import subprocess
 
 import numpy as np
@@ -31,27 +32,33 @@ N_RAYS = 512
 _runs = {}
 
 
-def _run(kind):
-    if kind in _runs:
-        return _runs[kind]
+def _run(kind, config="ref_config_ngp_fox.yaml", args=("0", "1")):
+    """One arm's run of the seeded 512-ray script: "ref" (unmodified), "fused" or "ops", on oracle/<config> with the trailing
+    ref_driver arguments ``args`` ([n_time_iters, dump_full_grads, fineness, gs_progress])"""
+    key = (kind, config, tuple(args))
+    if key in _runs:
+        return _runs[key]
     binary = REF if kind == "ref" else B200
     if not os.path.exists(binary):
         pytest.skip(f"{binary} not built (build() makes it from /root/reference)")
-    out = f"/tmp/f2b_shim_{kind}"
+    tag = kind + ("" if config == "ref_config_ngp_fox.yaml" else "_" + os.path.splitext(config)[0][len("ref_config_"):])
+    out = f"/tmp/f2b_shim_{tag}"
+    shutil.rmtree(out, ignore_errors=True)
     env = dict(os.environ)
     env.pop("F2B_SHIM", None); env.pop("F2B_RENDER", None)
     if kind == "ops":
         env["F2B_SHIM"] = "ops"
-    r = subprocess.run([binary, os.path.join(ROOT, "oracle", "ref_config_ngp_fox.yaml"), out, str(N_RAYS), "0", "1"],
+    r = subprocess.run([binary, os.path.join(ROOT, "oracle", config), out, str(N_RAYS), *args],
                        cwd=ROOT, capture_output=True, text=True, timeout=900, env=env)
-    open(diag_path(f"shim_{kind}.log"), "w").write(r.stdout[-8000:] + "\n--- stderr ---\n" + r.stderr[-8000:])
+    open(diag_path(f"shim_{tag}.log"), "w").write(r.stdout[-8000:] + "\n--- stderr ---\n" + r.stderr[-8000:])
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
     if kind == "ops":
         assert "replaced by the B200 subclasses" in r.stdout
     if kind == "fused":
         assert "replaced by the fused B200 host" in r.stdout
-    _runs[kind] = {f[:-4]: np.load(os.path.join(out, f)) for f in os.listdir(out) if f.endswith(".npy")}
-    return _runs[kind]
+    _runs[key] = {f[:-4]: np.load(os.path.join(out, f)) for f in os.listdir(out) if f.endswith(".npy")}
+    shutil.rmtree(out, ignore_errors=True)
+    return _runs[key]
 
 
 @pytest.fixture(params=["fused", "ops"])
@@ -70,8 +77,40 @@ def _node_fields(blob):
     return np.concatenate([t[:, :53], t[:, 56:60]], 1)
 
 
+def grad_of(d, name):
+    """A gradient group of a run as (sorted flat indices of its non-zero entries, float64 values).  A run without the dense
+    table gradient (dump_full_grads 0) holds the table's as its non-zero entries."""
+    if name == "grad_feat_pool" and name not in d:
+        return d["grad_feat_pool_nz_idx"].astype(np.int64), d["grad_feat_pool_nz_val"].astype(np.float64)
+    v = d[name].astype(np.float64).reshape(-1)
+    i = np.flatnonzero(v)
+    return i, v[i]
+
+
+def aligned(a, b):
+    """Two (indices, values) gradients -> dense float64 vectors over the union of their supports"""
+    u = np.union1d(a[0], b[0])
+    x, y = np.zeros(u.size), np.zeros(u.size)
+    x[np.searchsorted(u, a[0])], y[np.searchsorted(u, b[0])] = a[1], b[1]
+    return x, y
+
+
+def grad_groups(ref, *arms):
+    """The gradient groups the run takes: every group, less the appearance embedding when the config has none — which no
+    arm may then produce (the reference leaves its gradient undefined)"""
+    from test_ref_parity import run_settings
+    if run_settings(ref)[0]:
+        return GRAD_GROUPS
+    for d in (ref,) + arms:
+        assert "grad_app_emb" not in d
+    return tuple(g for g in GRAD_GROUPS if g != "grad_app_emb")
+
+
 def test_same_scene(pair):
-    a, b, _ = pair
+    check_same_scene(*pair[:2])
+
+
+def check_same_scene(a, b):
     np.testing.assert_array_equal(_node_fields(a["tree_nodes"]), _node_fields(b["tree_nodes"]))
     for k in ("pers_trans", "edge_pool", "prim_pool", "bias_pool", "field_mlp_params", "shader_mlp_params", "app_emb",
               "rays_o", "rays_d", "train_noise", "train_bg", "train_edge_idx", "train_edge_coord"):
@@ -79,7 +118,10 @@ def test_same_scene(pair):
 
 
 def test_sampler_through_reference_program(pair):
-    a, b, _ = pair
+    check_sampler(*pair[:2])
+
+
+def check_sampler(a, b):
     for k in ("val_bounds", "val_anchors", "train_bounds", "train_anchors", "edge_anchors"):
         np.testing.assert_array_equal(a[k], b[k], err_msg=k)
     for k in ("val_pts", "val_dt", "val_t", "val_first_oct_dis", "train_pts", "train_dt", "train_t", "train_first_oct_dis", "edge_pts"):
@@ -87,7 +129,10 @@ def test_sampler_through_reference_program(pair):
 
 
 def test_render_through_reference_program(pair):
-    a, b, kind = pair
+    check_render(*pair)
+
+
+def check_render(a, b, kind):
     for mode in ("val", "train"):
         ca, cb = a[f"{mode}_idx_start_end"], b[f"{mode}_idx_start_end"]
         na, nb = ca[:, 1] - ca[:, 0], cb[:, 1] - cb[:, 0]
@@ -106,9 +151,9 @@ def test_render_through_reference_program(pair):
     assert (_node_fields(a["train_tree_nodes_after"]) != _node_fields(b["train_tree_nodes_after"])).mean() <= 1e-4
     ef_a, ef_b = a["train_edge_feats"], b["train_edge_feats"]
     assert cos(ef_a, ef_b) >= 0.999
-    for name in ("grad_field_mlp", "grad_shader_mlp", "grad_app_emb"):
-        assert cos(a[name], b[name]) >= 0.98, (kind, name, cos(a[name], b[name]))
-    assert cos(a["grad_feat_pool"], b["grad_feat_pool"]) >= 0.97, (kind, cos(a["grad_feat_pool"], b["grad_feat_pool"]))
+    for name in grad_groups(a, b):
+        c = cos(*aligned(grad_of(a, name), grad_of(b, name)))
+        assert c >= (0.97 if name == "grad_feat_pool" else 0.98), (kind, name, c)
 
 
 GRAD_GROUPS = ("grad_field_mlp", "grad_shader_mlp", "grad_app_emb", "grad_feat_pool")
@@ -125,32 +170,54 @@ OPS_VS_FUSED_REL_BAR = 1e-5
 
 def test_step_gradient_magnitudes(pair):
     a, b, kind = pair
-    ratios = {k: float(np.log(np.linalg.norm(b[k].astype(np.float64)) / np.linalg.norm(a[k].astype(np.float64))))
-              for k in GRAD_GROUPS}
-    open(diag_path(f"shim_norm_ratio_{kind}.json"), "w").write(json.dumps(ratios))
-    assert all(abs(v) <= STEP_NORM_RATIO_BAR for v in ratios.values()), (kind, ratios)
+    check_step_gradient_magnitudes(a, b, f"shim_norm_ratio_{kind}.json")
+
+
+def check_step_gradient_magnitudes(a, b, diag_name):
+    ratios = {k: float(np.log(np.linalg.norm(grad_of(b, k)[1]) / np.linalg.norm(grad_of(a, k)[1]))) for k in grad_groups(a, b)}
+    open(diag_path(diag_name), "w").write(json.dumps(ratios))
+    assert all(abs(v) <= STEP_NORM_RATIO_BAR for v in ratios.values()), (diag_name, ratios)
+    return ratios
 
 
 def test_ops_arm_equals_fused_arm():
-    o, f = _run("ops"), _run("fused")
-    rel = {k: float(np.linalg.norm(o[k].astype(np.float64) - f[k]) / np.linalg.norm(f[k].astype(np.float64))) for k in GRAD_GROUPS}
-    open(diag_path("shim_ops_vs_fused.json"), "w").write(json.dumps(rel))
-    assert all(v <= OPS_VS_FUSED_REL_BAR for v in rel.values()), rel
+    check_ops_arm_equals_fused_arm(_run("ops"), _run("fused"), "shim_ops_vs_fused.json")
+
+
+def check_ops_arm_equals_fused_arm(o, f, diag_name):
+    rel = {}
+    for k in grad_groups(f, o):
+        x, y = aligned(grad_of(o, k), grad_of(f, k))
+        rel[k] = float(np.linalg.norm(x - y) / np.linalg.norm(y))
+    open(diag_path(diag_name), "w").write(json.dumps(rel))
+    assert all(v <= OPS_VS_FUSED_REL_BAR for v in rel.values()), (diag_name, rel)
+    return rel
 
 
 def test_fused_cpp_host_equals_python_host():
     """B200Renderer.cpp and f2nerf_b200/renderer.py are the same kernel sequence: every deterministic output of the seeded
     TRAIN step is bit-identical; the atomically accumulated gradients agree to fp32 summation order."""
-    from test_ref_parity import build_from_ref
+    check_fused_cpp_host_equals_python_host(_run("fused"))
+
+
+def check_fused_cpp_host_equals_python_host(c):
+    """-> the Python host's renderer after the step"""
+    from test_ref_parity import build_from_ref, run_settings
     from f2nerf_b200 import TRAIN, CustomOps, check_backward_nan
-    c = _run("fused")
     gdp, sampler, field, shader, renderer = build_from_ref(c)
-    gdp.mode_, gdp.iter_step_, gdp.ray_march_fineness_, gdp.gradient_scaling_progress_ = TRAIN, 1, 1.0, 0.25
+    use_app_emb, fineness, gs_progress = run_settings(c)
+    gdp.mode_, gdp.iter_step_, gdp.ray_march_fineness_, gdp.gradient_scaling_progress_ = TRAIN, 1, fineness, gs_progress
     rays_o, rays_d, emb_idx, gt = T(c["rays_o"]), T(c["rays_d"]), T(c["emb_idx"]), T(c["gt_colors"])
     torch.manual_seed(777)
     r = renderer.Render(rays_o, rays_d, None, emb_idx)
     loss = (torch.sqrt((r.colors - gt) ** 2 + 1e-4).mean() + torch.sqrt(CustomOps.WeightVar(r.weights, r.idx_start_end) + 1e-2).mean() * 1e-2
             + (r.disparity ** 2).mean() * 1e-2 + ((r.edge_feats[:, 0] - r.edge_feats[:, 1]) ** 2).mean() * 1e-1)
+    # the shader MLP's input rows: column 0 is fp16(1 + the ray's embedding), or exactly 1 without one (Renderer.cpp:179-187)
+    col0 = r.colors.grad_fn.keepalive[-1]["mlp_in"][:renderer.n_kept_pts_, 0].float()
+    if use_app_emb:
+        assert float((col0 != 1).float().mean()) >= 0.5
+    else:
+        assert bool((col0 == 1).all()), int((col0 != 1).sum())
     loss.backward()
     assert not check_backward_nan(renderer)
     np.testing.assert_array_equal(N(r.idx_start_end), c["train_idx_start_end"])
@@ -162,7 +229,18 @@ def test_fused_cpp_host_equals_python_host():
         np.testing.assert_array_equal(N(v).reshape(-1), c[k].reshape(-1), err_msg=k)
     np.testing.assert_array_equal(_node_fields(N(sampler.tree_nodes_gpu_)), _node_fields(c["train_tree_nodes_after"]))
     assert abs(float(loss) - float(c["train_loss"][0])) <= 1e-6 * abs(float(loss))
-    for name, g in (("grad_field_mlp", field.mlp_.params_.grad), ("grad_shader_mlp", shader.mlp_.params_.grad),
-                    ("grad_app_emb", renderer.app_emb_.grad), ("grad_feat_pool", field.feat_pool_.grad)):
-        a, b = N(g).astype(np.float64).reshape(-1), c[name].astype(np.float64).reshape(-1)
-        assert np.linalg.norm(a - b) <= 1e-5 * np.linalg.norm(b), (name, np.linalg.norm(a - b) / np.linalg.norm(b))
+    mine = {"grad_field_mlp": field.mlp_.params_.grad, "grad_shader_mlp": shader.mlp_.params_.grad,
+            "grad_app_emb": renderer.app_emb_.grad, "grad_feat_pool": field.feat_pool_.grad}
+    if not use_app_emb:
+        assert renderer.app_emb_.grad is None or not renderer.app_emb_.grad.any()
+    for name in grad_groups(c):
+        g = mine[name].reshape(-1)
+        if name == "grad_feat_pool" and name not in c:                  # the run's non-zero entries, scattered on the device
+            want = torch.zeros_like(g)
+            want[T(c["grad_feat_pool_nz_idx"]).long()] = T(c["grad_feat_pool_nz_val"])
+            err, ref_norm = float(torch.linalg.norm((g - want).double())), float(torch.linalg.norm(want.double()))
+        else:
+            a, b = N(g).astype(np.float64), c[name].astype(np.float64).reshape(-1)
+            err, ref_norm = float(np.linalg.norm(a - b)), float(np.linalg.norm(b))
+        assert err <= 1e-5 * ref_norm, (name, err / ref_norm)
+    return renderer

@@ -68,10 +68,12 @@ def diag_path(name):
 def load_golden(batch="ref_ngp_fox"):
     """A reference-parity fixture (oracle/make_golden.py): the scene of the reference run, its dumps of the seeded ray batch and
     a sample of its optimizer step, in one dict.  ``batch``: "ref_ngp_fox" (8 rays, every per-sample tensor) or
-    "ref_ngp_fox_512" (512 rays, per-sample tensors of the rays listed in ``sample_rays``)."""
+    "ref_ngp_fox_512" (512 rays, per-sample tensors of the rays listed in ``sample_rays``) or "ref_free_512" (that batch under the
+    free config's settings, without an optimizer sample)."""
     d = os.path.join(ROOT, "tests", "golden")
+    adam = os.path.join(d, batch + "_adam.npz")
     return dict(np.load(os.path.join(d, batch + "_run.npz")), **np.load(os.path.join(d, batch + "_rays.npz")),
-                **np.load(os.path.join(d, batch + "_adam.npz")))
+                **(np.load(adam) if os.path.exists(adam) else {}))
 
 
 def scene_blobs(cfg_name):

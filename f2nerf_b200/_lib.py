@@ -56,6 +56,9 @@ SIGNATURES = {
     "f2b_locate_points": [_P, c_int, _P, _P, c_int, _P, _P, _P],
     "f2b_query_logit_points": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_float, _P, _P],
     "f2b_query_logit_grid": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _P],
+    "f2b_warp_jacobian_points": [_P, c_int, _P, _P, c_int, _P, _P],
+    "f2b_query_grad_points": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_float, _P, _P, _P],
+    "f2b_render_normals_slots": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_iso_count": [_P, c_int, c_int, c_int, c_float, c_float, c_int, c_int, _P, _P, _P, _P],
     "f2b_iso_emit": [_P, c_int, c_int, c_int, c_float, c_float, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P],
     "f2b_field_shade_fwd": [_P, _P, _P, _P, _P, c_int, _P, _P, _P, _P],

@@ -36,6 +36,21 @@ __global__ void locate_points_kernel(const TreeNode* __restrict__ nodes, const T
   anchors[2 * size_t(i)] = ti; anchors[2 * size_t(i) + 1] = leaf;
 }
 
+// QueryFrameTransformJac at located points (DESIGN §3j): J [n,3,3] row-major, d warp_r / d x_c; 0 where no valid leaf holds the point
+__global__ void warp_jacobian_points_kernel(const TreeNode* __restrict__ nodes, const TransInfo* __restrict__ trans,
+                                            const float* __restrict__ pts, int n, float* __restrict__ jac) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float x = pts[3 * size_t(i)], y = pts[3 * size_t(i) + 1], z = pts[3 * size_t(i) + 2];
+  int ti = -1;
+  float J[3][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+  if (locate_leaf(nodes, x, y, z, ti) >= 0) warp_jacobian(trans + ti, x, y, z, J);
+#pragma unroll
+  for (int r = 0; r < 3; r++)
+#pragma unroll
+    for (int c = 0; c < 3; c++) jac[9 * size_t(i) + 3 * r + c] = J[r][c];
+}
+
 // ---- marching tetrahedra ------------------------------------------------------------------------------------------
 // The six Kuhn tetrahedra of a cell, corners as offset codes (bit 0 x, bit 1 y, bit 2 z), ordered by the axis
 // permutations xyz, xzy, yxz, yzx, zxy, zyx, with the last two corners swapped for the odd permutations so that every
@@ -174,6 +189,15 @@ extern "C" int f2b_locate_points(const void* tree_nodes, int n_nodes, const void
   locate_points_kernel<<<div_up(n_pts, 128), 128, 0, as_stream(stream)>>>((const TreeNode*)tree_nodes, (const TransInfo*)trans,
                                                                           pts, n_pts, warped, anchors);
   return check_launch("f2b_locate_points");
+}
+
+extern "C" int f2b_warp_jacobian_points(const void* tree_nodes, int n_nodes, const void* trans, const float* pts, int n_pts,
+                                        float* jac, void* stream) {
+  if (n_pts <= 0) return F2B_OK;
+  F2B_REQUIRE(tree_nodes && n_nodes > 0 && trans && pts && jac, "f2b_warp_jacobian_points: bad argument");
+  warp_jacobian_points_kernel<<<div_up(n_pts, 128), 128, 0, as_stream(stream)>>>((const TreeNode*)tree_nodes, (const TransInfo*)trans,
+                                                                                 pts, n_pts, jac);
+  return check_launch("f2b_warp_jacobian_points");
 }
 
 static bool iso_slab_ok(int nx, int ny, int nz, int ez0, int ez1) {

@@ -73,6 +73,32 @@ __device__ __forceinline__ uint32_t encode_level(const __half* __restrict__ tabl
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
+// Gradient of one level's blend with respect to p (the level's grid coordinates, p = x * scale + bias), dotted with the level's
+// dL/dfeat (d0, d1): sum_c (d0 f_c.x + d1 f_c.y) dw_c/dp, the derivative inside the cell `corners` chose (floor has zero
+// derivative).  (a, b, cc) are the fractions p - floor(p) that `corners` formed; the 8 half2 corners are re-gathered as
+// encode_level does.  Used by the gradient kernel (field.cu, DESIGN §3j).
+__device__ __forceinline__ void grad_level(const __half* __restrict__ table, int l, int local_size, const Corner8& c, float a,
+                                           float b, float cc, float d0, float d1, float g[3]) {
+  const __half* base = table + size_t(l) * local_size;
+  uint32_t raw[8];
+#pragma unroll
+  for (int k = 0; k < 8; k++) raw[k] = ldg_nc_u32(base + size_t(c.idx[k]) * 2);
+  float s[8];
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&raw[k]));
+    s[k] = ffma(d0, f.x, fmul(d1, f.y));
+  }
+  const float na = fsub(1.f, a), nb = fsub(1.f, b), nc = fsub(1.f, cc);
+  // corner k = (bx, by, bz) = (k >> 2, k >> 1 & 1, k & 1); w_k = wa wb wc, so dw_k/da = (bx ? 1 : -1) wb wc, and so on
+  g[0] = ffma(fmul(b, cc), fsub(s[7], s[3]), ffma(fmul(b, nc), fsub(s[6], s[2]),
+              ffma(fmul(nb, cc), fsub(s[5], s[1]), fmul(fmul(nb, nc), fsub(s[4], s[0])))));
+  g[1] = ffma(fmul(a, cc), fsub(s[7], s[5]), ffma(fmul(a, nc), fsub(s[6], s[4]),
+              ffma(fmul(na, cc), fsub(s[3], s[1]), fmul(fmul(na, nc), fsub(s[2], s[0])))));
+  g[2] = ffma(fmul(a, b), fsub(s[7], s[6]), ffma(fmul(a, nb), fsub(s[5], s[4]),
+              ffma(fmul(na, b), fsub(s[3], s[2]), fmul(fmul(na, nb), fsub(s[1], s[0])))));
+}
+
 // Encode all 16 levels of one sample into 16 half2 words (registers).  Shared with field.cu.
 // `scales` = the 16 level scales computed AT RUN TIME (shared memory): a compile-time-folded exp2f
 // would be correctly rounded, MUFU.EX2 (what the reference executes) is not.

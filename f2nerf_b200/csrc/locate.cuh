@@ -29,6 +29,37 @@ __device__ __forceinline__ void warp_point(const TransInfo* __restrict__ T, floa
   }
 }
 
+// QueryFrameTransformJac (PersSampler.cu:171-187): J[r][c] = d warp_r / d x_c at (X, Y, Z), in the roundings of the march's
+// phases A and B (sampler.cu): per projection rr = rcp(xz1), q = -xz0 / xz1^2 and the rows fma(a, rr, b * q), then each
+// mixing sum in Eigen's redux tree ((g0 + g1) + (g2 + g3)).  One thread forms all nine entries (DESIGN §3j).
+__device__ __forceinline__ void warp_jacobian(const TransInfo* __restrict__ T, float X, float Y, float Z, float J[3][3]) {
+  float t0[12], t1[12], t2[12];
+#pragma unroll
+  for (int i = 0; i < 12; i++) {
+    const float* a = T->w2xz[i];
+    const float xz0 = fadd(ffma(X, a[0], fmul(Y, a[1])), ffma(Z, a[2], a[3]));
+    const float xz1 = fadd(ffma(X, a[4], fmul(Y, a[5])), ffma(Z, a[6], a[7]));
+    const float rr = frcp(xz1);
+    const float q = fdiv(-xz0, fmul(xz1, xz1));
+    t0[i] = ffma(a[0], rr, fmul(a[4], q));
+    t1[i] = ffma(rr, a[1], fmul(q, a[5]));
+    t2[i] = ffma(rr, a[2], fmul(q, a[6]));
+  }
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    const float* w = T->weight[r];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const float* v = c == 0 ? t0 : (c == 1 ? t1 : t2);
+      float g[4];
+#pragma unroll
+      for (int s = 0; s < 4; s++)
+        g[s] = ffma(w[3 * s], v[3 * s], ffma(w[3 * s + 1], v[3 * s + 1], fmul(w[3 * s + 2], v[3 * s + 2])));
+      J[r][c] = fadd(fadd(g[0], g[1]), fadd(g[2], g[3]));
+    }
+  }
+}
+
 // The march visits nodes down to depth 23 (its 24-entry stack, sampler.cu kMaxDepth); the walk stops at the same depth.
 constexpr int kLocateMaxDepth = 24;
 

@@ -110,6 +110,48 @@ def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_B
     return out[:, :3].contiguous(), out[:, 3:4].contiguous(), out[:, 4:5].contiguous()
 
 
+@torch.no_grad()
+def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None):
+    """-> normals [N,3] CPU float32: the normal map of the rays in the normalised scene frame (DESIGN.md §3j).  Per ray,
+    N = sum_i w_i n_i over the samples the VALIDATE render keeps, with n_i = -g_i / |g_i| the outward density normal and w_i the
+    render's weights; the result is N / |N|, 0 where N = 0 (rays that miss the scene included).  The rays are rendered in the
+    tiled loop of ``RenderWholeImage`` (two streams, ``render_forward`` per chunk), each chunk followed on its stream by the
+    normals kernel over the chunk's slots; one device->host copy at the end.  The sums run in a fixed order, so a view gets the
+    same bits on every run and for any ``ray_batch_size``.  Turning the map into camera coordinates is one rotation by the
+    camera's pose, left to the caller."""
+    from . import ops
+    dev = _device_of(renderer, device)
+    o, d = _to_dev(rays_o, dev), _to_dev(rays_d, dev)
+    n_rays = d.shape[0]
+    normals = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
+    if n_rays == 0:
+        return normals.cpu()
+    f = renderer.scene_field_
+    trans = renderer.pts_sampler_.pers_trans_gpu_
+    with _Validate(renderer):
+        main = torch.cuda.current_stream(dev)
+        lanes = [renderer._side_stream(dev, 3), renderer._side_stream(dev, 4)]
+        ready = torch.cuda.Event()
+        ready.record(main)
+        f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
+        unused = [(f32(ray_batch_size, 3), f32(ray_batch_size), f32(ray_batch_size)) for _ in lanes]   # colours etc., per lane
+        alive = []
+        for k, i in enumerate(range(0, n_rays, ray_batch_size)):
+            j = min(i + ray_batch_size, n_rays)
+            st = lanes[k % 2]
+            if k < 2:
+                st.wait_event(ready)
+            with torch.cuda.stream(st):
+                r = renderer.render_forward(o[i:j], d[i:j], out=tuple(u[:j - i] for u in unused[k % 2]), lane=1 + k % 2)
+                ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
+                                         f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=normals[i:j])
+            alive.append(r)                                  # allocations of a lane stay referenced until the join below
+        for st in lanes:
+            main.wait_stream(st)
+        del alive
+    return normals.cpu()                                         # the one device->host copy
+
+
 def quantify(x):
     """ExpRunner::TestImages' ``quantify`` (ExpRunner.cpp:360-362): (x.clip(0,1) * 255).to(uint8).to(float32) / 255, bit-exact
     on the device.  The reference runs it on CPU tensors, where dividing by the scalar 255 is a true division; ATen's CUDA

@@ -8,6 +8,10 @@ the logit ``EMPTY_LOGIT``, so their density ``exp(logit - 3)`` is exactly 0.
 
 The surface is a level set of the density logit on a lattice, extracted by marching tetrahedra (``Isosurface``): closed and
 consistently oriented by construction, outward towards lower density.  DESIGN.md §3i has the details and the parity anchors.
+
+Surface normals (DESIGN.md §3j) come from the density itself: ``QueryGradient`` returns g = d logit / d x at world points (one
+kernel: the field query's forward, the field MLP's backward on the tensor pipe, the hash-grid blend's derivative and the leaf
+warp's Jacobian), ``QueryNormal`` the outward normal -g / |g|.
 """
 import math
 from typing import NamedTuple, Optional
@@ -37,11 +41,13 @@ class Mesh(NamedTuple):
     verts: torch.Tensor
     faces: torch.Tensor
     colors: Optional[torch.Tensor] = None
+    normals: Optional[torch.Tensor] = None
 
     def to_data_frame(self, dataset):
-        """The mesh in the data's own world frame: x * radius_ + center_ (undoes ``load_dataset``'s normalisation)."""
+        """The mesh in the data's own world frame: x * radius_ + center_ (undoes ``load_dataset``'s normalisation).  The frames
+        differ by a uniform scale and a translation, so the normals carry over unchanged."""
         center = torch.as_tensor(dataset.center_, dtype=torch.float32, device=self.verts.device)
-        return Mesh(self.verts * float(dataset.radius_) + center, self.faces, self.colors)
+        return Mesh(self.verts * float(dataset.radius_) + center, self.faces, self.colors, self.normals)
 
 
 def _octree(renderer):
@@ -77,6 +83,25 @@ def QueryDensity(renderer, pts):
     """Density at world points [n,3]: the renderer's density activation exp(logit - 3) (Renderer.cpp:100-103); 0 where no valid
     leaf holds the point.  The density is per unit of warped length, the quantity the renderer integrates along a ray."""
     return torch.exp(QueryLogit(renderer, pts) - 3.)
+
+
+def QueryGradient(renderer, pts):
+    """(logit [n], grad [n,3]) at world points [n,3]: the logit of ``QueryLogit`` (same bits) and its gradient d logit / d x in
+    the normalised scene frame (DESIGN.md §3j); ``EMPTY_LOGIT`` and a zero gradient where no valid leaf holds the point."""
+    nodes, trans = _octree(renderer)
+    return ops.query_grad_points(nodes, trans, *_field_args(renderer), _points(pts, renderer), EMPTY_LOGIT)
+
+
+def unit_normals(grad):
+    """-g / |g| per row of [n,3] (the outward normal, towards lower density); 0 where g = 0."""
+    n = torch.linalg.norm(grad, dim=1, keepdim=True)
+    return torch.where(n > 0, -grad / n.clamp_min(1e-38), torch.zeros_like(grad))
+
+
+def QueryNormal(renderer, pts):
+    """Outward unit normals [n,3] of the density at world points [n,3]: -g / |g| of ``QueryGradient``; 0 where the gradient is
+    0 or no valid leaf holds the point."""
+    return unit_normals(QueryGradient(renderer, pts)[1])
 
 
 def QueryColor(renderer, pts, dirs):
@@ -192,36 +217,47 @@ def vertex_normals(verts, faces):
     return n
 
 
-def VertexColors(renderer, verts, faces):
-    """Colour of each vertex seen from outside along its normal: ``QueryColor`` with view direction -n / |n|.  The normals are
-    sums of float atomics, so a colour can differ by an ulp from run to run."""
+def VertexColors(renderer, verts, faces, normals=None):
+    """Colour of each vertex seen from outside along its normal: ``QueryColor`` with view direction -n / |n|.  By default n is
+    the area-weighted face normal (``vertex_normals``: sums of float atomics, so a colour can differ by an ulp from run to run);
+    ``normals`` [V,3] (unit or 0, e.g. ``QueryNormal``) replaces it wherever it is non-zero."""
     n = vertex_normals(verts, faces)
+    if normals is not None:
+        n = torch.where((normals != 0).any(1, keepdim=True), normals, n)
     d = -n / torch.linalg.norm(n, dim=1, keepdim=True).clamp_min(1e-30)
     return QueryColor(renderer, verts, d)
 
 
-def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, density=None, colors=True):
+def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, density=None, colors=True, normals=False):
     """The scene's surface as a ``Mesh`` on the device, in the normalised frame (``Mesh.to_data_frame`` maps it back).
     The level is the density that reaches opacity ``alpha`` over one VALIDATE march step (``level_from_alpha``), or
-    ``density`` (per warp unit) when given; the lattice is ``DensityGrid(renderer, bbox_min, bbox_max, reso)``."""
+    ``density`` (per warp unit) when given; the lattice is ``DensityGrid(renderer, bbox_min, bbox_max, reso)``.
+    ``normals``: the vertices get the field's normals (``QueryNormal``), and the colours are seen along them (the face normal
+    where the field normal is 0)."""
     level = math.log(float(density)) + 3. if density is not None else level_from_alpha(renderer, alpha)
     g = DensityGrid(renderer, bbox_min, bbox_max, reso)
     verts, faces = Isosurface(g.logit, level, g.origin, g.voxel)
     del g
-    rgb = VertexColors(renderer, verts, faces) if colors and verts.shape[0] else None
-    return Mesh(verts, faces, rgb)
+    nrm = QueryNormal(renderer, verts) if normals else None
+    rgb = VertexColors(renderer, verts, faces, nrm) if colors and verts.shape[0] else None
+    return Mesh(verts, faces, rgb, nrm)
 
 
 def write_ply(path, mesh):
-    """Binary little-endian PLY: float x, y, z (+ uchar red, green, blue when the mesh has colours) and uchar-counted int
-    triangle lists."""
+    """Binary little-endian PLY: float x, y, z (+ float nx, ny, nz when the mesh has normals, + uchar red, green, blue when it
+    has colours) and uchar-counted int triangle lists."""
     v = mesh.verts.detach().cpu().numpy().astype("<f4")
     f = mesh.faces.detach().cpu().numpy().astype("<i4")
     fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if mesh.normals is not None:
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
     if mesh.colors is not None:
         fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
     vr = np.empty(len(v), fields)
     vr["x"], vr["y"], vr["z"] = v[:, 0], v[:, 1], v[:, 2]
+    if mesh.normals is not None:
+        nm = mesh.normals.detach().cpu().numpy().astype("<f4")
+        vr["nx"], vr["ny"], vr["nz"] = nm[:, 0], nm[:, 1], nm[:, 2]
     if mesh.colors is not None:
         c = np.clip(np.rint(mesh.colors.detach().cpu().numpy() * 255.), 0, 255).astype(np.uint8)
         vr["red"], vr["green"], vr["blue"] = c[:, 0], c[:, 1], c[:, 2]
@@ -229,6 +265,8 @@ def write_ply(path, mesh):
     fr["n"], fr["v"] = 3, f
     head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}", "property float x", "property float y",
             "property float z"]
+    if mesh.normals is not None:
+        head += ["property float nx", "property float ny", "property float nz"]
     if mesh.colors is not None:
         head += ["property uchar red", "property uchar green", "property uchar blue"]
     head += [f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]

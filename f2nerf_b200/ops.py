@@ -206,6 +206,38 @@ def query_logit_grid(tree_nodes, trans, table_f16, prim_pool, bias_pool, n_volum
     return out
 
 
+def warp_jacobian_points(tree_nodes, trans, pts):
+    """-> J [n,3,3] f32, J[i, r, c] = d warp_r / d x_c at the located point (0 where no valid leaf holds it)."""
+    _chk(pts, F32, "warp_jacobian_points: pts")
+    n = pts.shape[0]
+    jac = dev_empty((n, 3, 3), F32, pts)
+    call("f2b_warp_jacobian_points", tree_nodes, tree_nodes.numel() // 64, trans, pts, n, jac, stream())
+    return jac
+
+
+def query_grad_points(tree_nodes, trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, pts, empty_logit):
+    """-> (logit [n] f32, grad [n,3] f32): the logit of query_logit_points and its gradient in the scene frame."""
+    _chk(pts, F32, "query_grad_points: pts")
+    n = pts.shape[0]
+    logit = dev_empty((n,), F32, pts)
+    grad = dev_empty((n, 3), F32, pts)
+    call("f2b_query_grad_points", tree_nodes, tree_nodes.numel() // 64, trans, table_f16, prim_pool, bias_pool, int(n_volumes),
+         int(local_size), params_f16, pts, n, float(empty_logit), logit, grad, stream())
+    return logit, grad
+
+
+def render_normals_slots(trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, slots, kept_counts, w_slots,
+                         out=None):
+    """Unit normals [R,3] of a VALIDATE batch from the march's slots (sampler.SlotSamples) and the fused forward's kept counts
+    and slot weights; written into ``out`` when given."""
+    R, S = slots.n_rays, slots.slot
+    normals = out if out is not None else dev_empty((R, 3), F32, kept_counts)
+    partials = dev_empty((R * (S // 128), 3), F32, kept_counts)
+    call("f2b_render_normals_slots", trans, table_f16, prim_pool, bias_pool, int(n_volumes), int(local_size), params_f16, slots.s_pts,
+         slots.s_t, slots.s_anchors, kept_counts, w_slots, slots.rays_o, slots.rays_d, R, S, partials, normals, stream())
+    return normals
+
+
 def iso_count(logit, level, empty_logit, ez0, ez1, edge_mask, vert_counts, tri_counts):
     nz, ny, nx = logit.shape
     call("f2b_iso_count", logit, nx, ny, nz, float(level), float(empty_logit), int(ez0), int(ez1), edge_mask, vert_counts,

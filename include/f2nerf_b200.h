@@ -193,6 +193,26 @@ int f2b_query_logit_grid(const void* tree_nodes, int n_nodes, const void* trans,
                          const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
                          const void* mlp_params_f16, const float* origin3, const float* voxel3, int nx, int ny, int z0,
                          int nz, float empty_logit, float* logit, void* stream);
+/* Surface normals (DESIGN.md §3j).  The density gradient g = d logit / d x in the normalised scene frame: J^T . the hash-grid
+ * and field-MLP gradient at the warped point, J = QueryFrameTransformJac of the point's leaf in the march's roundings; dL/dfeat
+ * rounded to fp16 where the training backward rounds it, the ReLU mask taken from the fp16 hidden tile.
+ * f2b_warp_jacobian_points: J [n,3,3] (row r = d warp_r / d x) at located points, 0 where no valid leaf holds the point. */
+int f2b_warp_jacobian_points(const void* tree_nodes, int n_nodes, const void* trans, const float* pts /* [n,3] */, int n_pts,
+                             float* jac /* [n,3,3] */, void* stream);
+/* logit [n] bit-identical to f2b_query_logit_points, grad [n,3] = g; empty_logit and g = 0 where no valid leaf holds the point. */
+int f2b_query_grad_points(const void* tree_nodes, int n_nodes, const void* trans, const void* table_f16,
+                          const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                          const void* mlp_params_f16, const float* pts /* [n,3] */, int n_pts, float empty_logit,
+                          float* logit /* [n] */, float* grad /* [n,3] */, void* stream);
+/* Normal map of a VALIDATE batch from the slot buffers f2b_render_fwd_fused leaves: for the kept prefix of each ray
+ * (kept_counts, w_slots), n_i = -g_i / |g_i| (0 where g_i = 0) at the world point fma(t, d, o) of slot_t and the rays,
+ * N = sum_i w_i n_i summed serially in slot order within each 128-slot tile (tile_partials [n_rays * slot_size / 128, 3]
+ * scratch), then the tiles in order; normals [n_rays,3] = N / |N|, 0 where N = 0.  slot_size: a multiple of 128. */
+int f2b_render_normals_slots(const void* trans, const void* table_f16, const int* prim_pool, const float* bias_pool,
+                             int n_volumes, int local_size, const void* mlp_params_f16, const float* slot_pts, const float* slot_t,
+                             const int* slot_anchors /* [.,2] */, const int* kept_counts, const float* w_slots,
+                             const float* rays_o, const float* rays_d, int n_rays, int slot_size, float* tile_partials,
+                             float* normals /* [n_rays,3] */, void* stream);
 /* Isosurface {logit = level} of an nx x ny x nz logit lattice (x fastest) by marching tetrahedra on the Kuhn split of each
  * cell, lattice points outside the lattice reading empty_logit (<= level), for the cells of extended z-layers [ez0, ez1)
  * (0 <= ez0 < ez1 <= nz + 1; extended layer e holds lattice layer e - 1, see geometry.cu).  Pass 1 writes, per owner

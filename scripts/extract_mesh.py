@@ -25,6 +25,7 @@ def main(argv=None):
     ap.add_argument("--alpha", type=float, default=0.5)
     ap.add_argument("--bbox", type=float, nargs=6, default=None)
     ap.add_argument("--out", required=True)
+    ap.add_argument("--normals", action="store_true", help="field normals on the vertices (written as nx ny nz; colours seen along them)")
     ap.add_argument("--repeat", type=int, default=1, help="time the grid query and the extraction this many times (median)")
     a = ap.parse_args(argv)
 
@@ -52,13 +53,14 @@ def main(argv=None):
     del meshes
     n_pts = g.logit.numel()
     del g
-    colors, t_col = timed(lambda: G.VertexColors(r, verts, faces))
-    mesh = G.Mesh(verts, faces, colors).to_data_frame(scene.dataset)
+    normals, t_nrm = timed(lambda: G.QueryNormal(r, verts)) if a.normals else (None, 0.)
+    colors, t_col = timed(lambda: G.VertexColors(r, verts, faces, normals))
+    mesh = G.Mesh(verts, faces, colors, normals).to_data_frame(scene.dataset)
     G.write_ply(a.out, mesh)
     med = lambda x: sorted(x)[len(x) // 2]
     props = torch.cuda.get_device_properties(0)
     print(json.dumps(dict(reso=a.reso, alpha=a.alpha, level=level, lattice_points=n_pts, grid_query_s=med(t_grid),
-                          grid_points_per_s=n_pts / med(t_grid), extract_s=med(t_iso), colors_s=t_col, verts=int(verts.shape[0]),
+                          grid_points_per_s=n_pts / med(t_grid), extract_s=med(t_iso), colors_s=t_col, normals_s=t_nrm, verts=int(verts.shape[0]),
                           faces=int(faces.shape[0]), gpu=props.name, out=a.out)))
 
 

@@ -8,16 +8,18 @@
 # And the float64-autograd gradient module (tests/test_gpu_grad_autograd.py): 48 TRAIN steps, each with a float64 twin on the device.
 # And the C++ operator module (tests/test_gpu_cpp_ops_reference.py): it runs both reference binaries over 16 operator cases.
 # And the geometry module (tests/test_gpu_geometry.py): the tensor-core point query, and a 300-iteration ngp_fox training.
+# And the normals module (tests/test_gpu_normals.py): the tensor-core gradient kernel, and a 300-iteration ngp_fox training.
 # And the reference-configs module (tests/test_gpu_ref_configs.py): both reference binaries, three arms on free, big20 and big22.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
      "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
      tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py tests/test_gpu_train_maintenance.py
-     tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py tests/test_gpu_cpp_ops_reference.py tests/test_gpu_geometry.py)
+     tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py tests/test_gpu_cpp_ops_reference.py tests/test_gpu_geometry.py tests/test_gpu_normals.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
       --ignore=tests/test_gpu_mlp_fwd_reference.py --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
       --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py --ignore=tests/test_gpu_grad_autograd.py
-      --ignore=tests/test_gpu_cpp_ops_reference.py --ignore=tests/test_gpu_geometry.py --ignore=tests/test_gpu_ref_configs.py)
+      --ignore=tests/test_gpu_cpp_ops_reference.py --ignore=tests/test_gpu_geometry.py --ignore=tests/test_gpu_normals.py
+      --ignore=tests/test_gpu_ref_configs.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py

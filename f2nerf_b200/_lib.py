@@ -67,8 +67,6 @@ SIGNATURES = {
     "f2b_field_bwd_scatter": [_P, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_float, _P, _P, _P, _P],
     "f2b_shade_field_bwd_scatter": [_P, _P, _P, _P, _P, c_float, c_float, _P, _P, c_int, _P, _P, c_int, _P, _P, c_int, c_int, c_float,
                                     _P, _P, _P, _P, _P, _P, _P, _P, _P],
-    "f2b_mlp_fwd_v0": [_P, _P, c_int, c_int, _P, _P, _P],
-    "f2b_mlp_bwd_v0": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_field_fwd": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P],
     "f2b_field_fwd_slots": [_P, _P, _P, c_int, c_int, _P, _P, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P],
     "f2b_get_mlp_impl": [],
@@ -76,10 +74,8 @@ SIGNATURES = {
     "f2b_cast_f16_to_f32": [_P, _P, c_i64, c_float, _P],
     "f2b_sh_encode": [_P, c_int, c_int, _P, _P],
     "f2b_scatter_idx": [_P, _P, c_int, _P, _P],
-    "f2b_shader_prep": [_P, _P, _P, _P, c_int, _P, _P],
     "f2b_shader_act": [_P, c_int, _P, _P],
     "f2b_shader_act_bwd": [_P, _P, c_int, c_float, _P, _P],
-    "f2b_shader_prep_bwd": [_P, _P, _P, c_int, c_float, _P, _P, _P],
     "f2b_shader_prep_bwd_f16": [_P, _P, _P, _P, c_int, c_float, c_float, _P, _P, _P],
     "f2b_octree_proc": [_P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P],
     "f2b_octree_mark_invisible": [_P, c_int, _P, _P, _P, c_int, _P],
@@ -89,14 +85,11 @@ SIGNATURES = {
     "f2b_image_metrics": [_P, _P, c_int, c_int, _P, _P, _P, _P, _P],
     "f2b_adam_step": [_P, _P, _P, _P, c_i64, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                       ctypes.c_double, c_i64, _P, _P],
-    "f2b_early_stop": [_P, c_int, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P],
     "f2b_early_stop_rays": [_P, c_int, _P, _P, c_int, _P, _P, _P, _P, _P],
     "f2b_count_scan": [_P, c_int, _P, _P, _P],
     "f2b_slot_bounds": [_P, c_int, c_int, c_int, _P, _P],
     "f2b_compact_slots": [_P, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
-    "f2b_compact_samples": [_P, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_composite_fwd": [_P, c_int, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P],
-    "f2b_composite_bwd": [_P, c_int, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, c_float, _P, c_int, _P, _P],
     "f2b_composite_act_bwd": [_P, c_int, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, c_float, _P, c_float, _P, c_int, _P, _P],
     "f2b_flex_sum": [_P, c_int, _P, c_int, _P, _P],
     "f2b_flex_accumulate_sum": [_P, _P, c_int, c_int, _P, _P],
@@ -186,7 +179,7 @@ def stream():
 
 # kernels launched per entry point (for bench.py's gpu_launches claim; memsets are not counted)
 KERNELS_PER_CALL = {"f2b_render_sizeof": 0, "f2b_render_phase1": 7, "f2b_render_phase2_fwd": 10, "f2b_render_bwd": 6, "f2b_render_grad_finalize": 2,
-                    "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_early_stop": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
+                    "f2b_sampler_count": 2, "f2b_sampler_march": 2, "f2b_hash_level_scales": 1, "f2b_device_info": 0,
                     "f2b_abi_version": 0, "f2b_get_mlp_impl": 0, "f2b_image_metrics": 2}
 LAUNCHES = 0      # running count of product kernels launched through this binding
 TRACE = None      # set to a list to record (name, start_event, end_event, int_args) per call (bench.py)

@@ -76,43 +76,6 @@ early_stop_kernel(const float* __restrict__ logit, int logit_stride, const float
   if (lane == 0) counts[ray] = cnt;
 }
 
-// ---- gather-compaction of the surviving samples ------------------------------------------------
-__global__ void __launch_bounds__(256)
-compact_kernel(const uint8_t* __restrict__ keep, const int* __restrict__ old_bounds,
-               const int* __restrict__ new_bounds, int n_rays, const float* __restrict__ pts,
-               const float* __restrict__ dirs, const float* __restrict__ dt, const float* __restrict__ t,
-               const int* __restrict__ anchors, const uint4* __restrict__ feat, float* __restrict__ pts_o,
-               float* __restrict__ dirs_o, float* __restrict__ dt_o, float* __restrict__ t_o,
-               int* __restrict__ anchors_o, uint4* __restrict__ feat_o) {
-  const int ray = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (ray >= n_rays) return;
-  const int beg = old_bounds[2 * ray], end = old_bounds[2 * ray + 1];
-  int out = new_bounds[2 * ray];
-  for (int base = beg; base < end; base += 32) {
-    const int i = base + lane;
-    const bool k = (i < end) && keep[i];
-    const unsigned m = __ballot_sync(kFull, k);
-    if (k) {
-      const size_t o = size_t(out) + __popc(m & ((1u << lane) - 1u));
-      const size_t s = size_t(i);
-#pragma unroll
-      for (int c = 0; c < 3; c++) {
-        pts_o[o * 3 + c] = pts[s * 3 + c];
-        dirs_o[o * 3 + c] = dirs[s * 3 + c];
-        anchors_o[o * 3 + c] = anchors[s * 3 + c];
-      }
-      dt_o[o] = dt[s];
-      t_o[o] = t[s];
-      if (feat) {                                  // the sample's 32 encoded halfs (64 B) from the early-stop pass
-#pragma unroll
-        for (int c = 0; c < 4; c++) feat_o[o * 4 + c] = feat[s * 4 + c];
-      }
-    }
-    out += __popc(m);
-  }
-}
-
 // Same compaction straight out of the one-pass march's scratch slots (ray r owns slots
 // [r*slot, r*slot + count[r]); 28 B/sample there): directions are the ray's, anchors[:,2] is 0 — the
 // all-sample SampleResultFlex the reference materialises between march and early stop is never built.
@@ -214,7 +177,8 @@ composite_fwd_kernel(const float* __restrict__ logit, int logit_stride, const fl
 // ---- backward composite -----------------------------------------------------------------------
 // sweep 1 (front to back): exclusive optical depth A_i (serial order, parked in d_logit), S, Zs.
 // sweep 2 (back to front): per-sample gradients with a reverse warp scan for sum_{k>i} dA_k.
-template <bool FUSE_ACT>
+// The colour gradient goes straight through the scaled sigmoid's backward (SHShader.cpp:27-28) into the
+// shader MLP's fp16 dL/dout row [g_r, g_g, g_b, 0 x 13] * loss_scale; no fp32 d_rgb is written.
 __global__ void __launch_bounds__(256)
 composite_bwd_kernel(const float* __restrict__ logit, int logit_stride, const float* __restrict__ rgb,
                      const float* __restrict__ dt, const float* __restrict__ t,
@@ -222,10 +186,7 @@ composite_bwd_kernel(const float* __restrict__ logit, int logit_stride, const fl
                      const float* __restrict__ d_colors, const float* __restrict__ d_disp,
                      const float* __restrict__ d_depth, const float* __restrict__ d_weights,
                      float gs_progress, float* __restrict__ d_logit, int dlogit_stride,
-                     float* __restrict__ d_rgb, const __half* __restrict__ raw, __half* __restrict__ d_raw,
-                     float act_loss_scale) {
-  // FUSE_ACT: the colour gradient goes straight through the scaled sigmoid's backward (SHShader.cpp:27-28) into the
-  // shader MLP's fp16 dL/dout row [g_r, g_g, g_b, 0 x 13] * loss_scale instead of being written as fp32 d_rgb.
+                     const __half* __restrict__ raw, __half* __restrict__ d_raw, float act_loss_scale) {
   const int ray = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (ray >= n_rays) return;
@@ -301,21 +262,15 @@ composite_bwd_kernel(const float* __restrict__ logit, int logit_stride, const fl
       // TruncExp backward: g * exp(clamp(x, -100, 5))   (CustomOps.cpp:16-18)
       d_logit[size_t(i) * dlogit_stride] = ddens * expf(fminf(fmaxf(x, -100.f), 5.f));
       const float gr = w * dcr * scale, gg = w * dcg * scale, gb = w * dcb * scale;
-      if (FUSE_ACT) {
-        const uint2 rw = __ldg(reinterpret_cast<const uint2*>(raw + size_t(i) * 16));
-        const float2 o01 = __half22float2(*reinterpret_cast<const __half2*>(&rw.x));
-        const float2 o2x = __half22float2(*reinterpret_cast<const __half2*>(&rw.y));
-        const __half2 h0 = __floats2half2_rn(shade_act_bwd(o01.x, gr, act_loss_scale), shade_act_bwd(o01.y, gg, act_loss_scale));
-        const __half2 h1 = __floats2half2_rn(shade_act_bwd(o2x.x, gb, act_loss_scale), 0.f);
-        uint4 v0 = make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1), 0u, 0u);
-        uint4* dst = reinterpret_cast<uint4*>(d_raw + size_t(i) * 16);
-        dst[0] = v0;
-        dst[1] = make_uint4(0u, 0u, 0u, 0u);
-      } else {
-        d_rgb[size_t(i) * 3 + 0] = gr;
-        d_rgb[size_t(i) * 3 + 1] = gg;
-        d_rgb[size_t(i) * 3 + 2] = gb;
-      }
+      const uint2 rw = __ldg(reinterpret_cast<const uint2*>(raw + size_t(i) * 16));
+      const float2 o01 = __half22float2(*reinterpret_cast<const __half2*>(&rw.x));
+      const float2 o2x = __half22float2(*reinterpret_cast<const __half2*>(&rw.y));
+      const __half2 h0 = __floats2half2_rn(shade_act_bwd(o01.x, gr, act_loss_scale), shade_act_bwd(o01.y, gg, act_loss_scale));
+      const __half2 h1 = __floats2half2_rn(shade_act_bwd(o2x.x, gb, act_loss_scale), 0.f);
+      uint4 v0 = make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1), 0u, 0u);
+      uint4* dst = reinterpret_cast<uint4*>(d_raw + size_t(i) * 16);
+      dst[0] = v0;
+      dst[1] = make_uint4(0u, 0u, 0u, 0u);
     }
   }
 }
@@ -403,19 +358,6 @@ using namespace f2b;
 
 static inline int warp_grid(int n_rays) { return div_up(int64_t(n_rays) * 32, 256); }
 
-extern "C" int f2b_early_stop(const float* logit, int logit_stride, const float* dt, const int* pts_idx_bounds,
-                              int n_rays, float* weights, float* alphas, uint8_t* keep, int* ray_counts,
-                              int* new_bounds, int* total_kept, void* stream) {
-  if (n_rays <= 0) return F2B_OK;
-  F2B_REQUIRE(logit && dt && pts_idx_bounds && weights && alphas && keep && ray_counts && new_bounds && total_kept,
-              "f2b_early_stop: null pointer");
-  cudaStream_t st = as_stream(stream);
-  early_stop_kernel<<<warp_grid(n_rays), 256, 0, st>>>(logit, logit_stride, dt, pts_idx_bounds, n_rays, weights,
-                                                      alphas, keep, ray_counts);
-  scan_counts_kernel<<<1, 1024, 0, st>>>(ray_counts, n_rays, new_bounds, total_kept);
-  return check_launch("f2b_early_stop");
-}
-
 extern "C" int f2b_early_stop_rays(const float* logit, int logit_stride, const float* dt, const int* pts_idx_bounds,
                                    int n_rays, float* weights, float* alphas, uint8_t* keep, int* ray_counts, void* stream) {
   if (n_rays <= 0) return F2B_OK;
@@ -452,18 +394,6 @@ extern "C" int f2b_compact_slots(const uint8_t* keep, const int* slot_bounds, co
   return check_launch("f2b_compact_slots");
 }
 
-extern "C" int f2b_compact_samples(const uint8_t* keep, const int* old_bounds, const int* new_bounds, int n_rays,
-                                   const float* pts, const float* dirs, const float* dt, const float* t,
-                                   const int* anchors, const void* feat_f16, float* pts_o, float* dirs_o,
-                                   float* dt_o, float* t_o, int* anchors_o, void* feat_o_f16, void* stream) {
-  if (n_rays <= 0) return F2B_OK;
-  F2B_REQUIRE(!feat_f16 || feat_o_f16, "f2b_compact_samples: feat_f16 without feat_o_f16");
-  compact_kernel<<<warp_grid(n_rays), 256, 0, as_stream(stream)>>>(keep, old_bounds, new_bounds, n_rays, pts, dirs, dt, t,
-                                                                  anchors, (const uint4*)feat_f16, pts_o, dirs_o, dt_o,
-                                                                  t_o, anchors_o, (uint4*)feat_o_f16);
-  return check_launch("f2b_compact_samples");
-}
-
 extern "C" int f2b_composite_fwd(const float* logit, int logit_stride, const float* rgb, const float* dt,
                                  const float* t, const int* pts_idx_bounds, const float* bg_color, int n_rays,
                                  float* colors, float* disparity, float* depth, float* weights, void* stream) {
@@ -475,20 +405,6 @@ extern "C" int f2b_composite_fwd(const float* logit, int logit_stride, const flo
   return check_launch("f2b_composite_fwd");
 }
 
-extern "C" int f2b_composite_bwd(const float* logit, int logit_stride, const float* rgb, const float* dt,
-                                 const float* t, const int* pts_idx_bounds, const float* bg_color, int n_rays,
-                                 const float* d_colors, const float* d_disparity, const float* d_depth,
-                                 const float* d_weights, float grad_scaling_progress, float* d_logit,
-                                 int dlogit_stride, float* d_rgb, void* stream) {
-  if (n_rays <= 0) return F2B_OK;
-  F2B_REQUIRE(logit && rgb && dt && t && pts_idx_bounds && bg_color && d_colors && d_logit && d_rgb,
-              "f2b_composite_bwd: null pointer");
-  composite_bwd_kernel<false><<<warp_grid(n_rays), 256, 0, as_stream(stream)>>>(
-      logit, logit_stride, rgb, dt, t, pts_idx_bounds, bg_color, n_rays, d_colors, d_disparity, d_depth, d_weights,
-      grad_scaling_progress, d_logit, dlogit_stride, d_rgb, nullptr, nullptr, 0.f);
-  return check_launch("f2b_composite_bwd");
-}
-
 extern "C" int f2b_composite_act_bwd(const float* logit, int logit_stride, const float* rgb, const float* dt,
                                      const float* t, const int* pts_idx_bounds, const float* bg_color, int n_rays,
                                      const float* d_colors, const float* d_disparity, const float* d_depth,
@@ -497,9 +413,9 @@ extern "C" int f2b_composite_act_bwd(const float* logit, int logit_stride, const
   if (n_rays <= 0) return F2B_OK;
   F2B_REQUIRE(logit && rgb && dt && t && pts_idx_bounds && bg_color && d_colors && d_logit && raw_f16 && d_raw_f16,
               "f2b_composite_act_bwd: null pointer");
-  composite_bwd_kernel<true><<<warp_grid(n_rays), 256, 0, as_stream(stream)>>>(
+  composite_bwd_kernel<<<warp_grid(n_rays), 256, 0, as_stream(stream)>>>(
       logit, logit_stride, rgb, dt, t, pts_idx_bounds, bg_color, n_rays, d_colors, d_disparity, d_depth, d_weights,
-      grad_scaling_progress, d_logit, dlogit_stride, nullptr, (const __half*)raw_f16, (__half*)d_raw_f16, loss_scale);
+      grad_scaling_progress, d_logit, dlogit_stride, (const __half*)raw_f16, (__half*)d_raw_f16, loss_scale);
   return check_launch("f2b_composite_act_bwd");
 }
 

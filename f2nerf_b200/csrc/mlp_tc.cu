@@ -277,7 +277,7 @@ extern "C" int f2b_mlp_fwd_f32(const void* in_f16, const void* params_f16, int n
   return check_launch("f2b_mlp_fwd_f32(wgmma)");
 }
 
-// The public MLP entry points always run the wgmma kernels (1); the CUDA-core kernels are reached only as f2b_mlp_*_v0.
+// The MLP entry points always run the wgmma kernels (1).
 extern "C" int f2b_get_mlp_impl(void) { return 1; }
 
 // Field MLP (32 -> 64 -> 16) on encoded features + the shading-feature assembly in its epilogue:

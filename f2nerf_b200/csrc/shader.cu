@@ -1,5 +1,6 @@
-// shader.cu — SH view-direction encode, shader-MLP input assembly (constant-1 channel, appearance
-// embedding) and the scaled-sigmoid colour activation, fused around the MLP.
+// shader.cu — SH view-direction encode, the scaled-sigmoid colour activation and the backward of the
+// shader-MLP input assembly (constant-1 channel, appearance embedding).  The forward assembly runs in the
+// field MLP's epilogue (shade_row in shader.cuh, called from mlp_tc.cu and fused_fwd.cu).
 //
 // Replaces SHKenerl (src/Shader/SHShader.cu:10-106, degree <= 4 used by every shipped config),
 // the torch::cat / ones_like / ScatterIdx / ScatterAdd chain of Renderer::Render
@@ -30,25 +31,6 @@ __global__ void scatter_idx_kernel(int n_rays, const int* __restrict__ bounds, c
   for (int i = bounds[2 * ray] + lane; i < bounds[2 * ray + 1]; i += 32) out[i] = v;
 }
 
-// mlp_in[p] = fp16([1, feat[1..15]] + app_emb[cam(p)] | SH4(dir_p))
-__global__ void __launch_bounds__(128)
-shader_prep_kernel(const float* __restrict__ scene_feat, const float* __restrict__ dirs,
-                   const float* __restrict__ app_emb, const int* __restrict__ pt_emb_idx, int n,
-                   __half* __restrict__ mlp_in) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float feat[16];
-  const float4* f4 = reinterpret_cast<const float4*>(scene_feat + size_t(i) * 16);
-#pragma unroll
-  for (int q = 0; q < 4; q++) { const float4 a = __ldg(f4 + q); feat[4 * q] = a.x; feat[4 * q + 1] = a.y; feat[4 * q + 2] = a.z; feat[4 * q + 3] = a.w; }
-  uint4 row[4];
-  shade_row(feat, app_emb ? app_emb + size_t(pt_emb_idx[i]) * 16 : nullptr, __ldg(dirs + size_t(i) * 3),
-            __ldg(dirs + size_t(i) * 3 + 1), __ldg(dirs + size_t(i) * 3 + 2), row);
-  uint4* dst = reinterpret_cast<uint4*>(mlp_in + size_t(i) * 32);
-#pragma unroll
-  for (int q = 0; q < 4; q++) dst[q] = row[q];
-}
-
 // rgb = (1 + 2e-3) / (1 + exp(-o)) - 1e-3 on the fp16 MLP output (SHShader.cpp:27-28)
 __global__ void shader_act_kernel(const __half* __restrict__ raw, int n, float* __restrict__ rgb) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -76,22 +58,21 @@ __global__ void shader_act_bwd_kernel(const __half* __restrict__ raw, const floa
 }
 
 // Backward of the input assembly, one warp per ray: d scene_feat[:,1:16] = d mlp_in[:,1:16] / loss_scale
-// (channel 0 of scene_feat is the density logit, filled by the composite backward) and the appearance-
+// (channel 0 of scene_feat is the density logit, taken from the composite backward's d logit) and the appearance-
 // embedding gradient d app_emb[cam(ray)] += sum over the ray's samples of d mlp_in[:,0:16]
 // (ScatterAddFuncBackwardBlock, Scatter.cu:23-40 — there a dense [n_emb x n_blocks] compare-and-sum).  The
 // camera index is constant along a ray, so the sum is a register accumulation + one warp reduction + 16
 // atomicAdds per ray instead of one atomic per sample and channel.
 // Lane mapping: 4 lanes per sample (4 channels each), 8 samples per warp pass — every load is a full 32 B
 // sector of the row and every store instruction covers whole rows.
-// F16OUT: instead of the fp32 gradient the kernel emits what TCNNWPFunction::backward (TCNNWP.cpp:213-216)
-// makes of it one call later, half((d/loss_scale_shader) * loss_scale_field), with channel 0 taken from the
-// composite backward's d logit — the fp32 [P,16] round trip through HBM and its zero-fill disappear.
-template <bool F16OUT>
+// The output is not d scene_feat in fp32 but what TCNNWPFunction::backward (TCNNWP.cpp:213-216) makes of it
+// one call later, half((d/loss_scale_shader) * loss_scale_field): the field MLP's dL/dout row, with no fp32
+// [P,16] round trip through HBM and no zero-fill.
 __global__ void __launch_bounds__(256)
 shader_prep_bwd_kernel(const __half* __restrict__ d_mlp_in, const float* __restrict__ d_logit,
                        const int* __restrict__ bounds, const int* __restrict__ emb_idx, int n_rays,
-                       float inv_loss_scale, float out_scale, float* __restrict__ d_scene_feat,
-                       __half* __restrict__ d_out16, float* __restrict__ d_app_emb) {
+                       float inv_loss_scale, float out_scale, __half* __restrict__ d_out16,
+                       float* __restrict__ d_app_emb) {
   const int ray = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (ray >= n_rays) return;
@@ -105,19 +86,13 @@ shader_prep_bwd_kernel(const __half* __restrict__ d_mlp_in, const float* __restr
     float g[4] = {f0.x * inv_loss_scale, f0.y * inv_loss_scale, f1.x * inv_loss_scale, f1.y * inv_loss_scale};
 #pragma unroll
     for (int k = 0; k < 4; k++) acc[k] += g[k];
-    if (F16OUT) {
-      if (sub == 0) g[0] = __ldg(d_logit + i);
-      const __half2 h0 = __floats2half2_rn(g[0] * out_scale, g[1] * out_scale);
-      const __half2 h1 = __floats2half2_rn(g[2] * out_scale, g[3] * out_scale);
-      uint2 o;
-      o.x = *reinterpret_cast<const uint32_t*>(&h0);
-      o.y = *reinterpret_cast<const uint32_t*>(&h1);
-      reinterpret_cast<uint2*>(d_out16 + size_t(i) * 16)[sub] = o;
-    } else {
-      float* dst = d_scene_feat + size_t(i) * 16 + 4 * sub;
-      if (sub == 0) { dst[1] = g[1]; dst[2] = g[2]; dst[3] = g[3]; }
-      else *reinterpret_cast<float4*>(dst) = make_float4(g[0], g[1], g[2], g[3]);
-    }
+    if (sub == 0) g[0] = __ldg(d_logit + i);
+    const __half2 h0 = __floats2half2_rn(g[0] * out_scale, g[1] * out_scale);
+    const __half2 h1 = __floats2half2_rn(g[2] * out_scale, g[3] * out_scale);
+    uint2 o;
+    o.x = *reinterpret_cast<const uint32_t*>(&h0);
+    o.y = *reinterpret_cast<const uint32_t*>(&h1);
+    reinterpret_cast<uint2*>(d_out16 + size_t(i) * 16)[sub] = o;
   }
   if (d_app_emb) {
 #pragma unroll
@@ -153,16 +128,6 @@ extern "C" int f2b_scatter_idx(const int* pts_idx_bounds, const int* emb_idx, in
   return check_launch("f2b_scatter_idx");
 }
 
-extern "C" int f2b_shader_prep(const float* scene_feat, const float* dirs, const float* app_emb,
-                               const int* pt_emb_idx, int n_pts, void* mlp_in_f16, void* stream) {
-  if (n_pts <= 0) return F2B_OK;
-  F2B_REQUIRE(scene_feat && dirs && mlp_in_f16, "f2b_shader_prep: null pointer");
-  F2B_REQUIRE(!app_emb || pt_emb_idx, "f2b_shader_prep: app_emb without pt_emb_idx");
-  shader_prep_kernel<<<div_up(n_pts, 128), 128, 0, as_stream(stream)>>>(scene_feat, dirs, app_emb, pt_emb_idx, n_pts,
-                                                                       (__half*)mlp_in_f16);
-  return check_launch("f2b_shader_prep");
-}
-
 extern "C" int f2b_shader_act(const void* raw_out_f16, int n_pts, float* rgb, void* stream) {
   if (n_pts <= 0) return F2B_OK;
   shader_act_kernel<<<div_up(n_pts, 256), 256, 0, as_stream(stream)>>>((const __half*)raw_out_f16, n_pts, rgb);
@@ -177,24 +142,14 @@ extern "C" int f2b_shader_act_bwd(const void* raw_out_f16, const float* d_rgb, i
   return check_launch("f2b_shader_act_bwd");
 }
 
-extern "C" int f2b_shader_prep_bwd(const void* d_mlp_in_f16, const int* pts_idx_bounds, const int* emb_idx, int n_rays,
-                                   float inv_loss_scale, float* d_scene_feat, float* d_app_emb, void* stream) {
-  if (n_rays <= 0) return F2B_OK;
-  F2B_REQUIRE(d_mlp_in_f16 && pts_idx_bounds && d_scene_feat, "f2b_shader_prep_bwd: null pointer");
-  F2B_REQUIRE(!d_app_emb || emb_idx, "f2b_shader_prep_bwd: d_app_emb without emb_idx");
-  shader_prep_bwd_kernel<false><<<div_up(int64_t(n_rays) * 32, 256), 256, 0, as_stream(stream)>>>(
-      (const __half*)d_mlp_in_f16, nullptr, pts_idx_bounds, emb_idx, n_rays, inv_loss_scale, 1.f, d_scene_feat, nullptr, d_app_emb);
-  return check_launch("f2b_shader_prep_bwd");
-}
-
 extern "C" int f2b_shader_prep_bwd_f16(const void* d_mlp_in_f16, const float* d_logit, const int* pts_idx_bounds,
                                        const int* emb_idx, int n_rays, float inv_loss_scale, float field_loss_scale,
                                        void* d_field_out_f16, float* d_app_emb, void* stream) {
   if (n_rays <= 0) return F2B_OK;
   F2B_REQUIRE(d_mlp_in_f16 && d_logit && pts_idx_bounds && d_field_out_f16, "f2b_shader_prep_bwd_f16: null pointer");
   F2B_REQUIRE(!d_app_emb || emb_idx, "f2b_shader_prep_bwd_f16: d_app_emb without emb_idx");
-  shader_prep_bwd_kernel<true><<<div_up(int64_t(n_rays) * 32, 256), 256, 0, as_stream(stream)>>>(
-      (const __half*)d_mlp_in_f16, d_logit, pts_idx_bounds, emb_idx, n_rays, inv_loss_scale, field_loss_scale, nullptr,
+  shader_prep_bwd_kernel<<<div_up(int64_t(n_rays) * 32, 256), 256, 0, as_stream(stream)>>>(
+      (const __half*)d_mlp_in_f16, d_logit, pts_idx_bounds, emb_idx, n_rays, inv_loss_scale, field_loss_scale,
       (__half*)d_field_out_f16, d_app_emb);
   return check_launch("f2b_shader_prep_bwd_f16");
 }

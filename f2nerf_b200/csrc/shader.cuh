@@ -1,5 +1,6 @@
-// shader.cuh — device functions shared by shader.cu (stand-alone operators) and mlp_tc.cu (the same work fused into
-// the tensor-core MLP epilogues).  Explicit roundings: both users produce bit-identical rows.
+// shader.cuh — device functions shared by the stand-alone operators (shader.cu, composite.cu) and the kernels that fuse
+// the same work (the tensor-core MLP epilogues of mlp_tc.cu, fused_fwd.cu).  Explicit roundings: every user produces
+// bit-identical values.
 #pragma once
 #include "common.cuh"
 #include <cuda_fp16.h>

@@ -10,7 +10,7 @@ import torch
 from . import _lib
 from ._lib import call, stream
 
-F16, F32, I32, U8 = torch.float16, torch.float32, torch.int32, torch.uint8
+F16, F32, I32 = torch.float16, torch.float32, torch.int32
 
 
 def _chk(t, dtype, name):
@@ -128,13 +128,11 @@ def field_fwd(table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16
     return out, feat, hidden
 
 
-def mlp_fwd(x_f16, params_f16, n_hidden_matmuls, save_hidden=False, impl=None):
-    """impl="v0": the CUDA-core reference kernels; otherwise the tensor-core kernels."""
+def mlp_fwd(x_f16, params_f16, n_hidden_matmuls, save_hidden=False):
     n = x_f16.shape[0]
     out = dev_empty((n, 16), F16, x_f16)
     hidden = dev_empty((n_hidden_matmuls + 1, n, 64), F16, x_f16) if save_hidden else None
-    name = "f2b_mlp_fwd_v0" if impl == "v0" else "f2b_mlp_fwd"
-    call(name, x_f16, params_f16, int(n_hidden_matmuls), n, out, hidden, stream())
+    call("f2b_mlp_fwd", x_f16, params_f16, int(n_hidden_matmuls), n, out, hidden, stream())
     return out, hidden
 
 
@@ -148,13 +146,11 @@ def mlp_fwd_f32(x_f16, params_f16, n_hidden_matmuls, save_hidden=False, want_f16
     return out32, out16, hidden
 
 
-def mlp_bwd(dout_f16, x_f16, hidden, params_f16, n_hidden_matmuls, need_din=True, impl=None):
-    """impl="v0": the CUDA-core reference kernels; otherwise the tensor-core kernels."""
+def mlp_bwd(dout_f16, x_f16, hidden, params_f16, n_hidden_matmuls, need_din=True):
     n = x_f16.shape[0]
     din = dev_empty((n, 32), F16, x_f16) if need_din else None
     dparams = torch.zeros(params_f16.numel(), dtype=F32, device=x_f16.device)
-    name = "f2b_mlp_bwd_v0" if impl == "v0" else "f2b_mlp_bwd"
-    call(name, dout_f16, x_f16, hidden, params_f16, int(n_hidden_matmuls), n, din, dparams, stream())
+    call("f2b_mlp_bwd", dout_f16, x_f16, hidden, params_f16, int(n_hidden_matmuls), n, din, dparams, stream())
     return din, dparams
 
 
@@ -266,13 +262,6 @@ def scatter_idx(n_all_pts, idx_start_end, emb_idx):
     return out
 
 
-def shader_prep(scene_feat, dirs, app_emb=None, pt_emb_idx=None):
-    n = scene_feat.shape[0]
-    out = dev_empty((n, 32), F16, scene_feat)
-    call("f2b_shader_prep", scene_feat, dirs, app_emb, pt_emb_idx, n, out, stream())
-    return out
-
-
 def shader_act(raw_f16):
     n = raw_f16.shape[0]
     rgb = dev_empty((n, 3), F32, raw_f16)
@@ -287,11 +276,6 @@ def shader_act_bwd(raw_f16, d_rgb, loss_scale):
     return out
 
 
-def shader_prep_bwd(d_mlp_in_f16, bounds, emb_idx, inv_loss_scale, d_scene_feat, d_app_emb):
-    call("f2b_shader_prep_bwd", d_mlp_in_f16, bounds, emb_idx, bounds.shape[0], float(inv_loss_scale), d_scene_feat,
-         d_app_emb, stream())
-
-
 def shader_prep_bwd_f16(d_mlp_in_f16, d_logit, bounds, emb_idx, inv_loss_scale, field_loss_scale, d_field_out_f16, d_app_emb):
     """Fused tail of the shader backward: writes the field MLP's dL/dout (fp16, loss-scaled) for the first
     len(d_logit) rows of ``d_field_out_f16`` and accumulates d_app_emb."""
@@ -300,18 +284,6 @@ def shader_prep_bwd_f16(d_mlp_in_f16, d_logit, bounds, emb_idx, inv_loss_scale, 
 
 
 # ------------------------------------------------------------------ composite -------------------
-def early_stop(logit, logit_stride, dt, bounds):
-    R, P = bounds.shape[0], dt.shape[0]
-    weights, alphas = dev_empty((P,), F32, dt), dev_empty((P,), F32, dt)
-    keep = dev_empty((P,), U8, dt)
-    counts = dev_empty((max(R, 1),), I32, dt)
-    new_bounds = dev_empty((R, 2), I32, dt)
-    total = dev_empty((1,), I32, dt)
-    call("f2b_early_stop", logit, int(logit_stride), dt, bounds, R, weights, alphas, keep, counts, new_bounds, total,
-         stream())
-    return weights, alphas, keep, new_bounds, total
-
-
 def field_fwd_slots(table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, slot_pts, slot_anchors, counts, n_rays,
                     slot, out_logit, feat_slots):
     """Early-stop field pass over the march's slot layout (logit only); all tensor arguments may be ray-chunk views."""
@@ -336,29 +308,12 @@ def compact_slots(keep, slot_bounds, new_bounds, rays_d, s_pts, s_dt, s_t, s_anc
          feat_slots, *outs, feat_out, stream())
 
 
-def compact_samples(keep, old_bounds, new_bounds, n_kept, pts, dirs, dt, t, anchors, feat=None, feat_out=None):
-    outs = (dev_empty((n_kept, 3), F32, pts), dev_empty((n_kept, 3), F32, pts), dev_empty((n_kept,), F32, pts),
-            dev_empty((n_kept,), F32, pts), dev_empty((n_kept, 3), I32, pts))
-    call("f2b_compact_samples", keep, old_bounds, new_bounds, old_bounds.shape[0], pts, dirs, dt, t, anchors, feat, *outs,
-         feat_out, stream())
-    return outs
-
-
 def composite_fwd(logit, logit_stride, rgb, dt, t, bounds, bg):
     R, P = bounds.shape[0], dt.shape[0]
     colors, disp, depth = dev_empty((R, 3), F32, dt), dev_empty((R,), F32, dt), dev_empty((R,), F32, dt)
     weights = dev_empty((P,), F32, dt)
     call("f2b_composite_fwd", logit, int(logit_stride), rgb, dt, t, bounds, bg, R, colors, disp, depth, weights, stream())
     return colors, disp, depth, weights
-
-
-def composite_bwd(logit, logit_stride, rgb, dt, t, bounds, bg, d_colors, d_disp, d_depth, d_weights, gs_progress,
-                  d_logit, dlogit_stride):
-    R, P = bounds.shape[0], dt.shape[0]
-    d_rgb = dev_empty((P, 3), F32, dt)
-    call("f2b_composite_bwd", logit, int(logit_stride), rgb, dt, t, bounds, bg, R, d_colors, d_disp, d_depth, d_weights,
-         float(gs_progress), d_logit, int(dlogit_stride), d_rgb, stream())
-    return d_rgb
 
 
 # ------------------------------------------------------------------ reference free functions ----

@@ -271,12 +271,6 @@ int f2b_shade_field_bwd_scatter(const void* d_raw_f16, const void* mlp_in_f16, c
 
 /* Which kernels the MLP entry points above run: always 1 = the wgmma tensor-core kernels (recorded by benchmarks). */
 int f2b_get_mlp_impl(void);
-/* The CUDA-core twins of f2b_mlp_fwd / f2b_mlp_bwd (validation references for the tensor-core kernels). */
-int f2b_mlp_fwd_v0(const void* in_f16, const void* params_f16, int n_hidden_matmuls, int n_pts,
-                   void* out_f16, void* hidden_save_f16, void* stream);
-int f2b_mlp_bwd_v0(const void* dout_f16, const void* in_f16, const void* hidden_save_f16,
-                   const void* params_f16, int n_hidden_matmuls, int n_pts,
-                   void* din_f16, float* dparams_f32, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Shader — replaces SHShader::Query (src/Shader/SHShader.cpp:23-29, SHShader.cu:10-118).
@@ -284,27 +278,17 @@ int f2b_mlp_bwd_v0(const void* dout_f16, const void* in_f16, const void* hidden_
 int f2b_sh_encode(const float* dirs, int n_pts, int degree /* 1..4 */, float* out, void* stream);
 /* CustomOps::ScatterIdx (Scatter.cu:110-131): per-ray camera index broadcast to the ray's samples. */
 int f2b_scatter_idx(const int* pts_idx_bounds, const int* emb_idx, int n_rays, int* out, void* stream);
-/* Shader-MLP input assembly (Renderer.cpp:179-187 + SHShader.cpp:24-25 + tcnn identity cast):
- * mlp_in[p] = fp16([1, scene_feat[p,1:16]] + app_emb[pt_emb_idx[p]] | SH4(dirs[p])); app_emb nullable. */
-int f2b_shader_prep(const float* scene_feat /* [P,16] */, const float* dirs /* [P,3] */,
-                    const float* app_emb /* [n_img,16] or NULL */, const int* pt_emb_idx /* [P] or NULL */,
-                    int n_pts, void* mlp_in_f16 /* [P,32] */, void* stream);
 /* rgb = (1+2e-3)*sigmoid(raw[:, :3]) - 1e-3 on the fp16 MLP output (SHShader.cpp:27-28). */
 int f2b_shader_act(const void* raw_out_f16 /* [P,16] */, int n_pts, float* rgb /* [P,3] */, void* stream);
 /* Backward of the activation: d_raw[P,16] fp16 = loss_scale * d_rgb * sigmoid' (channels 3..15 zero). */
 int f2b_shader_act_bwd(const void* raw_out_f16, const float* d_rgb, int n_pts, float loss_scale,
                        void* d_raw_f16, void* stream);
-/* Backward of the input assembly (one warp per ray): d_scene_feat[p,1:16] = d_mlp_in[p,1:16]*inv_loss_scale
- * (column 0 is left to the composite backward) and, when d_app_emb != NULL,
- * d_app_emb[emb_idx[ray]] += sum over the ray's samples of d_mlp_in[p,0:16]*inv_loss_scale
+/* Backward of the shader-MLP input assembly (one warp per ray), fused with what follows it in the reference's graph: the
+ * slice/cat backward that puts the composite's d logit into column 0 (Renderer.cpp:179-183) and TCNNWPFunction::backward's
+ * input scaling (grad * loss_scale).to(fp16) (TCNNWP.cpp:213-216).  Emits the field MLP's dL/dout directly:
+ * d_field_out[p,0] = half(d_logit[p]*field_loss_scale), d_field_out[p,k] = half(d_mlp_in[p,k]*inv_loss_scale*field_loss_scale);
+ * and, when d_app_emb != NULL, d_app_emb[emb_idx[ray]] += sum over the ray's samples of d_mlp_in[p,0:16]*inv_loss_scale
  * (ScatterAddFuncBackwardBlock, Scatter.cu:23-40). */
-int f2b_shader_prep_bwd(const void* d_mlp_in_f16 /* [P,32] */, const int* pts_idx_bounds /* [R,2] */,
-                        const int* emb_idx /* [R] or NULL */, int n_rays, float inv_loss_scale,
-                        float* d_scene_feat /* [P,16] */, float* d_app_emb /* [n_emb,16] or NULL */, void* stream);
-/* Same, fused with what follows it in the reference's graph: the slice/cat backward that puts the composite's
- * d logit into column 0 (Renderer.cpp:179-183) and TCNNWPFunction::backward's input scaling
- * (grad * loss_scale).to(fp16) (TCNNWP.cpp:213-216).  Emits the field MLP's dL/dout directly:
- * d_field_out[p,0] = half(d_logit[p]*field_loss_scale), d_field_out[p,k] = half(d_mlp_in[p,k]*inv_loss_scale*field_loss_scale). */
 int f2b_shader_prep_bwd_f16(const void* d_mlp_in_f16 /* [P,32] */, const float* d_logit /* [P] */,
                             const int* pts_idx_bounds, const int* emb_idx, int n_rays, float inv_loss_scale,
                             float field_loss_scale, void* d_field_out_f16 /* [P,16] */, float* d_app_emb, void* stream);
@@ -379,13 +363,9 @@ int f2b_adam_step(float* param, const float* grad, float* exp_avg, float* exp_av
  * FilterIdxBounds/CountValidPts (Renderer.cu:8-50) and the gather-compaction (Renderer.cpp:126-132).
  * All per-ray sums run in the reference's serial left-to-right order (bit-compatible rounding).
  * ------------------------------------------------------------------------------------------ */
-/* No-grad early-stop pass: density logit (scene_feat[:,0], element stride logit_stride) + dt ->
- * weights, alphas (for UpdateOctNodes), keep mask (trans > 1e-4) and the compacted bounds. */
-int f2b_early_stop(const float* logit, int logit_stride, const float* dt, const int* pts_idx_bounds,
-                   int n_rays, float* weights, float* alphas, uint8_t* keep,
-                   int* ray_counts /* [n_rays] caller-owned scratch */,
-                   int* new_bounds /* [n_rays,2] */, int* total_kept /* [1] */, void* stream);
-/* The two halves of f2b_early_stop separately (ray-chunked pipelines scan once over all chunks' counts). */
+/* No-grad early-stop pass: density logit (scene_feat[:,0], element stride logit_stride) + dt -> weights, alphas (for
+ * UpdateOctNodes), keep mask (trans > 1e-4) and each ray's survivor count; f2b_count_scan of the counts gives the compacted
+ * bounds (ray-chunked pipelines scan once over all chunks' counts). */
 int f2b_early_stop_rays(const float* logit, int logit_stride, const float* dt, const int* pts_idx_bounds,
                         int n_rays, float* weights, float* alphas, uint8_t* keep, int* ray_counts, void* stream);
 /* counts[n] -> bounds[n,2] = {exclusive, inclusive} prefix sums, total[0] = sum (torch::cumsum at
@@ -393,36 +373,25 @@ int f2b_early_stop_rays(const float* logit, int logit_stride, const float* dt, c
 int f2b_count_scan(const int* counts, int n, int* bounds, int* total, void* stream);
 /* slot_bounds[r] = {(first_ray+r)*slot_size, (first_ray+r)*slot_size + ray_counts[r]}: pts_idx_bounds of the scratch layout. */
 int f2b_slot_bounds(const int* ray_counts, int n_rays, int slot_size, int first_ray, int* slot_bounds, void* stream);
-/* f2b_compact_samples reading the march's scratch slots directly (28 B/sample there: pts, dt, t, anchors[0:2]); the
- * per-sample direction is the ray's (rays_d [n_rays,3], normalised), anchors_o[:,2] = 0. */
+/* Gather-compact the surviving samples straight out of the march's scratch slots (28 B/sample there: pts, dt, t,
+ * anchors[0:2]) to rows new_bounds[r,0].. of pts_o / dirs_o [P',3], dt_o / t_o [P'], anchors_o [P',3]; the per-sample
+ * direction is the ray's (rays_d [n_rays,3], normalised), anchors_o[:,2] = 0.  Optionally also their encoded features
+ * (feat_slots_f16 [.,32] from the early-stop pass -> feat_o_f16 [P',32]) so the gradient pass does not gather the table again. */
 int f2b_compact_slots(const uint8_t* keep, const int* slot_bounds, const int* new_bounds, int n_rays,
                       const float* rays_d, const float* s_pts, const float* s_dt, const float* s_t,
                       const int* s_anchors, const void* feat_slots_f16 /* nullable */, float* pts_o, float* dirs_o,
                       float* dt_o, float* t_o, int* anchors_o, void* feat_o_f16 /* nullable */, void* stream);
-/* Gather-compact the surviving samples (44 B/pt) and, optionally, their encoded features (feat_f16 [P,32]
- * from the early-stop pass -> feat_o_f16 [P',32]) so the gradient pass does not gather the table again. */
-int f2b_compact_samples(const uint8_t* keep, const int* old_bounds, const int* new_bounds, int n_rays,
-                        const float* pts, const float* dirs, const float* dt, const float* t,
-                        const int* anchors, const void* feat_f16 /* nullable */,
-                        float* pts_o, float* dirs_o, float* dt_o, float* t_o, int* anchors_o,
-                        void* feat_o_f16 /* nullable */, void* stream);
 /* Forward composite. logit: scene_feat[:,0] (stride logit_stride); rgb [P,3]; t is the raw sample t
  * (the +1e-2 of Renderer.cpp:197 is applied inside).  Outputs per ray: colors[3], disparity, depth;
  * per point: weights. */
 int f2b_composite_fwd(const float* logit, int logit_stride, const float* rgb, const float* dt,
                       const float* t, const int* pts_idx_bounds, const float* bg_color, int n_rays,
                       float* colors, float* disparity, float* depth, float* weights, void* stream);
-/* Backward of the above (+ TruncExp backward + optional GradientScaling, CustomOps.cu:68-80):
- * given dL/dcolors [R,3], dL/ddisparity [R], dL/ddepth [R] (nullable), dL/dweights [P] (nullable)
- * -> dL/dlogit [P] (written with stride dlogit_stride), dL/drgb [P,3].
- * grad_scaling_progress >= 1 disables gradient scaling. */
-int f2b_composite_bwd(const float* logit, int logit_stride, const float* rgb, const float* dt,
-                      const float* t, const int* pts_idx_bounds, const float* bg_color, int n_rays,
-                      const float* d_colors, const float* d_disparity, const float* d_depth,
-                      const float* d_weights, float grad_scaling_progress,
-                      float* d_logit, int dlogit_stride, float* d_rgb, void* stream);
-/* f2b_composite_bwd with the colour activation's backward (f2b_shader_act_bwd) applied on the way out: instead of
- * d_rgb [P,3] fp32 it writes the shader MLP's dL/dout row d_raw [P,16] fp16 = loss_scale * d_rgb * sigmoid'(raw), 0 x 13. */
+/* Backward of the above (+ TruncExp backward + optional GradientScaling, CustomOps.cu:68-80) with the colour activation's
+ * backward (f2b_shader_act_bwd) applied on the way out: given dL/dcolors [R,3], dL/ddisparity [R], dL/ddepth [R] (nullable),
+ * dL/dweights [P] (nullable) -> dL/dlogit [P] (written with stride dlogit_stride) and, instead of dL/drgb, the shader MLP's
+ * dL/dout row d_raw [P,16] fp16 = loss_scale * dL/drgb * sigmoid'(raw), 0 x 13.  grad_scaling_progress >= 1 disables
+ * gradient scaling. */
 int f2b_composite_act_bwd(const float* logit, int logit_stride, const float* rgb, const float* dt, const float* t,
                           const int* pts_idx_bounds, const float* bg_color, int n_rays, const float* d_colors,
                           const float* d_disparity, const float* d_depth, const float* d_weights,

@@ -12,7 +12,7 @@
 # And the reference-configs module (tests/test_gpu_ref_configs.py): both reference binaries, three arms on free, big20 and big22.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
-     "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_fused_f16"
+     "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_f16"
      tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py tests/test_gpu_train_maintenance.py
      tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py tests/test_gpu_cpp_ops_reference.py tests/test_gpu_geometry.py tests/test_gpu_normals.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py

@@ -15,7 +15,7 @@ def declared_symbols():
 def test_header_declares_the_path():
     syms = declared_symbols()
     for need in ("f2b_sampler_count", "f2b_sampler_fill", "f2b_hash_fwd", "f2b_hash_bwd", "f2b_mlp_fwd", "f2b_mlp_bwd",
-                 "f2b_composite_fwd", "f2b_composite_bwd", "f2b_early_stop", "f2b_compact_samples", "f2b_sh_encode"):
+                 "f2b_composite_fwd", "f2b_composite_act_bwd", "f2b_early_stop_rays", "f2b_compact_slots", "f2b_sh_encode"):
         assert need in syms
 
 
@@ -24,6 +24,16 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(_lib.LIB_PATH)
     missing = [s for s in declared_symbols() if not hasattr(lib, s)]
     assert not missing, f"declared in include/f2nerf_b200.h but not exported: {missing}"
+
+
+def test_header_declares_every_exported_symbol():
+    """An f2b_ entry point the library exports but the header does not declare is reachable by no binding."""
+    import subprocess
+    from f2nerf_b200 import _lib
+    out = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    exported = {f[-1] for f in (line.split() for line in out.splitlines()) if f and f[-1].startswith("f2b_")}
+    undeclared = sorted(exported - set(declared_symbols()))
+    assert exported and not undeclared, f"exported but not declared in include/f2nerf_b200.h: {undeclared}"
 
 
 def test_python_binding_covers_the_header():

@@ -13,10 +13,11 @@ from .eval import ImageMetrics, RenderAllImages, RenderNormals, RenderPath, Rend
 from .field import Hash3DAnchored, TCNNWP
 from .ops import CustomOps, FlexOps
 from .optim import FusedAdam
+from .pose import RayGradient, RefinePose
 from .renderer import Renderer, RenderResult, check_backward_nan
 from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultFlex
 from .shader import SHShader
 
-__all__ = ["FusedAdam", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
+__all__ = ["FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
            "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

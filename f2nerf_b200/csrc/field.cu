@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "hash.cuh"
 #include "locate.cuh"
+#include "shader.cuh"
 #include "tc.cuh"
 
 namespace f2b {
@@ -239,6 +240,30 @@ struct GradSmem {
 };
 constexpr int kGradLd = 36;             // fp32 row pitch: conflict-free float4 row reads
 
+// sum_l 0.5 scale_l . grad_level(dfeat_l): the gradient with respect to the warped point (x, y, z) of volume v, given the row's 16
+// level pairs of dL/dfeat (fp32 values of the fp16 rows)
+__device__ __forceinline__ void warped_grad(const __half* __restrict__ table, const int* __restrict__ prim_pool,
+                                            const float* __restrict__ bias_pool, int n_volumes, int local_size, const float* s_scale,
+                                            float x, float y, float z, int v, const float* row, float gw[3]) {
+  const float x0 = fmul(fadd(x, 1.f), .5f), x1 = fmul(fadd(y, 1.f), .5f), x2 = fmul(fadd(z, 1.f), .5f);
+  gw[0] = gw[1] = gw[2] = 0.f;
+#pragma unroll 1
+  for (int l = 0; l < F2B_N_LEVELS; l++) {
+    const int tv = l * n_volumes + v;
+    const float* bias = bias_pool + tv * 3;
+    const float scale = s_scale[l];
+    Corner8 c;
+    corners(x0, x1, x2, scale, prim_pool + tv * 3, bias, (unsigned)local_size, c);
+    const float px = ffma(x0, scale, __ldg(bias)), py = ffma(x1, scale, __ldg(bias + 1)), pz = ffma(x2, scale, __ldg(bias + 2));
+    const float2 d = *reinterpret_cast<const float2*>(row + 2 * l);
+    float gl[3];
+    grad_level(table, l, local_size, c, fsub(px, floorf(px)), fsub(py, floorf(py)), fsub(pz, floorf(pz)), d.x, d.y, gl);
+    const float dpdw = fmul(.5f, scale);                          // p = ((w + 1) / 2) * scale + bias
+#pragma unroll
+    for (int k = 0; k < 3; k++) gw[k] = ffma(dpdw, gl[k], gw[k]);
+  }
+}
+
 template <bool SLOTS, class Src>
 __global__ void __launch_bounds__(kFT, kFieldDefaultMinB)
 field_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool,
@@ -353,24 +378,8 @@ field_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim
     // ---- my row: 16 level gradients, then J^T ----------------------------------------------------------------------------------
     float g[3] = {0.f, 0.f, 0.f};
     if (hit) {
-      const float x0 = fmul(fadd(x, 1.f), .5f), x1 = fmul(fadd(y, 1.f), .5f), x2 = fmul(fadd(z, 1.f), .5f);
-      float gw[3] = {0.f, 0.f, 0.f};
-      const float* row = s_rows + tid * kGradLd;
-#pragma unroll 1
-      for (int l = 0; l < F2B_N_LEVELS; l++) {
-        const int tv = l * n_volumes + v;
-        const float* bias = bias_pool + tv * 3;
-        const float scale = s_scale[l];
-        Corner8 c;
-        corners(x0, x1, x2, scale, prim_pool + tv * 3, bias, (unsigned)local_size, c);
-        const float px = ffma(x0, scale, __ldg(bias)), py = ffma(x1, scale, __ldg(bias + 1)), pz = ffma(x2, scale, __ldg(bias + 2));
-        const float2 d = *reinterpret_cast<const float2*>(row + 2 * l);
-        float gl[3];
-        grad_level(table, l, local_size, c, fsub(px, floorf(px)), fsub(py, floorf(py)), fsub(pz, floorf(pz)), d.x, d.y, gl);
-        const float dpdw = fmul(.5f, scale);                        // p = ((w + 1) / 2) * scale + bias
-#pragma unroll
-        for (int k = 0; k < 3; k++) gw[k] = ffma(dpdw, gl[k], gw[k]);
-      }
+      float gw[3];
+      warped_grad(table, prim_pool, bias_pool, n_volumes, local_size, s_scale, x, y, z, v, s_rows + tid * kGradLd, gw);
       float X, Y, Z, J[3][3];
       src.world(p, X, Y, Z);
       warp_jacobian(trans + v, X, Y, Z, J);
@@ -424,6 +433,183 @@ normals_finish_kernel(const float* __restrict__ tile_partials, const int* __rest
   const float len = fsqrt(fadd(fadd(fmul(N[0], N[0]), fmul(N[1], N[1])), fmul(N[2], N[2])));
 #pragma unroll
   for (int c = 0; c < 3; c++) normals[size_t(r) * 3 + c] = len > 0.f ? fdiv(N[c], len) : 0.f;
+}
+
+
+// ---- gradient of the rendered colour with respect to the rays (DESIGN §3k) -----------------------------------------------------
+// Per 128-row tile of a VALIDATE batch's compacted survivors: the field-MLP backward of f2b_mlp_bwd2 (hidden0 == NULL,
+// n_hidden_matmuls 0) on the row's fp16 dL/dout — the same MMAs on the same operand tiles, so dfeat has its bits — then per thread
+// grad_w = sum_l 0.5 scale_l grad_level(dfeat_l), dL/dx = J^T grad_w at the world point fma(t, d, o) the march formed, and the SH4
+// term dL/ddir = sum_k dL/dmlp_in[16 + k] dsh4_k/ddir.  Each row leaves (dL/dx, t dL/dx + dL/ddir) in row_work; ray_grad_finish_kernel
+// sums a ray's rows serially in row order.  t, dt, the kept set and the leaf are data, not differentiated.
+struct RayGradSmem {
+  static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB  the encoded features
+  static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB  H, then dH in place
+  static constexpr int ROWS = 0;        // [128][kGradLd] fp32 dfeat rows (over A0 / A1, both dead by then)
+  static constexpr int W0 = 24576;      // [64 x 32]  SW64       4 KB
+  static constexpr int WO = 28672;      // [16 x 64]  SW128      2 KB
+  static constexpr int DO = 30720;      // [128 x 16] f16 SW32   4 KB  dL/dout rows
+  static constexpr int SCALE = 34816;   // 16 level scales
+  static constexpr int BYTES = SCALE + 64 + 1024;
+};
+
+// the ray whose rows [bounds[r,0], bounds[r,1]) hold row p: the last ray starting at or before p (rays without rows start where the
+// next non-empty one does, so they are never last)
+__device__ __forceinline__ int ray_of_row(const int* __restrict__ bounds, int n_rays, int p) {
+  int lo = 0, hi = n_rays - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(bounds + 2 * mid) <= p) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+constexpr int kRayGradMinB = 3;          // 4 CTAs per SM would cap the kernel at 128 registers and spill
+
+__global__ void __launch_bounds__(kFT, kRayGradMinB)
+ray_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool, int n_volumes,
+                int local_size, const __half* __restrict__ params, const TransInfo* __restrict__ trans, const __half* __restrict__ feat,
+                const __half* __restrict__ d_out, const __half* __restrict__ d_in, const float* __restrict__ pts,
+                const float* __restrict__ t, const float* __restrict__ dirs, const int* __restrict__ anchors,
+                const float* __restrict__ rays_o, const int* __restrict__ bounds, int n_rays, int n_pts, float inv_field_scale,
+                float inv_shader_scale, float* __restrict__ row_work, float* __restrict__ d_pts, float* __restrict__ d_dirs,
+                __half* __restrict__ dfeat16) {
+  using S = RayGradSmem;
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* s_scale = reinterpret_cast<float*>(sm + S::SCALE);
+  float* s_rows = reinterpret_cast<float*>(sm + S::ROWS);
+  const int tid = threadIdx.x;
+
+  for (int i = tid; i < 64 * 4; i += kFT) {                       // W0 [64 x 32] -> SW64
+    const int r = i >> 2, c = i & 3;
+    *reinterpret_cast<uint4*>(sm + S::W0 + sw64_off(r, c)) = *reinterpret_cast<const uint4*>(params + r * 32 + c * 8);
+  }
+  for (int i = tid; i < 16 * 8; i += kFT) {                       // Wout [16 x 64] -> SW128
+    const int r = i >> 3, c = i & 7;
+    *reinterpret_cast<uint4*>(sm + S::WO + sw128_off(r, c)) = *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
+  }
+  if (tid < F2B_N_LEVELS) s_scale[tid] = level_scale(tid);
+  __syncthreads();
+  const uint32_t a0 = smem_u32(sm + S::A0), a1 = smem_u32(sm + S::A1), s_do = smem_u32(sm + S::DO);
+  const uint32_t w0 = smem_u32(sm + S::W0), wo = smem_u32(sm + S::WO);
+
+  const int n_tiles = (n_pts + kFT - 1) / kFT;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int p = tile * kFT + tid;
+    const bool valid = p < n_pts;
+    {                                                               // my operand rows; rows past n_pts are zero, as f2b_mlp_bwd2 fills them
+      const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
+      const uint4* xs = reinterpret_cast<const uint4*>(feat + size_t(p) * 32);
+      const uint4* ds = reinterpret_cast<const uint4*>(d_out + size_t(p) * 16);
+#pragma unroll
+      for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(sm + S::A0 + sw64_off(tid, c)) = valid ? __ldg(xs + c) : z4;
+#pragma unroll
+      for (int c = 0; c < 2; c++) *reinterpret_cast<uint4*>(sm + S::DO + sw32_off(tid, c)) = valid ? __ldg(ds + c) : z4;
+    }
+    fence_async_smem();
+    __syncthreads();
+    // ---- F0: H = relu(X . W0^T) ---------------------------------------------------------------------------------------------
+    {
+      Acc<64> acc;
+      wg_fence();
+      mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
+      wg_commit();
+      wg_wait();
+      acc_relu_to_tile(acc, sm + S::A1, tid);
+      fence_async_smem();
+      __syncthreads();
+      // ---- A: dH = dOut . Wout, masked by the fp16 hidden tile, over it in place ----------------------------------------------
+      wg_fence();
+      mma_m128<64, 1, 1>(acc, s_do, 32, wo, 128, false);
+      wg_commit();
+      wg_wait();
+      __syncthreads();                                              // every warp is done with H as an operand
+      relu_bwd_epilogue(acc, sm + S::A1, sm + S::A1, tid);
+    }
+    fence_async_smem();
+    __syncthreads();
+    // ---- C: dfeat = dH . W0 -> fp16 (as store_din packs it) -> fp32 rows -------------------------------------------------------
+    {
+      Acc<32> acc_in;
+      wg_fence();
+      mma_m128<32, 1, 4>(acc_in, a1, 128, w0, 64, false);
+      wg_commit();
+      wg_wait();
+      __syncthreads();                                              // every warp's MMA is done reading A1 (the rows overwrite it)
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int i = 0; i < 16; i += 2) {
+          const uint32_t bits = pk(acc_in.d[h][i], acc_in.d[h][i + 1]);
+          const int r = acc_row(tid, h, i), col = acc_col(tid, i);
+          if (dfeat16 && tile * kFT + r < n_pts) *reinterpret_cast<uint32_t*>(dfeat16 + size_t(tile * kFT + r) * 32 + col) = bits;
+          *reinterpret_cast<float2*>(s_rows + r * kGradLd + col) = __half22float2(*reinterpret_cast<const __half2*>(&bits));
+        }
+    }
+    __syncthreads();
+    // ---- my row: grad_w, J^T, the SH4 term ---------------------------------------------------------------------------------------
+    if (valid) {
+      const float x = __ldg(pts + size_t(p) * 3), y = __ldg(pts + size_t(p) * 3 + 1), z = __ldg(pts + size_t(p) * 3 + 2);
+      const int v = __ldg(anchors + size_t(p) * 3);
+      float gw[3];
+      warped_grad(table, prim_pool, bias_pool, n_volumes, local_size, s_scale, x, y, z, v, s_rows + tid * kGradLd, gw);
+      const int ray = ray_of_row(bounds, n_rays, p);
+      const float tp = __ldg(t + p);
+      const float dx = __ldg(dirs + size_t(p) * 3), dy = __ldg(dirs + size_t(p) * 3 + 1), dz = __ldg(dirs + size_t(p) * 3 + 2);
+      const float X = ffma(tp, dx, __ldg(rays_o + ray * 3)), Y = ffma(tp, dy, __ldg(rays_o + ray * 3 + 1)),
+                  Z = ffma(tp, dz, __ldg(rays_o + ray * 3 + 2));
+      float J[3][3];
+      warp_jacobian(trans + v, X, Y, Z, J);
+      float g[3];
+#pragma unroll
+      for (int k = 0; k < 3; k++) g[k] = fmul(ffma(J[0][k], gw[0], ffma(J[1][k], gw[1], fmul(J[2][k], gw[2]))), inv_field_scale);
+      float dsh[16];
+      {
+        const uint4* src = reinterpret_cast<const uint4*>(d_in + size_t(p) * 32 + 16);
+#pragma unroll
+        for (int q = 0; q < 2; q++) {
+          const uint4 u = __ldg(src + q);
+          const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+          for (int j = 0; j < 4; j++) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[j]));
+            dsh[8 * q + 2 * j] = fmul(f.x, inv_shader_scale);
+            dsh[8 * q + 2 * j + 1] = fmul(f.y, inv_shader_scale);
+          }
+        }
+      }
+      float gd[3];
+      sh4_grad(dx, dy, dz, dsh, gd);
+      float* w = row_work + size_t(p) * 6;
+#pragma unroll
+      for (int k = 0; k < 3; k++) { w[k] = g[k]; w[3 + k] = ffma(tp, g[k], gd[k]); }
+      if (d_pts) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) d_pts[size_t(p) * 3 + k] = g[k];
+      }
+      if (d_dirs) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) d_dirs[size_t(p) * 3 + k] = gd[k];
+      }
+    }
+    __syncthreads();                                                // the rows have been read before the next tile's A0 stores
+  }
+}
+
+// d_o[r] = sum of the ray's rows' dL/dx, d_d[r] = sum of their t dL/dx + dL/ddir, serially in row order
+__global__ void __launch_bounds__(128)
+ray_grad_finish_kernel(const float* __restrict__ row_work, const int* __restrict__ bounds, int n_rays, float* __restrict__ d_o,
+                       float* __restrict__ d_d) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rays) return;
+  float s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int p = bounds[2 * r]; p < bounds[2 * r + 1]; p++)
+#pragma unroll
+    for (int k = 0; k < 6; k++) s[k] = fadd(s[k], row_work[size_t(p) * 6 + k]);
+#pragma unroll
+  for (int k = 0; k < 3; k++) { d_o[size_t(r) * 3 + k] = s[k]; d_d[size_t(r) * 3 + k] = s[3 + k]; }
 }
 
 }  // namespace f2b
@@ -568,4 +754,31 @@ extern "C" int f2b_render_normals_slots(const void* trans, const void* table_f16
                     nullptr, w_slots, tile_partials, stream);
   normals_finish_kernel<<<div_up(n_rays, 128), 128, 0, as_stream(stream)>>>(tile_partials, kept_counts, n_rays, slot_size, normals);
   return check_launch("f2b_render_normals_slots");
+}
+
+extern "C" int f2b_ray_grad(const void* trans, const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
+                            int local_size, const void* field_params_f16, const void* feat_f16, const void* d_field_out_f16,
+                            const void* d_mlp_in_f16, const float* pts, const float* t, const float* dirs, const int* anchors,
+                            const float* rays_o, const int* pts_idx_bounds, int n_rays, int n_pts, float inv_field_loss_scale,
+                            float inv_shader_loss_scale, float* row_work, float* d_rays_o, float* d_rays_d, float* d_pts, float* d_dirs,
+                            void* dfeat16, void* stream) {
+  if (n_rays <= 0) return F2B_OK;
+  F2B_REQUIRE(pts_idx_bounds && rays_o && d_rays_o && d_rays_d && n_pts >= 0, "f2b_ray_grad: null pointer");
+  if (n_pts > 0) {
+    F2B_REQUIRE(trans && table_f16 && prim_pool && bias_pool && field_params_f16 && feat_f16 && d_field_out_f16 && d_mlp_in_f16 && pts &&
+                    t && dirs && anchors && row_work,
+                "f2b_ray_grad: null pointer");
+    F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_ray_grad: bad n_volumes/local_size");
+    int sms = 132;
+    f2b_device_info(&sms, nullptr);
+    const int n_tiles = div_up(n_pts, kFT);
+    const int grid = n_tiles < sms * kRayGradMinB ? n_tiles : sms * kRayGradMinB;
+    cudaFuncSetAttribute(ray_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RayGradSmem::BYTES);
+    ray_grad_kernel<<<grid, kFT, RayGradSmem::BYTES, as_stream(stream)>>>(
+        (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16, (const TransInfo*)trans,
+        (const __half*)feat_f16, (const __half*)d_field_out_f16, (const __half*)d_mlp_in_f16, pts, t, dirs, anchors, rays_o,
+        pts_idx_bounds, n_rays, n_pts, inv_field_loss_scale, inv_shader_loss_scale, row_work, d_pts, d_dirs, (__half*)dfeat16);
+  }
+  ray_grad_finish_kernel<<<div_up(n_rays, 128), 128, 0, as_stream(stream)>>>(row_work, pts_idx_bounds, n_rays, d_rays_o, d_rays_d);
+  return check_launch("f2b_ray_grad");
 }

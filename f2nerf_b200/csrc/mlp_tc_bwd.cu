@@ -36,11 +36,6 @@ struct BwdSmem {
   static constexpr int BYTES = STAGE0 + 2 * STAGE_BYTES + 1024;
 };
 
-__device__ __forceinline__ uint32_t pk(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
-
 template <int K>
 __device__ __forceinline__ void stage_w(const __half* __restrict__ w, int rows, unsigned char* dst) {
   constexpr int chunks = K / 8;
@@ -86,18 +81,6 @@ __device__ __forceinline__ void prefetch_tile(const __half* __restrict__ dout, c
     cp16(stage + S::H0 + sw128_off(r, c & 7), s_h0 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
     if (NH) cp16(stage + S::H1 + sw128_off(r, c & 7), s_h1 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
-}
-
-// masked epilogue: acc * [h > 0] -> fp16 dH tile (SW128); h_tile may be dh_tile (each element is read, then written, by one thread)
-__device__ __forceinline__ void relu_bwd_epilogue(const Acc<64>& acc, const unsigned char* h_tile, unsigned char* dh_tile, int t) {
-#pragma unroll
-  for (int h = 0; h < 2; h++)
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const uint32_t off = sw128_col(acc_row(t, h, i), acc_col(t, i));
-      const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(h_tile + off));
-      *reinterpret_cast<uint32_t*>(dh_tile + off) = pk(hf.x > 0.f ? acc.d[h][i] : 0.f, hf.y > 0.f ? acc.d[h][i + 1] : 0.f);
-    }
 }
 
 // dIn rows of the tile -> global fp16 [P,32]

@@ -32,6 +32,44 @@ __device__ __forceinline__ void sh4(float x, float y, float z, float o[16]) {
   o[15] = fmul(fmul(x, 0.59004358992664352f), __fmaf_rn(y2, 3.0f, -x2));
 }
 
+// d[16] . d sh4 / d(x, y, z): the gradient of sum_k d[k] o[k] with respect to the direction, from the polynomials of sh4 taken
+// with x, y, z independent (the caller chains through the normalisation).  Pose refinement (ray_grad_kernel, DESIGN §3k).
+__device__ __forceinline__ void sh4_grad(float x, float y, float z, const float d[16], float g[3]) {
+  const float xy = fmul(x, y), xz = fmul(x, z), yz = fmul(y, z), x2 = fmul(x, x), y2 = fmul(y, y), z2 = fmul(z, z);
+  const float c1 = 0.48860251190291987f, c4 = 1.0925484305920792f, c9 = 0.59004358992664352f, c10 = 2.8906114426405538f;
+  const float c11 = 0.45704579946446572f, c12 = 0.3731763325901154f, c14 = 1.4453057213202769f;
+  const float f15 = __fmaf_rn(z2, -5.0f, 1.0f);                   // 1 - 5 z^2
+  const float q9 = fmul(3.f * c9, fsub(y2, x2));                   // d o9 / dy = d o15 / dx = 3 c9 (y^2 - x^2)
+  float gx = fmul(-c1, d[3]);
+  gx = ffma(fmul(c4, y), d[4], gx);
+  gx = ffma(fmul(-c4, z), d[7], gx);
+  gx = ffma(fmul(2.f * 0.54627421529603959f, x), d[8], gx);
+  gx = ffma(fmul(-6.f * c9, xy), d[9], gx);
+  gx = ffma(fmul(c10, yz), d[10], gx);
+  gx = ffma(fmul(c11, f15), d[13], gx);
+  gx = ffma(fmul(2.f * c14, xz), d[14], gx);
+  gx = ffma(q9, d[15], gx);
+  float gy = fmul(-c1, d[1]);
+  gy = ffma(fmul(c4, x), d[4], gy);
+  gy = ffma(fmul(-c4, z), d[5], gy);
+  gy = ffma(fmul(-2.f * 0.54627421529603959f, y), d[8], gy);
+  gy = ffma(q9, d[9], gy);
+  gy = ffma(fmul(c10, xz), d[10], gy);
+  gy = ffma(fmul(c11, f15), d[11], gy);
+  gy = ffma(fmul(-2.f * c14, yz), d[14], gy);
+  gy = ffma(fmul(6.f * c9, xy), d[15], gy);
+  float gz = fmul(c1, d[2]);
+  gz = ffma(fmul(-c4, y), d[5], gz);
+  gz = ffma(fmul(2.f * 0.94617469575755997f, z), d[6], gz);
+  gz = ffma(fmul(-c4, x), d[7], gz);
+  gz = ffma(fmul(c10, xy), d[10], gz);
+  gz = ffma(fmul(-10.f * c11, yz), d[11], gz);
+  gz = ffma(fmul(c12, __fmaf_rn(z2, 15.f, -3.f)), d[12], gz);
+  gz = ffma(fmul(-10.f * c11, xz), d[13], gz);
+  gz = ffma(fmul(c14, fsub(x2, y2)), d[14], gz);
+  g[0] = gx; g[1] = gy; g[2] = gz;
+}
+
 // Shader-MLP input row: fp16([1, feat[1..15]] + app_emb[cam] | SH4(dir)) (Renderer.cpp:179-187, SHShader.cpp:23-26,
 // identity-encoding cast).  feat[0..15] = the field output (fp16-rounded values), feat[0] is ignored.
 __device__ __forceinline__ void shade_row(const float feat[16], const float* __restrict__ emb_row /* nullable */,

@@ -128,6 +128,24 @@ __device__ __forceinline__ void acc_relu_to_tile(const Acc<64>& acc, unsigned ch
     }
 }
 
+// two floats -> packed half2 bits (round to nearest)
+__device__ __forceinline__ uint32_t pk(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// masked epilogue: acc * [h > 0] -> fp16 dH tile (SW128); h_tile may be dh_tile (each element is read, then written, by one thread)
+__device__ __forceinline__ void relu_bwd_epilogue(const Acc<64>& acc, const unsigned char* h_tile, unsigned char* dh_tile, int t) {
+#pragma unroll
+  for (int h = 0; h < 2; h++)
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const uint32_t off = sw128_col(acc_row(t, h, i), acc_col(t, i));
+      const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(h_tile + off));
+      *reinterpret_cast<uint32_t*>(dh_tile + off) = pk(hf.x > 0.f ? acc.d[h][i] : 0.f, hf.y > 0.f ? acc.d[h][i + 1] : 0.f);
+    }
+}
+
 // accumulator -> fp32 rows [128][ld] in shared memory (ld = 20 for N = 16: conflict-free float4 row reads)
 template <int N>
 __device__ __forceinline__ void acc_to_rows(const Acc<N>& acc, float* rows, int ld, int t) {

@@ -234,6 +234,16 @@ def render_normals_slots(trans, table_f16, prim_pool, bias_pool, n_volumes, loca
     return normals
 
 
+def ray_grad(trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, feat_f16, d_field_out_f16, d_mlp_in_f16, pts,
+             t, dirs, anchors, rays_o, bounds, inv_field_loss_scale, inv_shader_loss_scale, row_work, d_rays_o, d_rays_d, d_pts=None,
+             d_dirs=None, dfeat16=None):
+    """f2b_ray_grad: the survivors' rows (len(t) of them) of a VALIDATE batch and the chain's fp16 dL/dout / dL/dinput rows ->
+    d_rays_o, d_rays_d [R,3] (the latter with respect to the unit direction); the per-row outputs when given."""
+    call("f2b_ray_grad", trans, table_f16, prim_pool, bias_pool, int(n_volumes), int(local_size), params_f16, feat_f16, d_field_out_f16,
+         d_mlp_in_f16, pts, t, dirs, anchors, rays_o, bounds, int(bounds.shape[0]), int(t.shape[0]), float(inv_field_loss_scale),
+         float(inv_shader_loss_scale), row_work, d_rays_o, d_rays_d, d_pts, d_dirs, dfeat16, stream())
+
+
 def iso_count(logit, level, empty_logit, ez0, ez1, edge_mask, vert_counts, tri_counts):
     nz, ny, nx = logit.shape
     call("f2b_iso_count", logit, nx, ny, nz, float(level), float(empty_logit), int(ez0), int(ez1), edge_mask, vert_counts,

@@ -213,6 +213,23 @@ int f2b_render_normals_slots(const void* trans, const void* table_f16, const int
                              const int* slot_anchors /* [.,2] */, const int* kept_counts, const float* w_slots,
                              const float* rays_o, const float* rays_d, int n_rays, int slot_size, float* tile_partials,
                              float* normals /* [n_rays,3] */, void* stream);
+/* Gradient of the rendered colour with respect to the rays of a VALIDATE batch (DESIGN.md §3k), behind the composite, shader-MLP and
+ * input-assembly backward: rows p < n_pts are the compacted survivors f2b_render_phase2_fwd leaves (pts, t, dirs, anchors [P,3], feat
+ * [P,32] fp16), d_field_out [P,16] fp16 = f2b_shader_prep_bwd_f16's dL/dout of the field MLP and d_mlp_in [P,32] fp16 = f2b_mlp_bwd2's
+ * dL/dinput of the shader, both loss-scaled.  Per row: dfeat = the field-MLP backward of d_field_out (bit-identical to f2b_mlp_bwd2's
+ * dL/dinput with hidden0 == NULL), grad_w = sum_l 0.5 scale_l dfeat_l . d blend_l / dp, dL/dx = J^T grad_w * inv_field_loss_scale
+ * with J = QueryFrameTransformJac of the row's leaf at the world point fma(t, dirs, rays_o[ray]) as the march formed it, and dL/ddir =
+ * sum_k d_mlp_in[p,16+k] * inv_shader_loss_scale * d sh4_k / d dir at the unit direction, its components taken as independent.
+ * Per ray (rows pts_idx_bounds[r,0] .. [r,1], summed serially in row order: the same bits for any launch and any batch split):
+ * d_rays_o[r] = sum dL/dx, d_rays_d[r] = sum (t dL/dx + dL/ddir), the gradient with respect to the unit direction (the caller chains
+ * through the normalisation).  t, dt, the kept set and the leaf are held fixed, not differentiated.  row_work: [P,6] fp32 scratch.
+ * Nullable per-row outputs: d_pts [P,3] = dL/dx, d_dirs [P,3] = dL/ddir, dfeat16 [P,32] fp16 = dfeat. */
+int f2b_ray_grad(const void* trans, const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                 const void* field_params_f16, const void* feat_f16, const void* d_field_out_f16, const void* d_mlp_in_f16,
+                 const float* pts, const float* t, const float* dirs, const int* anchors, const float* rays_o,
+                 const int* pts_idx_bounds, int n_rays, int n_pts, float inv_field_loss_scale, float inv_shader_loss_scale,
+                 float* row_work, float* d_rays_o /* [R,3] */, float* d_rays_d /* [R,3] */, float* d_pts, float* d_dirs, void* dfeat16,
+                 void* stream);
 /* Isosurface {logit = level} of an nx x ny x nz logit lattice (x fastest) by marching tetrahedra on the Kuhn split of each
  * cell, lattice points outside the lattice reading empty_logit (<= level), for the cells of extended z-layers [ez0, ez1)
  * (0 <= ez0 < ez1 <= nz + 1; extended layer e holds lattice layer e - 1, see geometry.cu).  Pass 1 writes, per owner

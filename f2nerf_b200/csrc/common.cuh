@@ -29,6 +29,12 @@ static inline int resident_per_sm(Kernel kernel, int threads, size_t smem_bytes)
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, smem_bytes) != cudaSuccess) n = 1;
   return n > 0 ? n : 1;
 }
+// grid of a persistent kernel over n_work tiles (or rays): one CTA per tile, at most per_sm CTAs on every SM
+static inline int persistent_grid(int n_work, int per_sm) {
+  int sms = 132;
+  f2b_device_info(&sms, nullptr);
+  return n_work < sms * per_sm ? n_work : sms * per_sm;
+}
 
 // ---- reference POD layouts (PersSampler.h:15-37), restated without Eigen -------------------
 struct __align__(32) TreeNode {      // 64 B

@@ -24,13 +24,17 @@ using namespace tc;
 constexpr int kFT = 128;
 constexpr int kFieldDefaultMinB = 4;   // resident CTAs per SM the kernel is compiled for; see DESIGN.md
 
-struct FieldSmem {
-  static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB
-  static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB
+// Shared memory of the field MLP's 128-row tile, the common prefix of the field kernels' layouts
+struct FieldTileSmem {
+  static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB  the encoded features
+  static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB  H (the gradient kernels: then dH in place)
   static constexpr int W0 = 24576;      // [64 x 32]  SW64       4 KB
   static constexpr int WO = 28672;      // [16 x 64]  SW128      2 KB
-  static constexpr int SCALE = 30720;   // 16 level scales
-  static constexpr int BYTES = 30720 + 64 + 1024;
+  static constexpr int END = 30720;
+};
+struct FieldSmem : FieldTileSmem {
+  static constexpr int SCALE = END;     // 16 level scales
+  static constexpr int BYTES = SCALE + 64 + 1024;
 };
 
 // Where a tile's rows come from.  rows(tile, n_pts): the tile's output rows are its first rows(...) rows (0: skip the tile,
@@ -43,12 +47,14 @@ struct SampleSource {      // the march's warped samples: a compact [P] layout, 
   const int* slot_counts;  // slot layout: ray r owns slots [r*slot_size, r*slot_size + count[r]); NULL: compact
   int slot_size;
   static constexpr float empty = 0.f;   // unused: every output row has a point
-  // slot_size is a multiple of the tile, so a tile lies inside one ray
   __device__ __forceinline__ int rows(int tile, int n_pts) const {
+    return slot_counts ? slot_rows(tile, n_pts, slot_counts, slot_size) : n_pts - tile * kFT;
+  }
+  // slot layout: slot_size is a multiple of the tile, so a tile lies inside one ray
+  static __device__ __forceinline__ int slot_rows(int tile, int n_pts, const int* counts, int slot_size) {
     const int t0 = tile * kFT;
-    if (!slot_counts) return n_pts - t0;
     const int ray = t0 / slot_size;
-    return min(n_pts, ray * slot_size + __ldg(slot_counts + ray)) - t0;
+    return min(n_pts, ray * slot_size + __ldg(counts + ray)) - t0;
   }
   __device__ __forceinline__ bool point(int p, float& x, float& y, float& z, int& v) const {
     x = __ldg(pts + size_t(p) * 3); y = __ldg(pts + size_t(p) * 3 + 1); z = __ldg(pts + size_t(p) * 3 + 2);
@@ -100,11 +106,7 @@ struct KeptSlotSource {
   const float* rays_d;
   int slot_size;
   static constexpr float empty = 0.f;   // unused: every output row has a point
-  __device__ __forceinline__ int rows(int tile, int n_pts) const {
-    const int t0 = tile * kFT;
-    const int ray = t0 / slot_size;
-    return min(n_pts, ray * slot_size + __ldg(kept + ray)) - t0;
-  }
+  __device__ __forceinline__ int rows(int tile, int n_pts) const { return SampleSource::slot_rows(tile, n_pts, kept, slot_size); }
   __device__ __forceinline__ bool point(int p, float& x, float& y, float& z, int& v) const {
     x = __ldg(s_pts + size_t(p) * 3); y = __ldg(s_pts + size_t(p) * 3 + 1); z = __ldg(s_pts + size_t(p) * 3 + 2);
     v = __ldg(s_anchors + size_t(p) * 2);
@@ -119,27 +121,58 @@ struct KeptSlotSource {
   }
 };
 
+// ---- steps of the field MLP on a 128-row tile, shared by the field kernels ------------------------------------------------------
+// W0 / Wout into the tile's weight slots, Wout row 0 also to wo0 (may be NULL; fp16 [64]), and the 16 level scales into s_scale
+// (run-time MUFU.EX2, like the reference).  The weights are staged by shifts and masks rather than by tc::stage_weights, whose
+// signed division compiles to different code in these kernels.
+__device__ __forceinline__ void stage_field(const __half* __restrict__ params, unsigned char* sm, float* s_scale, unsigned char* wo0,
+                                            int t) {
+  for (int i = t; i < 64 * 4; i += kFT) {                         // W0 [64 x 32] -> SW64
+    const int r = i >> 2, c = i & 3;
+    *reinterpret_cast<uint4*>(sm + FieldTileSmem::W0 + sw64_off(r, c)) = *reinterpret_cast<const uint4*>(params + r * 32 + c * 8);
+  }
+  for (int i = t; i < 16 * 8; i += kFT) {                         // Wout [16 x 64] -> SW128
+    const int r = i >> 3, c = i & 7;
+    *reinterpret_cast<uint4*>(sm + FieldTileSmem::WO + sw128_off(r, c)) =
+        *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
+  }
+  if (wo0 && t < 8) reinterpret_cast<uint4*>(wo0)[t] = reinterpret_cast<const uint4*>(params + 64 * 32)[t];
+  if (t < F2B_N_LEVELS) s_scale[t] = level_scale(t);
+}
+
+// layer 0: H = relu(A0 . W0^T) -> fp16 into A1.  `during()` runs while the MMA is in flight.
+template <class During>
+__device__ __forceinline__ void field_layer0(Acc<64>& acc, uint32_t a0, uint32_t w0, unsigned char* a1_tile, int t, During&& during) {
+  wg_fence();
+  mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
+  wg_commit();
+  during();
+  wg_wait();
+  acc_relu_to_tile(acc, a1_tile, t);
+}
+
+// output layer: acc_out = A1 . Wout^T.  `during()` runs while the MMA is in flight.
+template <class During>
+__device__ __forceinline__ void field_out_layer(Acc<16>& acc_out, uint32_t a1, uint32_t wo, During&& during) {
+  wg_fence();
+  mma_m128<16, 0, 4>(acc_out, a1, 128, wo, 128, false);
+  wg_commit();
+  during();
+  wg_wait();
+}
+
 template <bool LOGIT_ONLY, int MINB, class Src>
 __global__ void __launch_bounds__(kFT, MINB)
 field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool,
                  const float* __restrict__ bias_pool, int n_volumes, int local_size,
                  const __half* __restrict__ params, const Src src, int n_pts,
                  float* __restrict__ out, __half* __restrict__ feat_save, __half* __restrict__ hidden_save) {
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   float* s_scale = reinterpret_cast<float*>(sm + FieldSmem::SCALE);
   float* s_rows = reinterpret_cast<float*>(sm + FieldSmem::A1);     // output rows [128][20] fp32 (A1 is dead by then)
   const int tid = threadIdx.x;
 
-  for (int i = tid; i < 64 * 4; i += kFT) {                       // W0 [64 x 32] -> SW64
-    const int r = i >> 2, c = i & 3;
-    *reinterpret_cast<uint4*>(sm + FieldSmem::W0 + sw64_off(r, c)) = *reinterpret_cast<const uint4*>(params + r * 32 + c * 8);
-  }
-  for (int i = tid; i < 16 * 8; i += kFT) {                       // Wout [16 x 64] -> SW128
-    const int r = i >> 3, c = i & 7;
-    *reinterpret_cast<uint4*>(sm + FieldSmem::WO + sw128_off(r, c)) = *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
-  }
-  if (tid < F2B_N_LEVELS) s_scale[tid] = level_scale(tid);        // run-time MUFU.EX2, like the reference
+  stage_field(params, sm, s_scale, nullptr, tid);
   __syncthreads();
   const uint32_t a0 = smem_u32(sm + FieldSmem::A0), a1 = smem_u32(sm + FieldSmem::A1);
   const uint32_t w0 = smem_u32(sm + FieldSmem::W0), wo = smem_u32(sm + FieldSmem::WO);
@@ -169,36 +202,31 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
     fence_async_smem();
     __syncthreads();                                              // (also: the previous tile's output rows have been read)
     // ---- layer 0 on the tensor pipe -------------------------------------------------------------------
-    wg_fence();
-    mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
-    wg_commit();
-    if (feat_save) {                                              // whole-line copy-out of the tile while the MMA reads it
-      const int rows = min(kFT, n_pts - tile * kFT);
-      uint4* dst = reinterpret_cast<uint4*>(feat_save + size_t(tile) * kFT * 32);
+    field_layer0(acc, a0, w0, sm + FieldSmem::A1, tid, [&] {
+      if (feat_save) {                                            // whole-line copy-out of the tile while the MMA reads it
+        const int rows = min(kFT, n_pts - tile * kFT);
+        uint4* dst = reinterpret_cast<uint4*>(feat_save + size_t(tile) * kFT * 32);
 #pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const int c = tid + kFT * j, r = c >> 2;
-        if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A0 + sw64_off(r, c & 3));
+        for (int j = 0; j < 4; j++) {
+          const int c = tid + kFT * j, r = c >> 2;
+          if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A0 + sw64_off(r, c & 3));
+        }
       }
-    }
-    wg_wait();
-    acc_relu_to_tile(acc, sm + FieldSmem::A1, tid);
+    });
     fence_async_smem();
     __syncthreads();
     // ---- output layer -------------------------------------------------------------------------------
-    wg_fence();
-    mma_m128<16, 0, 4>(acc_out, a1, 128, wo, 128, false);
-    wg_commit();
-    if (!LOGIT_ONLY && hidden_save) {
-      const int rows = min(kFT, n_pts - tile * kFT);
-      uint4* dst = reinterpret_cast<uint4*>(hidden_save + size_t(tile) * kFT * 64);
+    field_out_layer(acc_out, a1, wo, [&] {
+      if (!LOGIT_ONLY && hidden_save) {
+        const int rows = min(kFT, n_pts - tile * kFT);
+        uint4* dst = reinterpret_cast<uint4*>(hidden_save + size_t(tile) * kFT * 64);
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
-        const int c = tid + kFT * j, r = c >> 3;
-        if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A1 + sw128_off(r, c & 7));
+        for (int j = 0; j < 8; j++) {
+          const int c = tid + kFT * j, r = c >> 3;
+          if (r < rows) dst[c] = *reinterpret_cast<const uint4*>(sm + FieldSmem::A1 + sw128_off(r, c & 7));
+        }
       }
-    }
-    wg_wait();
+    });
     __syncthreads();                                              // every warp is done with A1 (operand / copy-out)
     acc_to_rows(acc_out, s_rows, kRowLd16, tid);
     __syncthreads();
@@ -226,13 +254,9 @@ field_fwd_kernel(const __half* __restrict__ table, const int* __restrict__ prim_
 // the tensor pipe (W0 as the MN-major operand, as mlp_tc_bwd.cu), rounded to fp16 as the training backward rounds it, then per
 // thread the 16 level gradients and the leaf's Jacobian.  Points: logit and g per row.  Kept slots: sum_i w_i n_i over the tile's
 // rows, serial in row order, one partial per tile (normals_finish_kernel sums a ray's partials in tile order).
-struct GradSmem {
-  static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB
-  static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB  H, then dH in place
+struct GradSmem : FieldTileSmem {
   static constexpr int ROWS = 0;        // [128][kGradLd] fp32 dfeat rows (over A0 / A1, both dead by then)
-  static constexpr int W0 = 24576;      // [64 x 32]  SW64       4 KB
-  static constexpr int WO = 28672;      // [16 x 64]  SW128      2 KB
-  static constexpr int SCALE = 30720;   // 16 level scales
+  static constexpr int SCALE = END;     // 16 level scales
   static constexpr int LOGIT = 30784;   // [128] fp32 output channel 0
   static constexpr int WO0 = 31296;     // [64] f16 Wout row 0
   static constexpr int ADD = 31424;     // [3][128] fp32 w_i n_i (slot source)
@@ -271,8 +295,7 @@ field_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim
                   int n_pts, float empty, float* __restrict__ logit_out, float* __restrict__ grad_out, const float* __restrict__ w_slots,
                   float* __restrict__ tile_partials) {
   using S = GradSmem;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   float* s_scale = reinterpret_cast<float*>(sm + S::SCALE);
   float* s_logit = reinterpret_cast<float*>(sm + S::LOGIT);
   const __half* s_wo0 = reinterpret_cast<const __half*>(sm + S::WO0);
@@ -280,16 +303,7 @@ field_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim
   float* s_add = reinterpret_cast<float*>(sm + S::ADD);
   const int tid = threadIdx.x;
 
-  for (int i = tid; i < 64 * 4; i += kFT) {                       // W0 [64 x 32] -> SW64
-    const int r = i >> 2, c = i & 3;
-    *reinterpret_cast<uint4*>(sm + S::W0 + sw64_off(r, c)) = *reinterpret_cast<const uint4*>(params + r * 32 + c * 8);
-  }
-  for (int i = tid; i < 16 * 8; i += kFT) {                       // Wout [16 x 64] -> SW128
-    const int r = i >> 3, c = i & 7;
-    *reinterpret_cast<uint4*>(sm + S::WO + sw128_off(r, c)) = *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
-  }
-  if (tid < 8) reinterpret_cast<uint4*>(sm + S::WO0)[tid] = reinterpret_cast<const uint4*>(params + 64 * 32)[tid];
-  if (tid < F2B_N_LEVELS) s_scale[tid] = level_scale(tid);
+  stage_field(params, sm, s_scale, sm + S::WO0, tid);
   __syncthreads();
   const uint32_t a0 = smem_u32(sm + S::A0), a1 = smem_u32(sm + S::A1);
   const uint32_t w0 = smem_u32(sm + S::W0), wo = smem_u32(sm + S::WO);
@@ -320,20 +334,13 @@ field_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim
     // ---- forward: layer 0, output layer (field_fwd_kernel's MMAs) ---------------------------------------------------------
     {
       Acc<64> acc;
-      wg_fence();
-      mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
-      wg_commit();
-      wg_wait();
-      acc_relu_to_tile(acc, sm + S::A1, tid);
+      field_layer0(acc, a0, w0, sm + S::A1, tid, [] {});
     }
     fence_async_smem();
     __syncthreads();
     {
       Acc<16> acc_out;
-      wg_fence();
-      mma_m128<16, 0, 4>(acc_out, a1, 128, wo, 128, false);
-      wg_commit();
-      wg_wait();
+      field_out_layer(acc_out, a1, wo, [] {});
       if ((tid & 3) == 0) {                                         // column 0 of the accumulator: elements 0 and 2 of each half
 #pragma unroll
         for (int h = 0; h < 2; h++) { s_logit[acc_row(tid, h, 0)] = acc_out.d[h][0]; s_logit[acc_row(tid, h, 2)] = acc_out.d[h][2]; }
@@ -442,14 +449,10 @@ normals_finish_kernel(const float* __restrict__ tile_partials, const int* __rest
 // grad_w = sum_l 0.5 scale_l grad_level(dfeat_l), dL/dx = J^T grad_w at the world point fma(t, d, o) the march formed, and the SH4
 // term dL/ddir = sum_k dL/dmlp_in[16 + k] dsh4_k/ddir.  Each row leaves (dL/dx, t dL/dx + dL/ddir) in row_work; ray_grad_finish_kernel
 // sums a ray's rows serially in row order.  t, dt, the kept set and the leaf are data, not differentiated.
-struct RayGradSmem {
-  static constexpr int A0 = 0;          // [128 x 32] f16 SW64   8 KB  the encoded features
-  static constexpr int A1 = 8192;       // [128 x 64] f16 SW128 16 KB  H, then dH in place
+struct RayGradSmem : FieldTileSmem {
   static constexpr int ROWS = 0;        // [128][kGradLd] fp32 dfeat rows (over A0 / A1, both dead by then)
-  static constexpr int W0 = 24576;      // [64 x 32]  SW64       4 KB
-  static constexpr int WO = 28672;      // [16 x 64]  SW128      2 KB
-  static constexpr int DO = 30720;      // [128 x 16] f16 SW32   4 KB  dL/dout rows
-  static constexpr int SCALE = 34816;   // 16 level scales
+  static constexpr int DO = END;        // [128 x 16] f16 SW32   4 KB  dL/dout rows
+  static constexpr int SCALE = DO + 4096;   // 16 level scales
   static constexpr int BYTES = SCALE + 64 + 1024;
 };
 
@@ -476,21 +479,12 @@ ray_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim_p
                 float inv_shader_scale, float* __restrict__ row_work, float* __restrict__ d_pts, float* __restrict__ d_dirs,
                 __half* __restrict__ dfeat16) {
   using S = RayGradSmem;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   float* s_scale = reinterpret_cast<float*>(sm + S::SCALE);
   float* s_rows = reinterpret_cast<float*>(sm + S::ROWS);
   const int tid = threadIdx.x;
 
-  for (int i = tid; i < 64 * 4; i += kFT) {                       // W0 [64 x 32] -> SW64
-    const int r = i >> 2, c = i & 3;
-    *reinterpret_cast<uint4*>(sm + S::W0 + sw64_off(r, c)) = *reinterpret_cast<const uint4*>(params + r * 32 + c * 8);
-  }
-  for (int i = tid; i < 16 * 8; i += kFT) {                       // Wout [16 x 64] -> SW128
-    const int r = i >> 3, c = i & 7;
-    *reinterpret_cast<uint4*>(sm + S::WO + sw128_off(r, c)) = *reinterpret_cast<const uint4*>(params + 64 * 32 + r * 64 + c * 8);
-  }
-  if (tid < F2B_N_LEVELS) s_scale[tid] = level_scale(tid);
+  stage_field(params, sm, s_scale, nullptr, tid);
   __syncthreads();
   const uint32_t a0 = smem_u32(sm + S::A0), a1 = smem_u32(sm + S::A1), s_do = smem_u32(sm + S::DO);
   const uint32_t w0 = smem_u32(sm + S::W0), wo = smem_u32(sm + S::WO);
@@ -513,11 +507,7 @@ ray_grad_kernel(const __half* __restrict__ table, const int* __restrict__ prim_p
     // ---- F0: H = relu(X . W0^T) ---------------------------------------------------------------------------------------------
     {
       Acc<64> acc;
-      wg_fence();
-      mma_m128<64, 0, 2>(acc, a0, 64, w0, 64, false);
-      wg_commit();
-      wg_wait();
-      acc_relu_to_tile(acc, sm + S::A1, tid);
+      field_layer0(acc, a0, w0, sm + S::A1, tid, [] {});
       fence_async_smem();
       __syncthreads();
       // ---- A: dH = dOut . Wout, masked by the fp16 hidden tile, over it in place ----------------------------------------------
@@ -646,10 +636,7 @@ static void field_launch(const void* table_f16, const int* prim_pool, const floa
                          const void* mlp_params_f16, const Src& src, int n_pts, float* out_f32, void* feat_save_f16,
                          void* hidden_save_f16, void* stream) {
   constexpr int MB = kFieldDefaultMinB;
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
-  const int n_tiles = div_up(n_pts, kFT);
-  const int grid = n_tiles < sms * MB ? n_tiles : sms * MB;
+  const int grid = persistent_grid(div_up(n_pts, kFT), MB);
   cudaFuncSetAttribute(field_fwd_kernel<LO, MB, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, FieldSmem::BYTES);
   field_fwd_kernel<LO, MB, Src><<<grid, kFT, FieldSmem::BYTES, as_stream(stream)>>>(
       (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)mlp_params_f16, src, n_pts, out_f32,
@@ -713,10 +700,7 @@ template <bool SLOTS, class Src>
 static void grad_launch(const void* trans, const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
                         int local_size, const void* mlp_params_f16, const Src& src, int n, float empty, float* logit, float* grad,
                         const float* w_slots, float* tile_partials, void* stream) {
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
-  const int n_tiles = div_up(n, kFT);
-  const int grid = n_tiles < sms * kFieldDefaultMinB ? n_tiles : sms * kFieldDefaultMinB;
+  const int grid = persistent_grid(div_up(n, kFT), kFieldDefaultMinB);
   cudaFuncSetAttribute(field_grad_kernel<SLOTS, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, GradSmem::BYTES);
   field_grad_kernel<SLOTS, Src><<<grid, kFT, GradSmem::BYTES, as_stream(stream)>>>(
       (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)mlp_params_f16, (const TransInfo*)trans,
@@ -769,10 +753,7 @@ extern "C" int f2b_ray_grad(const void* trans, const void* table_f16, const int*
                     t && dirs && anchors && row_work,
                 "f2b_ray_grad: null pointer");
     F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_ray_grad: bad n_volumes/local_size");
-    int sms = 132;
-    f2b_device_info(&sms, nullptr);
-    const int n_tiles = div_up(n_pts, kFT);
-    const int grid = n_tiles < sms * kRayGradMinB ? n_tiles : sms * kRayGradMinB;
+    const int grid = persistent_grid(div_up(n_pts, kFT), kRayGradMinB);
     cudaFuncSetAttribute(ray_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RayGradSmem::BYTES);
     ray_grad_kernel<<<grid, kFT, RayGradSmem::BYTES, as_stream(stream)>>>(
         (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16, (const TransInfo*)trans,

@@ -50,15 +50,6 @@ struct FusedSmem {
   static constexpr int BYTES = BAR + 16 + 16 + 64 + 1024;   // + alignment slack (the tiles need 1024-byte alignment)
 };
 
-template <int K>
-__device__ __forceinline__ void stage_w_fused(const __half* __restrict__ w, int rows, unsigned char* dst) {
-  constexpr int chunks = K / 8;
-  for (int i = threadIdx.x; i < rows * chunks; i += blockDim.x) {
-    const int r = i / chunks, c = i % chunks;
-    *reinterpret_cast<uint4*>(dst + (K == 64 ? sw128_off(r, c) : sw64_off(r, c))) = *reinterpret_cast<const uint4*>(w + r * K + c * 8);
-  }
-}
-
 __device__ __forceinline__ float h16(uint32_t acc_bits) { return __half2float(__float2half_rn(__uint_as_float(acc_bits))); }
 
 // barrier over the walker's 128 threads (named barrier 1; barrier 0 stays the CTA-wide one)
@@ -79,8 +70,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
                         int* __restrict__ ticket, float* __restrict__ colors, float* __restrict__ disparity,
                         float* __restrict__ depth, int* __restrict__ kept_counts, float* __restrict__ weights_slots) {
   using S = FusedSmem;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   const int tid = threadIdx.x;                                   // thread == sample
   unsigned char* wsm = sm + S::WALK0;
   int* s_ray = reinterpret_cast<int*>(sm + S::BAR);
@@ -90,11 +80,11 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   float* s_add = reinterpret_cast<float*>(wsm + S::ADD);         // [5][128] addends of the five per-ray sums
   float* s_rows = reinterpret_cast<float*>(wsm + S::ROWS);
 
-  stage_w_fused<32>(fparams, 64, sm + S::FW0);
-  stage_w_fused<64>(fparams + 64 * 32, 16, sm + S::FWO);
-  stage_w_fused<32>(sparams, 64, sm + S::SW0);
-  stage_w_fused<64>(sparams + 64 * 32, 64, sm + S::SWH);
-  stage_w_fused<64>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO);
+  stage_weights<32, 0>(fparams, 64, sm + S::FW0, tid);
+  stage_weights<64, 0>(fparams + 64 * 32, 16, sm + S::FWO, tid);
+  stage_weights<32, 0>(sparams, 64, sm + S::SW0, tid);
+  stage_weights<64, 0>(sparams + 64 * 32, 64, sm + S::SWH, tid);
+  stage_weights<64, 0>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO, tid);
   if (threadIdx.x < F2B_N_LEVELS) s_scale[threadIdx.x] = level_scale(threadIdx.x);
   fence_async_smem();
   __syncthreads();
@@ -277,12 +267,9 @@ extern "C" int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool,
               "f2b_render_fwd_fused: null pointer");
   F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_render_fwd_fused: bad n_volumes/local_size");
   F2B_REQUIRE(slot_size > 0 && int64_t(n_rays) * slot_size < (int64_t(1) << 31), "f2b_render_fwd_fused: n_rays * slot_size overflows int32");
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
   if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("f2b_render_fwd_fused: memset failed"); return F2B_ECUDA; }
   cudaFuncSetAttribute(render_fwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem::BYTES);
-  const int per_sm = resident_per_sm(render_fwd_fused_kernel, kRT, FusedSmem::BYTES);
-  const int grid = n_rays < sms * per_sm ? n_rays : sms * per_sm;
+  const int grid = persistent_grid(n_rays, resident_per_sm(render_fwd_fused_kernel, kRT, FusedSmem::BYTES));
   render_fwd_fused_kernel<<<grid, kRT, FusedSmem::BYTES, as_stream(stream)>>>(
       (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,
       (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,

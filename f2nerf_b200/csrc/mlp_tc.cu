@@ -40,30 +40,6 @@ struct TcSmem {                         // offsets from a 1024-byte aligned base
   static constexpr int BYTES = WO + 2048 + 1024;  // + alignment slack
 };
 
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
-
-// weights [rows x K] fp16 row-major (global) -> swizzled K-major tile in shared memory
-template <int K>
-__device__ __forceinline__ void stage_weights(const __half* __restrict__ w, int rows, unsigned char* dst) {
-  constexpr int chunks = K / 8;                                  // 16-byte chunks per row
-  for (int i = threadIdx.x; i < rows * chunks; i += blockDim.x) {
-    const int r = i / chunks, c = i % chunks;
-    const uint4 v = *reinterpret_cast<const uint4*>(w + r * K + c * 8);
-    *reinterpret_cast<uint4*>(dst + (K == 64 ? sw128_off(r, c) : sw64_off(r, c))) = v;
-  }
-}
-
-// 16-byte asynchronous global -> shared copy (LDGSTS); src_bytes == 0 zero-fills the destination
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // Input tile (128 rows x 64 B, contiguous in global memory) -> swizzled K-major tile, fully coalesced:
 // the CTA's 128 threads sweep the 8 KB linearly, 16 B per thread and pass.
 __device__ __forceinline__ void prefetch_input(const __half* __restrict__ in, int tile, int n_pts, uint32_t a0_tile) {
@@ -72,7 +48,7 @@ __device__ __forceinline__ void prefetch_input(const __half* __restrict__ in, in
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     const int c = threadIdx.x + kTcTile * j, r = c >> 2;
-    cp_async16(a0_tile + sw64_off(r, c & 3), src + (r < rows ? size_t(c) * 16 : 0), r < rows ? 16u : 0u);
+    cp_async<16>(a0_tile + sw64_off(r, c & 3), src + (r < rows ? size_t(c) * 16 : 0), r < rows ? 16u : 0u);
   }
 }
 
@@ -108,8 +84,7 @@ __global__ void __launch_bounds__(kTcTile)
 mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ params, int n_pts,
                   __half* __restrict__ out, float* __restrict__ out_f32, __half* __restrict__ hidden_save, EpiArgs epi) {
   using S = TcSmem<NH>;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   float* s_rows = reinterpret_cast<float*>(sm + S::H0);             // output rows [128][20] fp32 (H0 is dead by then)
   const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kTcTile - 1) / kTcTile;
@@ -118,9 +93,9 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
   int tile = blockIdx.x;
   if (tile < n_tiles) prefetch_input(in, tile, n_pts, a0);       // overlaps the weight staging
   cp_async_commit();
-  stage_weights<32>(params, 64, sm + S::W0);
-  if (NH) stage_weights<64>(params + 64 * 32, 64, sm + S::WH);
-  stage_weights<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
+  stage_weights<32, 0>(params, 64, sm + S::W0, tid);
+  if (NH) stage_weights<64, 0>(params + 64 * 32, 64, sm + S::WH, tid);
+  stage_weights<64, 0>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO, tid);
 
   const uint32_t h0 = smem_u32(sm + S::H0), h1 = smem_u32(sm + S::H1);
   const uint32_t w0 = smem_u32(sm + S::W0), wh = smem_u32(sm + S::WH), wo = smem_u32(sm + S::WO);
@@ -171,10 +146,10 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
       row_ld16(s_rows, kRowLd16, tid, r);
       if (valid) {
         uint4 v0, v1;
-        v0.x = pack_half2(__uint_as_float(r[0]), __uint_as_float(r[1]));   v0.y = pack_half2(__uint_as_float(r[2]), __uint_as_float(r[3]));
-        v0.z = pack_half2(__uint_as_float(r[4]), __uint_as_float(r[5]));   v0.w = pack_half2(__uint_as_float(r[6]), __uint_as_float(r[7]));
-        v1.x = pack_half2(__uint_as_float(r[8]), __uint_as_float(r[9]));   v1.y = pack_half2(__uint_as_float(r[10]), __uint_as_float(r[11]));
-        v1.z = pack_half2(__uint_as_float(r[12]), __uint_as_float(r[13])); v1.w = pack_half2(__uint_as_float(r[14]), __uint_as_float(r[15]));
+        v0.x = pk(__uint_as_float(r[0]), __uint_as_float(r[1]));   v0.y = pk(__uint_as_float(r[2]), __uint_as_float(r[3]));
+        v0.z = pk(__uint_as_float(r[4]), __uint_as_float(r[5]));   v0.w = pk(__uint_as_float(r[6]), __uint_as_float(r[7]));
+        v1.x = pk(__uint_as_float(r[8]), __uint_as_float(r[9]));   v1.y = pk(__uint_as_float(r[10]), __uint_as_float(r[11]));
+        v1.z = pk(__uint_as_float(r[12]), __uint_as_float(r[13])); v1.w = pk(__uint_as_float(r[14]), __uint_as_float(r[15]));
         if (out) {
           uint4* dst = reinterpret_cast<uint4*>(out + size_t(p) * 16);
           dst[0] = v0; dst[1] = v1;
@@ -202,10 +177,10 @@ mlp_fwd_tc_kernel(const __half* __restrict__ in, const __half* __restrict__ para
         uint4 row[4] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
         if (valid) {
           uint4 v0, v1;
-          v0.x = pack_half2(__uint_as_float(r[0]), __uint_as_float(r[1]));   v0.y = pack_half2(__uint_as_float(r[2]), __uint_as_float(r[3]));
-          v0.z = pack_half2(__uint_as_float(r[4]), __uint_as_float(r[5]));   v0.w = pack_half2(__uint_as_float(r[6]), __uint_as_float(r[7]));
-          v1.x = pack_half2(__uint_as_float(r[8]), __uint_as_float(r[9]));   v1.y = pack_half2(__uint_as_float(r[10]), __uint_as_float(r[11]));
-          v1.z = pack_half2(__uint_as_float(r[12]), __uint_as_float(r[13])); v1.w = pack_half2(__uint_as_float(r[14]), __uint_as_float(r[15]));
+          v0.x = pk(__uint_as_float(r[0]), __uint_as_float(r[1]));   v0.y = pk(__uint_as_float(r[2]), __uint_as_float(r[3]));
+          v0.z = pk(__uint_as_float(r[4]), __uint_as_float(r[5]));   v0.w = pk(__uint_as_float(r[6]), __uint_as_float(r[7]));
+          v1.x = pk(__uint_as_float(r[8]), __uint_as_float(r[9]));   v1.y = pk(__uint_as_float(r[10]), __uint_as_float(r[11]));
+          v1.z = pk(__uint_as_float(r[12]), __uint_as_float(r[13])); v1.w = pk(__uint_as_float(r[14]), __uint_as_float(r[15]));
           float feat[16];
           const __half2* h = reinterpret_cast<const __half2*>(&v0);
           const __half2* g = reinterpret_cast<const __half2*>(&v1);
@@ -243,12 +218,8 @@ using namespace f2b;
 template <int NH, int EPI>
 static void launch_fwd(const void* in_f16, const void* params_f16, int n_pts, void* out_f16, float* out_f32,
                        void* hidden_save_f16, const EpiArgs& epi, void* stream) {
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
   cudaFuncSetAttribute(mlp_fwd_tc_kernel<NH, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<NH>::BYTES);
-  const int per_sm = resident_per_sm(mlp_fwd_tc_kernel<NH, EPI>, kTcTile, TcSmem<NH>::BYTES);
-  const int n_tiles = div_up(n_pts, kTcTile);
-  const int grid = n_tiles < sms * per_sm ? n_tiles : sms * per_sm;
+  const int grid = persistent_grid(div_up(n_pts, kTcTile), resident_per_sm(mlp_fwd_tc_kernel<NH, EPI>, kTcTile, TcSmem<NH>::BYTES));
   mlp_fwd_tc_kernel<NH, EPI><<<grid, kTcTile, TcSmem<NH>::BYTES, as_stream(stream)>>>(
       (const __half*)in_f16, (const __half*)params_f16, n_pts, (__half*)out_f16, out_f32, (__half*)hidden_save_f16, epi);
 }

@@ -36,19 +36,6 @@ struct BwdSmem {
   static constexpr int BYTES = STAGE0 + 2 * STAGE_BYTES + 1024;
 };
 
-template <int K>
-__device__ __forceinline__ void stage_w(const __half* __restrict__ w, int rows, unsigned char* dst) {
-  constexpr int chunks = K / 8;
-  for (int i = threadIdx.x; i < rows * chunks; i += blockDim.x) {
-    const int r = i / chunks, c = i % chunks;
-    *reinterpret_cast<uint4*>(dst + (K == 64 ? sw128_off(r, c) : sw64_off(r, c))) = *reinterpret_cast<const uint4*>(w + r * K + c * 8);
-  }
-}
-
-__device__ __forceinline__ void cp16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-
 // One tile's operand rows (dOut 32 B, x 64 B, h0 128 B, h1 128 B per sample; each a contiguous block in global
 // memory) -> swizzled tiles of one stage, 16 B per thread and pass, linear sweep = full 128 B lines.
 template <int NH>
@@ -66,20 +53,20 @@ __device__ __forceinline__ void prefetch_tile(const __half* __restrict__ dout, c
   for (int j = 0; j < 2; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 1;
     const bool ok = r < rows;
-    cp16(stage + S::DO + sw32_off(r, c & 1), s_do + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::DO + sw32_off(r, c & 1), s_do + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 2;
     const bool ok = r < rows;
-    cp16(stage + S::X + sw64_off(r, c & 3), s_x + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::X + sw64_off(r, c & 3), s_x + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
 #pragma unroll
   for (int j = 0; j < 8; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 3;
     const bool ok = r < rows;
-    cp16(stage + S::H0 + sw128_off(r, c & 7), s_h0 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
-    if (NH) cp16(stage + S::H1 + sw128_off(r, c & 7), s_h1 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::H0 + sw128_off(r, c & 7), s_h0 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    if (NH) cp_async<16>(stage + S::H1 + sw128_off(r, c & 7), s_h1 + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
 }
 
@@ -122,18 +109,17 @@ mlp_bwd_tc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
                   const __half* __restrict__ hid_last, const __half* __restrict__ params, int n_pts,
                   __half* __restrict__ din, float* __restrict__ dparams) {
   using S = BwdSmem<NH>;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kBT - 1) / kBT;
   const uint32_t stage0 = smem_u32(sm + S::STAGE0);
 
   int tile = blockIdx.x;
   if (tile < n_tiles) prefetch_tile<NH>(dout, in, hidden, hid_last, tile, n_pts, stage0);
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  stage_w<32>(params, 64, sm + S::W0);
-  if (NH) stage_w<64>(params + 64 * 32, 64, sm + S::WH);
-  stage_w<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
+  cp_async_commit();
+  stage_weights<32, 0>(params, 64, sm + S::W0, threadIdx.x);
+  if (NH) stage_weights<64, 0>(params + 64 * 32, 64, sm + S::WH, threadIdx.x);
+  stage_weights<64, 0>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO, threadIdx.x);
   const uint32_t s_w0 = smem_u32(sm + S::W0), s_wh = smem_u32(sm + S::WH), s_wo = smem_u32(sm + S::WO);
   Acc<64> act;
   Acc<32> act_in;
@@ -148,8 +134,8 @@ mlp_bwd_tc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
     __syncthreads();                                             // every warp's MMAs are done with the stage refilled below
     const int next = tile + gridDim.x;
     if (next < n_tiles) prefetch_tile<NH>(dout, in, hidden, hid_last, next, n_pts, stage0 + (buf ^ 1) * S::STAGE_BYTES);
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
+    cp_async_commit();
+    cp_async_wait<1>();                                          // this tile's operands have landed
     fence_async_smem();
     __syncthreads();
     unsigned char* const st = sm + S::STAGE0 + buf * S::STAGE_BYTES;
@@ -186,7 +172,7 @@ mlp_bwd_tc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
     wg_wait();
     if (din) store_din(act_in, din, tile, n_pts, tid);
   }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  cp_async_wait<0>();
   if (any) flush_weight_grads<NH>(gw0, gwo, gwh, dparams, tid);
 }
 
@@ -233,13 +219,13 @@ __device__ __forceinline__ void prefetch_tile_rc(const __half* __restrict__ dout
   for (int j = 0; j < 2; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 1;
     const bool ok = r < rows;
-    cp16(stage + S::DO + sw32_off(r, c & 1), s_do + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::DO + sw32_off(r, c & 1), s_do + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 2;
     const bool ok = r < rows;
-    cp16(stage + S::X + sw64_off(r, c & 3), s_x + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::X + sw64_off(r, c & 3), s_x + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
 }
 
@@ -248,18 +234,17 @@ __global__ void __launch_bounds__(kBT)
 mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in, const __half* __restrict__ params, int n_pts,
                   __half* __restrict__ din, float* __restrict__ dparams) {
   using S = RcSmem<NH>;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   const int tid = threadIdx.x;
   const int n_tiles = (n_pts + kBT - 1) / kBT;
   const uint32_t stage0 = smem_u32(sm + S::STAGE0);
 
   int tile = blockIdx.x;
   if (tile < n_tiles) prefetch_tile_rc<NH>(dout, in, tile, n_pts, stage0);
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  stage_w<32>(params, 64, sm + S::W0);
-  if (NH) stage_w<64>(params + 64 * 32, 64, sm + S::WH);
-  stage_w<64>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO);
+  cp_async_commit();
+  stage_weights<32, 0>(params, 64, sm + S::W0, threadIdx.x);
+  if (NH) stage_weights<64, 0>(params + 64 * 32, 64, sm + S::WH, threadIdx.x);
+  stage_weights<64, 0>(params + 64 * 32 + NH * 64 * 64, 16, sm + S::WO, threadIdx.x);
   const uint32_t s_w0 = smem_u32(sm + S::W0), s_wh = smem_u32(sm + S::WH), s_wo = smem_u32(sm + S::WO);
   const uint32_t s_h0 = smem_u32(sm + S::H0), s_h1 = smem_u32(sm + S::H1), s_d1 = smem_u32(sm + S::D1);
   Acc<64> act;
@@ -275,8 +260,8 @@ mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
     __syncthreads();                                             // every warp's MMAs are done with the stage refilled below
     const int next = tile + gridDim.x;
     if (next < n_tiles) prefetch_tile_rc<NH>(dout, in, next, n_pts, stage0 + (buf ^ 1) * S::STAGE_BYTES);
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
+    cp_async_commit();
+    cp_async_wait<1>();                                          // this tile's operands have landed
     fence_async_smem();
     __syncthreads();                                             // (also: the previous tile's MMAs are done with H0 / H1 / D1)
     const uint32_t sb = stage0 + buf * S::STAGE_BYTES;
@@ -332,7 +317,7 @@ mlp_bwd_rc_kernel(const __half* __restrict__ dout, const __half* __restrict__ in
     wg_wait();
     if (din) store_din(act_in, din, tile, n_pts, tid);
   }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  cp_async_wait<0>();
   if (any) flush_weight_grads<NH>(gw0, gwo, gwh, dparams, tid);
 }
 
@@ -362,10 +347,6 @@ struct FbsSmem {
   static constexpr int BYTES = STAGE0 + 2 * STAGE_BYTES + 1024;
 };
 
-__device__ __forceinline__ void cp4(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-
 // the tile's points (3 fp32 per row, contiguous) to s_pts and volume ids (vol[i * vol_stride]) to s_vol; rows past n_pts are zero-filled
 __device__ __forceinline__ void prefetch_pts_vol(const float* __restrict__ pts, const int* __restrict__ vol, int vol_stride, int tile,
                                                  int n_pts, uint32_t s_pts, uint32_t s_vol) {
@@ -375,10 +356,10 @@ __device__ __forceinline__ void prefetch_pts_vol(const float* __restrict__ pts, 
   for (int j = 0; j < 3; j++) {
     const int c = threadIdx.x + kBT * j;
     const bool ok = c < rows * 3;
-    cp4(s_pts + 4 * c, pts + t0 * 3 + (ok ? c : 0), ok ? 4u : 0u);
+    cp_async<4>(s_pts + 4 * c, pts + t0 * 3 + (ok ? c : 0), ok ? 4u : 0u);
   }
   const bool ok = int(threadIdx.x) < rows;
-  cp4(s_vol + 4 * threadIdx.x, vol + (t0 + (ok ? threadIdx.x : 0)) * vol_stride, ok ? 4u : 0u);
+  cp_async<4>(s_vol + 4 * threadIdx.x, vol + (t0 + (ok ? threadIdx.x : 0)) * vol_stride, ok ? 4u : 0u);
 }
 
 // byte offset of fp16 column `col` of row `r` in the DIN tile.  The 80 B row pitch makes the accumulator stores conflict-free and
@@ -407,8 +388,7 @@ field_bwd_scatter_kernel(const __half* __restrict__ dout, const __half* __restri
                          const float* __restrict__ bias_pool, int n_volumes, int local_size, float grad_mul,
                          float* __restrict__ dparams, float* __restrict__ grad_table, __half* __restrict__ din) {
   using S = FbsSmem;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tiles = (n_pts + kBT - 1) / kBT;
   const uint32_t stage0 = smem_u32(sm + S::STAGE0);
@@ -418,9 +398,9 @@ field_bwd_scatter_kernel(const __half* __restrict__ dout, const __half* __restri
     prefetch_tile_rc<0>(dout, in, tile, n_pts, stage0);
     prefetch_pts_vol(pts, vol, vol_stride, tile, n_pts, stage0 + S::PTS, stage0 + S::VOL);
   }
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  stage_w<32>(params, 64, sm + S::W0);
-  stage_w<64>(params + 64 * 32, 16, sm + S::WO);
+  cp_async_commit();
+  stage_weights<32, 0>(params, 64, sm + S::W0, threadIdx.x);
+  stage_weights<64, 0>(params + 64 * 32, 16, sm + S::WO, threadIdx.x);
   const uint32_t s_w0 = smem_u32(sm + S::W0), s_wo = smem_u32(sm + S::WO), s_h0 = smem_u32(sm + S::H0);
   unsigned char* const s_din = sm + S::DIN;
   Acc<64> act;
@@ -439,8 +419,8 @@ field_bwd_scatter_kernel(const __half* __restrict__ dout, const __half* __restri
       prefetch_tile_rc<0>(dout, in, next, n_pts, nb);
       prefetch_pts_vol(pts, vol, vol_stride, next, n_pts, nb + S::PTS, nb + S::VOL);
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
+    cp_async_commit();
+    cp_async_wait<1>();                                          // this tile's operands have landed
     fence_async_smem();
     __syncthreads();                                             // (also: the previous tile's MMAs and scatter are done with H0 / DIN)
     const unsigned char* const st = sm + S::STAGE0 + buf * S::STAGE_BYTES;
@@ -483,7 +463,7 @@ field_bwd_scatter_kernel(const __half* __restrict__ dout, const __half* __restri
       scatter_row(s_din, st + S::PTS, st + S::VOL, r, lane, tile * kBT + r < n_pts, prim_pool, bias_pool, n_volumes, local_size,
                   grad_mul, grad_table);
   }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  cp_async_wait<0>();
   if (int(blockIdx.x) < n_tiles) flush_weight_grads<0>(gw0, gwo, gwh, dparams, tid);
 }
 
@@ -558,11 +538,11 @@ __device__ __forceinline__ void prefetch_tile_sfb(const __half* __restrict__ d_r
   for (int j = 0; j < 4; j++) {
     const int c = threadIdx.x + kBT * j, r = c >> 2;
     const bool ok = r < rows;
-    cp16(stage + S::FX + sw64_off(r, c & 3), s_fx + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
+    cp_async<16>(stage + S::FX + sw64_off(r, c & 3), s_fx + (ok ? size_t(c) * 16 : 0), ok ? 16u : 0u);
   }
   prefetch_pts_vol(pts, vol, vol_stride, tile, n_pts, stage + S::PTS, stage + S::VOL);
   const bool ok = int(threadIdx.x) < rows;
-  cp4(stage + S::DLOG + 4 * threadIdx.x, d_logit + t0 + (ok ? threadIdx.x : 0), ok ? 4u : 0u);
+  cp_async<4>(stage + S::DLOG + 4 * threadIdx.x, d_logit + t0 + (ok ? threadIdx.x : 0), ok ? 4u : 0u);
 }
 
 // warp-collective: d_app[e] += sum of the warp's rows with embedding index e, per run of equal e (a camera index is constant along a
@@ -599,15 +579,14 @@ shade_field_bwd_scatter_kernel(const __half* __restrict__ d_raw, const __half* _
                                float* __restrict__ grad_table, float* __restrict__ d_app, int* __restrict__ ticket,
                                __half* __restrict__ d_in16, __half* __restrict__ d_scene16, __half* __restrict__ dfeat16) {
   using S = SfbSmem;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* sm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned char* sm = smem_base();
   int* s_tk = reinterpret_cast<int*>(sm + S::TICKET);                 // read after barriers only ("memory" clobbers)
   if (threadIdx.x == 0) s_tk[0] = atomicAdd(ticket, 1);
-  stage_w<32>(sparams, 64, sm + S::SW0);
-  stage_w<64>(sparams + 64 * 32, 64, sm + S::SWH);
-  stage_w<64>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO);
-  stage_w<32>(fparams, 64, sm + S::FW0);
-  stage_w<64>(fparams + 64 * 32, 16, sm + S::FWO);
+  stage_weights<32, 0>(sparams, 64, sm + S::SW0, threadIdx.x);
+  stage_weights<64, 0>(sparams + 64 * 32, 64, sm + S::SWH, threadIdx.x);
+  stage_weights<64, 0>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO, threadIdx.x);
+  stage_weights<32, 0>(fparams, 64, sm + S::FW0, threadIdx.x);
+  stage_weights<64, 0>(fparams + 64 * 32, 16, sm + S::FWO, threadIdx.x);
   __syncthreads();
 
   if (threadIdx.x >= kBT) {
@@ -657,7 +636,7 @@ shade_field_bwd_scatter_kernel(const __half* __restrict__ d_raw, const __half* _
   const uint32_t s_h0 = smem_u32(sm + S::H0), s_h1 = smem_u32(sm + S::H1), s_d1 = smem_u32(sm + S::D1), s_fdo = smem_u32(sm + S::FDO);
   int tile = s_tk[0];
   if (tile < n_tiles) prefetch_tile_sfb(d_raw, mlp_in, feat, d_logit, pts, vol, vol_stride, tile, n_pts, stage0);
-  asm volatile("cp.async.commit_group;" ::: "memory");
+  cp_async_commit();
   Acc<64> act;
   Acc<32> act_in;
   Acc64<32> sgw0, fgw0;
@@ -672,8 +651,8 @@ shade_field_bwd_scatter_kernel(const __half* __restrict__ d_raw, const __half* _
     bar_sync(kBarMma, kBT);                                      // every warp's MMAs are done with the stage refilled below
     const int next = s_tk[b ^ 1];
     if (next < n_tiles) prefetch_tile_sfb(d_raw, mlp_in, feat, d_logit, pts, vol, vol_stride, next, n_pts, stage0 + (b ^ 1) * S::STAGE_BYTES);
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 1;" ::: "memory");         // this tile's operands have landed
+    cp_async_commit();
+    cp_async_wait<1>();                                          // this tile's operands have landed
     fence_async_smem();
     bar_sync(kBarMma, kBT);
     const unsigned char* const st = sm + S::STAGE0 + b * S::STAGE_BYTES;
@@ -786,7 +765,7 @@ shade_field_bwd_scatter_kernel(const __half* __restrict__ d_raw, const __half* _
     if (tid == 0) *reinterpret_cast<int*>(slot + S::R_TILE) = -1;
     bar_arrive(kBarFull + (k & 1), 2 * kBT);
   }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  cp_async_wait<0>();
   if (any) {
     flush_weight_grads<1>(sgw0, sgwo, sgwh, d_sparams, tid);
     flush_weight_grads<0>(fgw0, fgwo, sgwh, d_fparams, tid);
@@ -806,13 +785,11 @@ extern "C" int f2b_field_bwd_scatter(const void* dout_f16, const void* feat_f16,
               "f2b_field_bwd_scatter: null pointer");
   F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0 && vol_stride > 0,
               "f2b_field_bwd_scatter: bad n_volumes/local_size/vol_stride");
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
   constexpr int bytes = FbsSmem::BYTES;
   cudaFuncSetAttribute(field_bwd_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  const int n_tiles = div_up(n_pts, kBT);
-  const int cap = sms * resident_per_sm(field_bwd_scatter_kernel, kBT, bytes);   // persistent: weight gradients flushed once per CTA
-  field_bwd_scatter_kernel<<<n_tiles < cap ? n_tiles : cap, kBT, bytes, as_stream(stream)>>>(
+  // persistent: weight gradients flushed once per CTA
+  const int grid = persistent_grid(div_up(n_pts, kBT), resident_per_sm(field_bwd_scatter_kernel, kBT, bytes));
+  field_bwd_scatter_kernel<<<grid, kBT, bytes, as_stream(stream)>>>(
       (const __half*)dout_f16, (const __half*)feat_f16, (const __half*)params_f16, n_pts, pts, vol, vol_stride, prim_pool, bias_pool,
       n_volumes, local_size, grad_mul, dparams_f32, grad_table_f32, (__half*)din_f16);
   return check_launch("f2b_field_bwd_scatter");
@@ -835,12 +812,9 @@ extern "C" int f2b_shade_field_bwd_scatter(const void* d_raw_f16, const void* ml
     set_error("f2b_shade_field_bwd_scatter: memset failed");
     return F2B_ECUDA;
   }
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
   constexpr int bytes = SfbSmem::BYTES;
   cudaFuncSetAttribute(shade_field_bwd_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  const int n_tiles = div_up(n_pts, kBT);
-  shade_field_bwd_scatter_kernel<<<n_tiles < sms ? n_tiles : sms, kSfbThreads, bytes, as_stream(stream)>>>(
+  shade_field_bwd_scatter_kernel<<<persistent_grid(div_up(n_pts, kBT), 1), kSfbThreads, bytes, as_stream(stream)>>>(
       (const __half*)d_raw_f16, (const __half*)mlp_in_f16, (const __half*)sparams_f16, d_logit, pt_emb_idx, inv_loss_scale,
       field_loss_scale, (const __half*)feat_f16, (const __half*)fparams_f16, n_pts, pts, vol, vol_stride, prim_pool, bias_pool, n_volumes,
       local_size, grad_mul, d_sparams_f32, d_fparams_f32, grad_table_f32, d_app_emb, ticket, (__half*)d_in16, (__half*)d_scene16,
@@ -854,15 +828,13 @@ extern "C" int f2b_mlp_bwd2(const void* dout_f16, const void* in_f16, const void
   if (n_pts <= 0) return F2B_OK;
   F2B_REQUIRE(dout_f16 && in_f16 && params_f16 && dparams_f32, "f2b_mlp_bwd: null pointer");
   F2B_REQUIRE(n_hidden_matmuls == 0 || n_hidden_matmuls == 1, "f2b_mlp_bwd: n_hidden_matmuls must be 0 or 1");
-  int sms = 132;
-  f2b_device_info(&sms, nullptr);
   const int n_tiles = div_up(n_pts, kBT);
   // persistent grid: as many CTAs as are resident at once (each flushes its weight gradients once)
-#define F2B_BWD_LAUNCH(KERNEL, BYTES, ...)                                                          \
-  {                                                                                                 \
-    cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);               \
-    const int cap = sms * resident_per_sm(KERNEL, kBT, BYTES);                                      \
-    KERNEL<<<n_tiles < cap ? n_tiles : cap, kBT, BYTES, as_stream(stream)>>>(__VA_ARGS__);          \
+#define F2B_BWD_LAUNCH(KERNEL, BYTES, ...)                                                        \
+  {                                                                                               \
+    cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);             \
+    const int grid = persistent_grid(n_tiles, resident_per_sm(KERNEL, kBT, BYTES));               \
+    KERNEL<<<grid, kBT, BYTES, as_stream(stream)>>>(__VA_ARGS__);                                 \
   }
   if (!hidden0_f16) {                                             // no saved activations: rebuild them on the tensor pipe
     if (n_hidden_matmuls == 0)

@@ -49,6 +49,40 @@ __device__ __forceinline__ uint32_t sw128_col(int r, int col) { return sw128_off
 // generic-proxy smem writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// the dynamic shared memory from its first 1024-byte boundary, where the swizzled tiles start (launches add 1024 B of slack)
+__device__ __forceinline__ unsigned char* smem_base() {
+  extern __shared__ unsigned char smem_raw[];
+  return reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
+
+// weights [rows x K] fp16 row-major (global) -> swizzled K-major tile in shared memory (K = 32: SW64, K = 64: SW128), by threads
+// t, t + NT, t + 2 NT, ... of the CTA (NT = 0: blockDim.x, read where the loop steps)
+template <int K, int NT>
+__device__ __forceinline__ void stage_weights(const __half* __restrict__ w, int rows, unsigned char* dst, int t) {
+  constexpr int chunks = K / 8;                                  // 16-byte chunks per row
+  for (int i = t; i < rows * chunks;) {
+    const int r = i / chunks, c = i % chunks;
+    *reinterpret_cast<uint4*>(dst + (K == 64 ? sw128_off(r, c) : sw64_off(r, c))) = *reinterpret_cast<const uint4*>(w + r * K + c * 8);
+    if constexpr (NT > 0) i += NT;
+    else i += blockDim.x;
+  }
+}
+
+// ---- cp.async -------------------------------------------------------------------------------------
+// asynchronous global -> shared copy (LDGSTS) of N = 16 bytes (L2 only) or 4 bytes; src_bytes == 0 zero-fills the destination
+template <int N>
+__device__ __forceinline__ void cp_async(uint32_t dst, const void* src, uint32_t src_bytes) {
+  static_assert(N == 16 || N == 4, "cp.async of 16 or 4 bytes");
+  if constexpr (N == 16)
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+  else
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 // ---- wgmma ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

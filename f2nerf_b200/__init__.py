@@ -9,7 +9,7 @@ from . import _lib  # noqa: F401  (fails loudly when the CUDA extension is missi
 from .checkpoint import Scene, gradient_scaling_progress, load_scene, load_states
 from .dataset import RayGenerator, load_dataset
 from .octree_build import build_edge_pool, build_tree_nodes, initial_octree
-from .eval import ImageMetrics, RenderAllImages, RenderNormals, RenderPath, RenderWholeImage, TestImages
+from .eval import ImageMetrics, RenderAllImages, RenderDepth, RenderNormals, RenderPath, RenderWholeImage, TestImages
 from .field import Hash3DAnchored, TCNNWP
 from .ops import CustomOps, FlexOps
 from .optim import FusedAdam
@@ -19,5 +19,5 @@ from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultF
 from .shader import SHShader
 
 __all__ = ["FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
-           "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
+           "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderDepth", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

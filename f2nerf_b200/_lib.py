@@ -59,6 +59,8 @@ SIGNATURES = {
     "f2b_warp_jacobian_points": [_P, c_int, _P, _P, c_int, _P, _P],
     "f2b_query_grad_points": [_P, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_float, _P, _P, _P],
     "f2b_render_normals_slots": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
+    "f2b_ray_termination_slots": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P],
+    "f2b_depth_consistency": [_P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_float, c_float, _P, _P, _P],
     "f2b_ray_grad": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, c_float, _P, _P, _P,
                      _P, _P, _P, _P],
     "f2b_iso_count": [_P, c_int, c_int, c_int, c_float, c_float, c_int, c_int, _P, _P, _P, _P],

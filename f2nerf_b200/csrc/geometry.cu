@@ -1,5 +1,6 @@
 // geometry.cu — a trained scene's geometry on the device: point location through the perspective-warp octree and
-// isosurface extraction from a logit lattice by marching tetrahedra (DESIGN.md §3i).  The field query itself is the
+// isosurface extraction from a logit lattice by marching tetrahedra (DESIGN.md §3i); the opacity and median depth of rendered
+// rays and the depth-consistency test of points against a view (DESIGN.md §3l).  The field query itself is the
 // fused encode + MLP kernel of field.cu with a located-point source (f2b_query_logit_points / _grid).
 //
 // Isosurface.  The lattice is nx x ny x nz logits (x fastest); lattice points outside it read empty_logit (a virtual pad
@@ -15,6 +16,7 @@
 // tetrahedron, triangle), each triangle oriented outward (towards the lower logit).  Work goes in z-slabs of cells
 // [ez0, ez1): the counts cover owner layers [ez0, min(ez1 + 1, nz + 1)) (the extra layer numbers the vertices the slab's
 // top cells share with the next slab), so the per-slab scratch is 13 B per owner point and 12 B per cell of the slab.
+#include "camera.cuh"
 #include "common.cuh"
 #include "locate.cuh"
 
@@ -178,9 +180,138 @@ __global__ void iso_emit_kernel(Lattice L, float level, float ox, float oy, floa
   }
 }
 
+// ---- depth of a view and depth consistency (DESIGN §3l) ------------------------------------------------------------
+// One warp per ray.  Lanes load 32 consecutive kept weights (coalesced); the running sum is chained through the lanes in slot
+// order, one fadd per sample starting from +0, so W is the serial left-to-right fp32 sum (lanes past the kept prefix add +0,
+// which leaves the sum unchanged).  The running sum at the end of every 32-slot chunk goes to shared memory; the median is then
+// found without a second pass over the ray: a ballot over the chunk ends picks the first chunk that reaches 0.5 W, and one
+// more chain over that chunk, started from the previous chunk's end, gives the same partial sums bit for bit.
+constexpr int kTermWarps = 8;
+
+__global__ void __launch_bounds__(kTermWarps * 32)
+ray_termination_kernel(const float* __restrict__ slot_t, const int* __restrict__ kept, const float* __restrict__ w_slots,
+                       const float* __restrict__ rays_o, const float* __restrict__ rays_d, int n_rays, int slot_size,
+                       float* __restrict__ opacity, float* __restrict__ median_t, float* __restrict__ point) {
+  extern __shared__ float s_ends[];                               // [kTermWarps][chunks] running sum at each chunk's end
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int ray = blockIdx.x * kTermWarps + warp;
+  if (ray >= n_rays) return;
+  const int chunks = (slot_size + 31) >> 5;
+  float* ends = s_ends + warp * chunks;
+  const int k = __ldg(kept + ray);
+  const float* w = w_slots + size_t(ray) * slot_size;
+  float run = 0.f;
+  for (int base = 0; base < k; base += 32) {
+    const float v = base + lane < k ? __ldg(w + base + lane) : 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; j++) run = fadd(run, __shfl_sync(0xffffffffu, v, j));
+    if (lane == 0) ends[base >> 5] = run;
+  }
+  __syncwarp();
+  const float W = run;
+  float tm = 0.f, px = 0.f, py = 0.f, pz = 0.f;
+  if (W > 0.f) {
+    const float half = fmul(.5f, W);
+    const int n_chunks = (k + 31) >> 5;
+    int c = -1;
+    for (int g = 0; g < n_chunks && c < 0; g += 32) {
+      const unsigned hit = __ballot_sync(0xffffffffu, g + lane < n_chunks && ends[g + lane] >= half);
+      if (hit) c = g + __ffs(hit) - 1;
+    }
+    const int base = c << 5;
+    const float v = base + lane < k ? __ldg(w + base + lane) : 0.f;
+    float r = c > 0 ? ends[c - 1] : 0.f, mine = 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; j++) {
+      r = fadd(r, __shfl_sync(0xffffffffu, v, j));
+      if (lane == j) mine = r;                                   // the running sum through my sample
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, base + lane < k && mine >= half);
+    const int m = base + __ffs(hit) - 1;
+    tm = __ldg(slot_t + size_t(ray) * slot_size + m);
+    px = ffma(tm, __ldg(rays_d + ray * 3), __ldg(rays_o + ray * 3));
+    py = ffma(tm, __ldg(rays_d + ray * 3 + 1), __ldg(rays_o + ray * 3 + 1));
+    pz = ffma(tm, __ldg(rays_d + ray * 3 + 2), __ldg(rays_o + ray * 3 + 2));
+  }
+  if (lane == 0) {
+    opacity[ray] = W > 0.f ? W : 0.f;
+    median_t[ray] = tm;
+    if (point) { point[ray * 3] = px; point[ray * 3 + 1] = py; point[ray * 3 + 2] = pz; }
+  }
+}
+
+// One thread per candidate point: project into view b (pose P = [R | o] camera-to-world, the camera looking down -z), take the
+// nearest cell of the out_h x out_w grid, and count the view when its depth map agrees there.
+__global__ void __launch_bounds__(128)
+depth_consistency_kernel(const float* __restrict__ pts, const int* __restrict__ source, int n_pts, int view,
+                         const float* __restrict__ pose, const float* __restrict__ intri, const float* __restrict__ dist_params,
+                         int out_h, int out_w, float step_i, float step_j, const float* __restrict__ opacity,
+                         const float* __restrict__ median_t, float min_opacity, float rel_tol, int* __restrict__ count,
+                         int* __restrict__ cell) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pts) return;
+  if (source && __ldg(source + i) == view) {
+    if (cell) cell[i] = -1;
+    return;
+  }
+  const float dx = fsub(__ldg(pts + 3 * size_t(i)), __ldg(pose + 3));
+  const float dy = fsub(__ldg(pts + 3 * size_t(i) + 1), __ldg(pose + 7));
+  const float dz = fsub(__ldg(pts + 3 * size_t(i) + 2), __ldg(pose + 11));
+  float xc[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++)                                     // R^T (p - o): column k of R
+    xc[k] = ffma(__ldg(pose + 8 + k), dz, ffma(__ldg(pose + 4 + k), dy, fmul(__ldg(pose + k), dx)));
+  int idx = -1;
+  if (xc[2] < 0.f) {
+    const float u = fdiv(xc[0], -xc[2]), v = fdiv(xc[1], xc[2]);  // dir = (u, -v, -1) in the camera frame
+    const float u2 = fmul(u, u), uv = fmul(u, v), v2 = fmul(v, v);
+    float du, dv;
+    distort(load_dist(dist_params), u, v, u2, uv, v2, fadd(u2, v2), du, dv);
+    const float x = ffma(__ldg(intri), fadd(u, du), __ldg(intri + 2));        // fx u_d + cx
+    const float y = ffma(__ldg(intri + 4), fadd(v, dv), __ldg(intri + 5));    // fy v_d + cy
+    const float fb = fdiv(fsub(x, .5f), step_j), fa = fdiv(fsub(y, .5f), step_i);   // the grid's pixel centres sit at +.5
+    if (fb > -1.f && fb < float(out_w) && fa > -1.f && fa < float(out_h)) {
+      const int b = __float2int_rn(fb), a = __float2int_rn(fa);
+      if (b >= 0 && b < out_w && a >= 0 && a < out_h) idx = a * out_w + b;
+    }
+  }
+  if (cell) cell[i] = idx;
+  if (idx < 0 || !(__ldg(opacity + idx) >= min_opacity)) return;
+  const float tb = __ldg(median_t + idx);
+  const float dist = fsqrt(fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz)));
+  if (fabsf(fsub(dist, tb)) <= fmul(rel_tol, tb)) count[i] += 1;
+}
+
 }  // namespace f2b
 
 using namespace f2b;
+
+extern "C" int f2b_ray_termination_slots(const float* slot_t, const int* kept_counts, const float* w_slots, const float* rays_o,
+                                         const float* rays_d, int n_rays, int slot_size, float* opacity, float* median_t,
+                                         float* point, void* stream) {
+  if (n_rays <= 0) return F2B_OK;
+  F2B_REQUIRE(slot_t && kept_counts && w_slots && rays_o && rays_d && opacity && median_t, "f2b_ray_termination_slots: null pointer");
+  F2B_REQUIRE(slot_size > 0 && slot_size <= 32 * 1024, "f2b_ray_termination_slots: slot_size %d outside [1, 32768]", slot_size);
+  F2B_REQUIRE(int64_t(n_rays) * slot_size < (int64_t(1) << 31), "f2b_ray_termination_slots: n_rays * slot_size overflows int32");
+  const size_t smem = size_t(kTermWarps) * ((slot_size + 31) / 32) * sizeof(float);
+  ray_termination_kernel<<<div_up(n_rays, kTermWarps), kTermWarps * 32, smem, as_stream(stream)>>>(
+      slot_t, kept_counts, w_slots, rays_o, rays_d, n_rays, slot_size, opacity, median_t, point);
+  return check_launch("f2b_ray_termination_slots");
+}
+
+extern "C" int f2b_depth_consistency(const float* pts, const int* source, int n_pts, int view, const float* pose, const float* intri,
+                                     const float* dist_params, int height, int width, int out_h, int out_w, const float* opacity,
+                                     const float* median_t, float min_opacity, float rel_tol, int* count, int* cell, void* stream) {
+  if (n_pts <= 0) return F2B_OK;
+  F2B_REQUIRE(pts && pose && intri && dist_params && opacity && median_t && count, "f2b_depth_consistency: null pointer");
+  F2B_REQUIRE(out_h >= 2 && out_h <= height && out_w >= 2 && out_w <= width, "f2b_depth_consistency: grid %dx%d outside image %dx%d",
+              out_h, out_w, height, width);
+  F2B_REQUIRE(int64_t(out_h) * out_w < (int64_t(1) << 31), "f2b_depth_consistency: %d x %d cells overflow int32", out_h, out_w);
+  depth_consistency_kernel<<<div_up(n_pts, 128), 128, 0, as_stream(stream)>>>(
+      pts, source, n_pts, view, pose, intri, dist_params, out_h, out_w, linspace_step(height, out_h), linspace_step(width, out_w),
+      opacity, median_t, min_opacity, rel_tol, count, cell);
+  return check_launch("f2b_depth_consistency");
+}
 
 extern "C" int f2b_locate_points(const void* tree_nodes, int n_nodes, const void* trans, const float* pts, int n_pts,
                                  float* warped, int* anchors, void* stream) {

@@ -7,26 +7,9 @@
 // fuses further mul+sub pairs that the PTX still shows separately) and is spelled out with explicit roundings, so rays are bit-identical to the reference's (tests/test_ref_parity.py).
 // f2b_camera_rays is the whole-camera path of the evaluation modes (Dataset::RaysOfCamera / RaysFromPose), an ATen sequence in the
 // reference, in one kernel (tests/test_gpu_eval.py).
-#include "common.cuh"
+#include "camera.cuh"
 
 namespace f2b {
-
-struct Dist { float k1, k2, p1, p2, two_p1, two_p2; };
-
-// apply_camera_distortion (Dataset.cu:16-28) as compiled: radial = fma(r2,k1, r2*(r2*k2));
-// du = fma(fma(u2,2,r2), p2, fma(uv, 2p1, u*radial)); dv = fma(fma(v2,2,r2), p1, fma(v, radial, uv*2p2))
-__device__ __forceinline__ void distort(const Dist& d, float u, float v, float u2, float uv, float v2, float r2, float& du, float& dv) {
-  const float radial = ffma(r2, d.k1, fmul(r2, fmul(r2, d.k2)));
-  du = ffma(ffma(u2, 2.f, r2), d.p2, ffma(uv, d.two_p1, fmul(u, radial)));
-  dv = ffma(ffma(v2, 2.f, r2), d.p1, ffma(v, radial, fmul(uv, d.two_p2)));
-}
-
-__device__ __forceinline__ Dist load_dist(const float* dp) {
-  Dist d;
-  d.k1 = __ldg(dp); d.k2 = __ldg(dp + 1); d.p1 = __ldg(dp + 2); d.p2 = __ldg(dp + 3);
-  d.two_p1 = fadd(d.p1, d.p1); d.two_p2 = fadd(d.p2, d.p2);
-  return d;
-}
 
 // iterative_camera_undistortion (Dataset.cu:30-69) on the OpenCV-style point (u0, v0).  It is inlined twice in the reference
 // build, into Img2WorldRayKernel and into CameraUndistortKernel (:71-76); ptxas schedules the two loops differently but makes
@@ -143,7 +126,7 @@ extern "C" int f2b_camera_rays(const float* pose, const float* intri, const floa
   F2B_REQUIRE(int64_t(out_h) * out_w < (int64_t(1) << 31), "f2b_camera_rays: %d x %d rays overflow int32", out_h, out_w);
   // torch::linspace(0.f, H - 1.f, n): end and step in fp32 on the host, exactly as ATen forms them
   const float end_i = float(height) - 1.f, end_j = float(width) - 1.f;
-  const float step_i = out_h > 1 ? (end_i - 0.f) / float(out_h - 1) : 0.f, step_j = out_w > 1 ? (end_j - 0.f) / float(out_w - 1) : 0.f;
+  const float step_i = linspace_step(height, out_h), step_j = linspace_step(width, out_w);
   const int n = out_h * out_w;
   camera_rays_kernel<<<div_up(n, 128), 128, 0, as_stream(stream)>>>(out_h, out_w, end_i, step_i, end_j, step_j, pose, intri,
                                                                     dist_params, rays_o, rays_d);

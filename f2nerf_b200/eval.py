@@ -110,6 +110,35 @@ def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_B
     return out[:, :3].contiguous(), out[:, 3:4].contiguous(), out[:, 4:5].contiguous()
 
 
+def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None):
+    """The tiled VALIDATE loop of ``RenderWholeImage`` with a kernel behind every chunk: ``render_forward`` of rays [i, j) on one of
+    two lane streams, then ``each(result, i, j)`` on the same stream, over the chunk's slots.  ``out`` = (colors [N,3], disparity [N],
+    depth [N]) to write into, else per-lane scratch; ``bg``: render_forward's background override.  No host sync; the lanes are
+    joined to the current stream at the end.  The caller sets VALIDATE mode."""
+    n_rays = d.shape[0]
+    main = torch.cuda.current_stream(dev)
+    lanes = [renderer._side_stream(dev, 3), renderer._side_stream(dev, 4)]
+    ready = torch.cuda.Event()
+    ready.record(main)
+    if out is None:
+        f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
+        unused = [(f32(ray_batch_size, 3), f32(ray_batch_size), f32(ray_batch_size)) for _ in lanes]   # colours etc., per lane
+    alive = []
+    for k, i in enumerate(range(0, n_rays, ray_batch_size)):
+        j = min(i + ray_batch_size, n_rays)
+        st = lanes[k % 2]
+        if k < 2:
+            st.wait_event(ready)
+        with torch.cuda.stream(st):
+            dst = tuple(u[:j - i] for u in unused[k % 2]) if out is None else tuple(u[i:j] for u in out)
+            r = renderer.render_forward(o[i:j], d[i:j], out=dst, lane=1 + k % 2, bg=bg)
+            each(r, i, j)
+        alive.append(r)                                      # allocations of a lane stay referenced until the join below
+    for st in lanes:
+        main.wait_stream(st)
+    del alive
+
+
 @torch.no_grad()
 def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None):
     """-> normals [N,3] CPU float32: the normal map of the rays in the normalised scene frame (DESIGN.md §3j).  Per ray,
@@ -128,28 +157,40 @@ def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, devic
         return normals.cpu()
     f = renderer.scene_field_
     trans = renderer.pts_sampler_.pers_trans_gpu_
+
+    def each(r, i, j):
+        ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_, f.mlp_.params_f16(),
+                                 r._keep[0], r.kept_counts, r._w_slots, out=normals[i:j])
+
     with _Validate(renderer):
-        main = torch.cuda.current_stream(dev)
-        lanes = [renderer._side_stream(dev, 3), renderer._side_stream(dev, 4)]
-        ready = torch.cuda.Event()
-        ready.record(main)
-        f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
-        unused = [(f32(ray_batch_size, 3), f32(ray_batch_size), f32(ray_batch_size)) for _ in lanes]   # colours etc., per lane
-        alive = []
-        for k, i in enumerate(range(0, n_rays, ray_batch_size)):
-            j = min(i + ray_batch_size, n_rays)
-            st = lanes[k % 2]
-            if k < 2:
-                st.wait_event(ready)
-            with torch.cuda.stream(st):
-                r = renderer.render_forward(o[i:j], d[i:j], out=tuple(u[:j - i] for u in unused[k % 2]), lane=1 + k % 2)
-                ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
-                                         f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=normals[i:j])
-            alive.append(r)                                  # allocations of a lane stay referenced until the join below
-        for st in lanes:
-            main.wait_stream(st)
-        del alive
+        _slot_chunks(renderer, o, d, ray_batch_size, dev, each)
     return normals.cpu()                                         # the one device->host copy
+
+
+@torch.no_grad()
+def RenderDepth(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None):
+    """-> (opacity [N], median_depth [N], depth [N]) CPU float32, in normalised scene units along the unit ray direction (times
+    ``dataset.radius_`` for data units; DESIGN.md §3l).  Per ray, over the samples the VALIDATE render keeps, with w_i the render's
+    weights: opacity W = sum_i w_i (fp32, serially in sample order); median_depth = t_m of the first sample m whose running sum
+    reaches W / 2 (a sample's own t: no interpolation, no offset); 0 for both where W = 0 (rays that miss included).  ``depth`` is
+    the renderer's own expectation sum_i w_i (t_i + 0.01) / (1 - T + 1e-4), bit for bit.  The rays are rendered in the tiled loop
+    of ``RenderNormals``, each chunk followed on its stream by the termination kernel over the chunk's slots; one device->host
+    copy at the end.  The same bits on every run and for any ``ray_batch_size``."""
+    from . import ops
+    dev = _device_of(renderer, device)
+    o, d = _to_dev(rays_o, dev), _to_dev(rays_d, dev)
+    n_rays = d.shape[0]
+    res = torch.zeros((3, n_rays), dtype=torch.float32, device=dev)          # opacity, median depth, depth
+    if n_rays == 0:
+        return tuple(res.cpu())
+    colors, disp = torch.empty((n_rays, 3), dtype=torch.float32, device=dev), torch.empty((n_rays,), dtype=torch.float32, device=dev)
+
+    def each(r, i, j):
+        ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=res[0, i:j], median_t=res[1, i:j])
+
+    with _Validate(renderer):
+        _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=(colors, disp, res[2]))
+    return tuple(res.cpu())                                      # the one device->host copy
 
 
 def quantify(x):

@@ -12,6 +12,11 @@ consistently oriented by construction, outward towards lower density.  DESIGN.md
 Surface normals (DESIGN.md §3j) come from the density itself: ``QueryGradient`` returns g = d logit / d x at world points (one
 kernel: the field query's forward, the field MLP's backward on the tensor pipe, the hash-grid blend's derivative and the leaf
 warp's Jacobian), ``QueryNormal`` the outward normal -g / |g|.
+
+A point cloud (DESIGN.md §3l) samples the surface where the views see it rather than on a lattice, so it keeps the detail of an
+unbounded scene near and far: ``ExtractPointCloud`` renders every view on a grid, puts a point at each opaque pixel's median
+sample (``eval.RenderDepth``'s termination kernel), coloured by the pixel's foreground colour, and keeps the points whose depth
+the other views confirm (``f2b_depth_consistency``).
 """
 import math
 from typing import NamedTuple, Optional
@@ -48,6 +53,20 @@ class Mesh(NamedTuple):
         differ by a uniform scale and a translation, so the normals carry over unchanged."""
         center = torch.as_tensor(dataset.center_, dtype=torch.float32, device=self.verts.device)
         return Mesh(self.verts * float(dataset.radius_) + center, self.faces, self.colors, self.normals)
+
+
+class PointCloud(NamedTuple):
+    """``points`` [P,3] fp32, ``colors`` [P,3] fp32 in [0, 1], ``normals`` [P,3] fp32 (unit or 0) or None, ``source`` [P,2] int32
+    (dataset view, grid cell a * w + b of the view's h x w grid); on the device, in the frame the cloud was made in."""
+    points: torch.Tensor
+    colors: torch.Tensor
+    normals: Optional[torch.Tensor]
+    source: torch.Tensor
+
+    def to_data_frame(self, dataset):
+        """The cloud in the data's own world frame: x * radius_ + center_, as ``Mesh.to_data_frame``; normals carry over."""
+        center = torch.as_tensor(dataset.center_, dtype=torch.float32, device=self.points.device)
+        return PointCloud(self.points * float(dataset.radius_) + center, self.colors, self.normals, self.source)
 
 
 def _octree(renderer):
@@ -243,11 +262,78 @@ def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, den
     return Mesh(verts, faces, rgb, nrm)
 
 
+def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0.9, min_views=2, rel_tol=0.01, normals=False):
+    """The scene's surface as a coloured ``PointCloud`` on the device, in the normalised frame (``to_data_frame`` maps it back).
+    Pass 1, per view of ``views`` (default ``dataset.train_set_``): the VALIDATE render of the view's own camera on the
+    (height // reso_level) x (width // reso_level) grid, with a black background, and the termination kernel on its slots (as
+    ``eval.RenderDepth``).  Every pixel with opacity W >= ``min_opacity`` gives a candidate: the world point of its median sample,
+    the colour C / W (the composite without background over the opacity, clipped to [0, 1]), with ``normals`` the pixel's normal
+    (as ``eval.RenderNormals``).  Pass 2, when ``min_views`` > 0: every candidate is projected into every other view of ``views``
+    (``f2b_depth_consistency``) and kept when at least ``min_views`` of them see an opaque pixel (opacity >= ``min_opacity``)
+    whose median depth is within ``rel_tol`` of the point's distance.  Points are ordered by (position of the view in ``views``,
+    cell); a run gives the same bits every time.  One host sync per view."""
+    from .eval import RAY_BATCH_SIZE, _slot_chunks, _Validate
+    views = [int(v) for v in (dataset.train_set_ if views is None else views)]
+    reso_level, min_views = int(reso_level), int(min_views)
+    if not views:
+        raise ValueError("ExtractPointCloud: no views")
+    if reso_level < 1:
+        raise ValueError("ExtractPointCloud: reso_level must be >= 1")
+    if not 0. < float(min_opacity) <= 1.:
+        raise ValueError("ExtractPointCloud: min_opacity must lie in (0, 1]")
+    if not 0 <= min_views <= len(views) - 1:
+        raise ValueError(f"ExtractPointCloud: min_views {min_views} outside [0, {len(views) - 1}] (the other views of {len(views)})")
+    if not float(rel_tol) >= 0.:
+        raise ValueError("ExtractPointCloud: rel_tol must be >= 0")
+    H, W = dataset.height_, dataset.width_
+    h, w = H // reso_level, W // reso_level
+    if h < 2 or w < 2:
+        raise ValueError(f"ExtractPointCloud: reso_level {reso_level} leaves a {h} x {w} grid of a {H} x {W} image")
+    n = h * w
+    dev = dataset.poses_.device
+    f = renderer.scene_field_
+    trans = renderer.pts_sampler_.pers_trans_gpu_
+    black = torch.zeros((3,), dtype=torch.float32, device=dev)
+    f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
+    maps, pts, cols, nrms, srcs = [], [], [], [], []
+    with torch.no_grad(), _Validate(renderer):
+        for b in views:
+            o, d = dataset._camera_rays(dataset.poses_[b], dataset.intri_[b], dataset.dist_params_[b], h, w)
+            opa, med, point, rgb = f32(n), f32(n), f32(n, 3), f32(n, 3)
+            nm = f32(n, 3) if normals else None
+
+            def each(r, i, j):
+                ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=opa[i:j], median_t=med[i:j], point=point[i:j])
+                if normals:
+                    ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
+                                             f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=nm[i:j])
+
+            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black)
+            cell = torch.nonzero(opa >= float(min_opacity)).squeeze(1)            # the host sync of the view; cells ascending
+            maps.append((opa, med))
+            pts.append(point[cell])
+            cols.append((rgb[cell] / opa[cell, None]).clamp_(0., 1.))
+            nrms.append(nm[cell] if normals else None)
+            srcs.append(torch.stack([torch.full_like(cell, b), cell], 1).to(torch.int32))
+        points, colors, source = torch.cat(pts), torch.cat(cols), torch.cat(srcs)
+        nrm = torch.cat(nrms) if normals else None
+        if min_views > 0 and points.shape[0] > 0:
+            count = torch.zeros((points.shape[0],), dtype=torch.int32, device=dev)
+            src_view = source[:, 0].contiguous()
+            for b, (opa, med) in zip(views, maps):
+                ops.depth_consistency(points, src_view, b, dataset.poses_[b], dataset.intri_[b], dataset.dist_params_[b], H, W, h, w,
+                                      opa, med, min_opacity, rel_tol, count)
+            keep = count >= min_views
+            points, colors, source = points[keep], colors[keep], source[keep]
+            nrm = nrm[keep] if normals else None
+    return PointCloud(points, colors, nrm, source)
+
+
 def write_ply(path, mesh):
-    """Binary little-endian PLY: float x, y, z (+ float nx, ny, nz when the mesh has normals, + uchar red, green, blue when it
-    has colours) and uchar-counted int triangle lists."""
-    v = mesh.verts.detach().cpu().numpy().astype("<f4")
-    f = mesh.faces.detach().cpu().numpy().astype("<i4")
+    """Binary little-endian PLY of a ``Mesh`` or a ``PointCloud``: float x, y, z (+ float nx, ny, nz when it has normals, + uchar
+    red, green, blue when it has colours) and, for a mesh, uchar-counted int triangle lists (a point cloud has no face element)."""
+    cloud = isinstance(mesh, PointCloud)
+    v = (mesh.points if cloud else mesh.verts).detach().cpu().numpy().astype("<f4")
     fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
     if mesh.normals is not None:
         fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
@@ -261,16 +347,20 @@ def write_ply(path, mesh):
     if mesh.colors is not None:
         c = np.clip(np.rint(mesh.colors.detach().cpu().numpy() * 255.), 0, 255).astype(np.uint8)
         vr["red"], vr["green"], vr["blue"] = c[:, 0], c[:, 1], c[:, 2]
-    fr = np.empty(len(f), [("n", "u1"), ("v", "<i4", (3,))])
-    fr["n"], fr["v"] = 3, f
     head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}", "property float x", "property float y",
             "property float z"]
     if mesh.normals is not None:
         head += ["property float nx", "property float ny", "property float nz"]
     if mesh.colors is not None:
         head += ["property uchar red", "property uchar green", "property uchar blue"]
-    head += [f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]
+    if not cloud:
+        f = mesh.faces.detach().cpu().numpy().astype("<i4")
+        fr = np.empty(len(f), [("n", "u1"), ("v", "<i4", (3,))])
+        fr["n"], fr["v"] = 3, f
+        head += [f"element face {len(f)}", "property list uchar int vertex_indices"]
+    head += ["end_header"]
     with open(path, "wb") as out:
         out.write(("\n".join(head) + "\n").encode("ascii"))
         out.write(vr.tobytes())
-        out.write(fr.tobytes())
+        if not cloud:
+            out.write(fr.tobytes())

@@ -234,6 +234,27 @@ def render_normals_slots(trans, table_f16, prim_pool, bias_pool, n_volumes, loca
     return normals
 
 
+def ray_termination_slots(slots, kept_counts, w_slots, opacity=None, median_t=None, point=None):
+    """(opacity [R], median_t [R]) of a VALIDATE batch from the march's slots and the fused forward's kept counts and slot weights
+    (DESIGN §3l); written into the given views, and the median sample's world point into ``point`` [R,3] when given."""
+    R, S = slots.n_rays, slots.slot
+    opacity = opacity if opacity is not None else dev_empty((R,), F32, kept_counts)
+    median_t = median_t if median_t is not None else dev_empty((R,), F32, kept_counts)
+    call("f2b_ray_termination_slots", slots.s_t, kept_counts, w_slots, slots.rays_o, slots.rays_d, R, S, opacity, median_t, point,
+         stream())
+    return opacity, median_t
+
+
+def depth_consistency(pts, source, view, pose, intri, dist_params, height, width, out_h, out_w, opacity, median_t, min_opacity,
+                      rel_tol, count, cell=None):
+    """f2b_depth_consistency: count[i] += 1 where point i agrees with view ``view``'s depth maps (DESIGN §3l); the point's cell
+    in that view into ``cell`` when given."""
+    _chk(pts, F32, "depth_consistency: pts")
+    call("f2b_depth_consistency", pts, source, int(pts.shape[0]), int(view), pose, intri, dist_params, int(height), int(width),
+         int(out_h), int(out_w), opacity, median_t, float(min_opacity), float(rel_tol), count, cell, stream())
+    return count
+
+
 def ray_grad(trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, feat_f16, d_field_out_f16, d_mlp_in_f16, pts,
              t, dirs, anchors, rays_o, bounds, inv_field_loss_scale, inv_shader_loss_scale, row_work, d_rays_o, d_rays_d, d_pts=None,
              d_dirs=None, dfeat16=None):

@@ -267,12 +267,14 @@ class Renderer:
         (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 keeps the operator pipeline (the launch sequences)."""
         return n_rays > 0 and os.environ.get("F2B_FUSED_FORWARD", "1") == "1"
 
-    def render_forward(self, rays_o, rays_d, out=None, lane=0):
+    def render_forward(self, rays_o, rays_d, out=None, lane=0, bg=None):
         """Renderer::Render (Renderer.cpp:52-213) for a batch that takes no gradient (VALIDATE mode): the march, then hash encode
         -> field MLP -> early stop -> SH + shader MLP -> composite in ONE kernel that walks each ray front to back and stops at
         the first opaque sample (csrc/fused_fwd.cu).  No host sync, no per-sample tensor in HBM; values bit-identical to the
         operator pipeline.  ``out`` = (colors [R,3], disparity [R], depth [R]) views to write into (whole-image rendering writes
         its image buffers directly); ``lane`` > 0 uses that extra scratch set so two chunks can be in flight on two streams.
+        ``bg``: a background colour [3] or [R,3] in place of the renderer's own; with a zero background the colour is exactly the
+        composite sum_i w_i c_i of the kept samples.
         Not reproduced: the reference's torch::rand draws for the MLP outputs (rng.py) — their sizes would need the host sync."""
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
@@ -280,7 +282,10 @@ class Renderer:
         sampler.march_rays(slots)
         if lane == 0:
             self.sample_result_ = LazySampleResult(slots)
-        bg = self._bg(n_rays, dev)
+        if bg is None:
+            bg = self._bg(n_rays, dev)
+        else:
+            bg = torch.as_tensor(bg, dtype=torch.float32, device=dev).expand(n_rays, 3).contiguous()
         S = slots.slot
         with torch.no_grad():
             table16 = field.table_f16()

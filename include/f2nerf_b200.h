@@ -213,6 +213,26 @@ int f2b_render_normals_slots(const void* trans, const void* table_f16, const int
                              const int* slot_anchors /* [.,2] */, const int* kept_counts, const float* w_slots,
                              const float* rays_o, const float* rays_d, int n_rays, int slot_size, float* tile_partials,
                              float* normals /* [n_rays,3] */, void* stream);
+/* Depth of a VALIDATE batch from the same slot buffers (DESIGN.md §3l).  Per ray r with k = kept_counts[r]: opacity[r] = W, the
+ * fp32 sum of w_slots[r*S + i], i < k, serially in slot order from +0; median_t[r] = slot_t[r*S + m] for the first m whose
+ * running sum (the same partial sums) is >= 0.5f * W; point[r] (nullable, [n_rays,3]) = fmaf(median_t, rays_d, rays_o) per
+ * component, rays_d the unit directions of the march's slots.  Where W is not > 0 (no kept sample, a ray that misses, all
+ * weights 0): opacity = median_t = 0 and point = 0.  The bits do not depend on the launch.  slot_size <= 32768. */
+int f2b_ray_termination_slots(const float* slot_t, const int* kept_counts, const float* w_slots, const float* rays_o,
+                              const float* rays_d, int n_rays, int slot_size, float* opacity /* [n_rays] */,
+                              float* median_t /* [n_rays] */, float* point, void* stream);
+/* Depth consistency of points [n_pts,3] (normalised frame) with view `view`: pose [3,4] camera-to-world (dir = R (u, -v, -1)),
+ * intri [3,3], dist_params [4] (k1, k2, p1, p2) and its opacity / median_t maps on the out_h x out_w grid
+ * linspace(0, height-1, out_h) x linspace(0, width-1, out_w) that f2b_camera_rays renders (cell a * out_w + b).  Points with
+ * source[i] == view are skipped (source nullable).  Otherwise x_c = R^T (p - o); in front when z_c < 0; u = x_c / -z_c,
+ * v = y_c / z_c, the forward distortion of the ray generation, x = fx u_d + cx, y = fy v_d + cy, and the nearest cell (pixel
+ * centres at linspace + .5).  count[i] += 1 when the cell is inside the grid, opacity there >= min_opacity and
+ * | |p - o| - median_t | <= rel_tol * median_t.  cell [n_pts] (nullable): the cell, -1 for skipped points, points behind the
+ * camera and points outside the grid.  out_h, out_w >= 2. */
+int f2b_depth_consistency(const float* pts, const int* source, int n_pts, int view, const float* pose, const float* intri,
+                          const float* dist_params, int height, int width, int out_h, int out_w, const float* opacity,
+                          const float* median_t, float min_opacity, float rel_tol, int* count /* [n_pts], in/out */,
+                          int* cell, void* stream);
 /* Gradient of the rendered colour with respect to the rays of a VALIDATE batch (DESIGN.md §3k), behind the composite, shader-MLP and
  * input-assembly backward: rows p < n_pts are the compacted survivors f2b_render_phase2_fwd leaves (pts, t, dirs, anchors [P,3], feat
  * [P,32] fp16), d_field_out [P,16] fp16 = f2b_shader_prep_bwd_f16's dL/dout of the field MLP and d_mlp_in [P,32] fp16 = f2b_mlp_bwd2's

@@ -1,0 +1,48 @@
+"""Export a trained scene's surface as a coloured PLY point cloud, fused from the training views on the device.
+
+    python scripts/export_points.py <runtime_config.yaml> <checkpoint_dir> --out cloud.ply [--reso-level 1]
+                                    [--min-opacity 0.9] [--min-views 2] [--normals]
+
+load_scene -> ExtractPointCloud (f2nerf_b200/geometry.py, DESIGN.md §3l); the cloud is written in the data's own world frame
+(PointCloud.to_data_frame).  Prints one JSON line: views, grid, point count, time and the GPU.
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("config")
+    ap.add_argument("checkpoint_dir")
+    ap.add_argument("--out", required=True)
+    ap.add_argument("--reso-level", type=int, default=1, help="render each view on a (height // r) x (width // r) grid")
+    ap.add_argument("--min-opacity", type=float, default=0.9, help="pixels below this opacity give no point")
+    ap.add_argument("--min-views", type=int, default=2, help="other views that must confirm a point's depth (0: keep all)")
+    ap.add_argument("--normals", action="store_true", help="the pixels' field normals (written as nx ny nz)")
+    a = ap.parse_args(argv)
+
+    import torch
+    from f2nerf_b200 import geometry as G, load_scene
+
+    scene = load_scene(a.config, a.checkpoint_dir, device="cuda")
+    ds = scene.dataset
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    pc = G.ExtractPointCloud(scene.renderer, ds, reso_level=a.reso_level, min_opacity=a.min_opacity, min_views=a.min_views,
+                             normals=a.normals)
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    G.write_ply(a.out, pc.to_data_frame(ds))
+    print(json.dumps(dict(views=len(ds.train_set_), grid=[ds.height_ // a.reso_level, ds.width_ // a.reso_level],
+                          min_opacity=a.min_opacity, min_views=a.min_views, points=int(pc.points.shape[0]), extract_s=dt,
+                          gpu=torch.cuda.get_device_properties(0).name, out=a.out)))
+
+
+if __name__ == "__main__":
+    main()

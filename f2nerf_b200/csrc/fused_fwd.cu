@@ -18,6 +18,8 @@
 // operand tiles (row results do not depend on which other rows share the tile), shade_row / shade_act (shader.cuh), and the
 // composite's SERIAL left-to-right sums (FlexOps.cu:5-73 order, as composite.cu) — colours / depth / disparity / weights come
 // out bit-identical to f2b_render_phase1 + _phase2_fwd (tests/test_gpu_render.py::test_fused_forward_matches_unfused).
+// f2b_render_fwd_fused_app is the same kernel with one appearance row added to every ray's shader input (DESIGN.md §3m), bit-identical
+// to the launch sequences with that row as a [1,16] table (tests/test_gpu_appearance.py).
 #include "common.cuh"
 #include "hash.cuh"
 #include "shader.cuh"
@@ -29,9 +31,9 @@ using namespace tc;
 constexpr int kRT = 128;
 
 // Shared memory of a CTA (one ray walker, 128 threads):
-//   [0, 20 KB) the two MLPs' weights | A0 8 KB + H0 16 KB | ray ticket + level scales.  The composite's scratch (tau, optical
-//   depth, the five addend rows) lives inside the walker's H0 tile, which is dead whenever the scratch is live (between an MLP's
-//   last MMA and the next MLP's first epilogue).
+//   [0, 20 KB) the two MLPs' weights | A0 8 KB + H0 16 KB | ray ticket + level scales (+ the appearance row, kApp only).  The
+//   composite's scratch (tau, optical depth, the five addend rows) lives inside the walker's H0 tile, which is dead whenever the
+//   scratch is live (between an MLP's last MMA and the next MLP's first epilogue).
 struct FusedSmem {
   static constexpr int SWH = 0;           // shader Wh   [64 x 64] SW128  8 KB
   static constexpr int FWO = 8192;        // field  Wout [16 x 64] SW128  2 KB
@@ -48,6 +50,8 @@ struct FusedSmem {
   static constexpr int ROWS = H0 + 4608;  // float rows[128][20]     (inside H0) an MLP's 16 outputs per sample
   static constexpr int BAR = WALK0 + WALK;        // 16 B: ray ticket (4); then 16 B | 16 level scales
   static constexpr int BYTES = BAR + 16 + 16 + 64 + 1024;   // + alignment slack (the tiles need 1024-byte alignment)
+  static constexpr int EMB = BAR + 16 + 16 + 64;  // float emb[16]: the appearance row of every ray of the launch (kApp only)
+  static constexpr int BYTES_APP = BYTES + 64;
 };
 
 __device__ __forceinline__ float h16(uint32_t acc_bits) { return __half2float(__float2half_rn(__uint_as_float(acc_bits))); }
@@ -60,7 +64,9 @@ __device__ __forceinline__ int walker_sync_count(bool pred) {
   return n;
 }
 
-// 3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers.
+// 3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers.  kApp: every ray is shaded with the one appearance
+// row app_emb [16], staged in shared memory once per CTA (read there by the shading-input assembly, not held in registers).
+template <bool kApp>
 __global__ void __launch_bounds__(kRT, 3)
 render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool,
                         int n_volumes, int local_size, const __half* __restrict__ fparams, const __half* __restrict__ sparams,
@@ -68,13 +74,15 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
                         const int* __restrict__ s_anchors, const int* __restrict__ counts, const float* __restrict__ rays_d,
                         const float* __restrict__ bg, int n_rays, int slot, const int* __restrict__ total_all,
                         int* __restrict__ ticket, float* __restrict__ colors, float* __restrict__ disparity,
-                        float* __restrict__ depth, int* __restrict__ kept_counts, float* __restrict__ weights_slots) {
+                        float* __restrict__ depth, int* __restrict__ kept_counts, float* __restrict__ weights_slots,
+                        const float* __restrict__ app_emb) {
   using S = FusedSmem;
   unsigned char* sm = smem_base();
   const int tid = threadIdx.x;                                   // thread == sample
   unsigned char* wsm = sm + S::WALK0;
   int* s_ray = reinterpret_cast<int*>(sm + S::BAR);
   float* s_scale = reinterpret_cast<float*>(sm + S::BAR + 16 + 16);
+  float* s_emb = reinterpret_cast<float*>(sm + S::EMB);
   float* s_tau = reinterpret_cast<float*>(wsm + S::TAU);
   float* s_acc = reinterpret_cast<float*>(wsm + S::ACC);         // exclusive optical depth per sample, [128] = inclusive end
   float* s_add = reinterpret_cast<float*>(wsm + S::ADD);         // [5][128] addends of the five per-ray sums
@@ -86,6 +94,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
   stage_weights<64, 0>(sparams + 64 * 32, 64, sm + S::SWH, tid);
   stage_weights<64, 0>(sparams + 64 * 32 + 64 * 64, 16, sm + S::SWO, tid);
   if (threadIdx.x < F2B_N_LEVELS) s_scale[threadIdx.x] = level_scale(threadIdx.x);
+  if (kApp && threadIdx.x < 16) s_emb[threadIdx.x] = __ldg(app_emb + threadIdx.x);
   fence_async_smem();
   __syncthreads();
   const uint32_t a0 = smem_u32(wsm + S::A0), h0 = smem_u32(wsm + S::H0);
@@ -183,7 +192,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       // ---- shader MLP input: [1, feat 1..15 | SH4(dir)] -> 64 -> 64 -> 16, colour activation --------------------------
       {
         uint4 row[4] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-        if (valid) shade_row(feat, nullptr, dx, dy, dz, row);
+        if (valid) shade_row_t<true>(feat, kApp ? s_emb : nullptr, dx, dy, dz, row);
 #pragma unroll
         for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = row[c];
       }
@@ -255,26 +264,55 @@ gather_kept_weights_kernel(const float* __restrict__ w_slots, const int* __restr
 
 using namespace f2b;
 
+namespace {
+template <bool kApp>
+int launch_render_fwd_fused(const char* name, const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
+                            int local_size, const void* field_params_f16, const void* shader_params_f16, const float* slot_pts,
+                            const float* slot_dt, const float* slot_t, const int* slot_anchors, const int* ray_counts,
+                            const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all, int* ticket,
+                            float* colors, float* disparity, float* depth, int* kept_counts, float* weights_slots,
+                            const float* app_emb, void* stream) {
+  if (n_rays <= 0) return F2B_OK;
+  F2B_REQUIRE(table_f16 && prim_pool && bias_pool && field_params_f16 && shader_params_f16 && slot_pts && slot_dt && slot_t &&
+                  slot_anchors && ray_counts && rays_d && bg && ticket && colors && disparity && depth && kept_counts &&
+                  (!kApp || app_emb),
+              "%s: null pointer", name);
+  F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "%s: bad n_volumes/local_size", name);
+  F2B_REQUIRE(slot_size > 0 && int64_t(n_rays) * slot_size < (int64_t(1) << 31), "%s: n_rays * slot_size overflows int32", name);
+  if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("%s: memset failed", name); return F2B_ECUDA; }
+  const int smem = kApp ? FusedSmem::BYTES_APP : FusedSmem::BYTES;
+  cudaFuncSetAttribute(render_fwd_fused_kernel<kApp>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const int grid = persistent_grid(n_rays, resident_per_sm(render_fwd_fused_kernel<kApp>, kRT, smem));
+  render_fwd_fused_kernel<kApp><<<grid, kRT, smem, as_stream(stream)>>>(
+      (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,
+      (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,
+      total_all, ticket, colors, disparity, depth, kept_counts, weights_slots, app_emb);
+  return check_launch(name);
+}
+}  // namespace
+
 extern "C" int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
                                     const void* field_params_f16, const void* shader_params_f16, const float* slot_pts,
                                     const float* slot_dt, const float* slot_t, const int* slot_anchors, const int* ray_counts,
                                     const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all,
                                     int* ticket, float* colors, float* disparity, float* depth, int* kept_counts,
                                     float* weights_slots, void* stream) {
-  if (n_rays <= 0) return F2B_OK;
-  F2B_REQUIRE(table_f16 && prim_pool && bias_pool && field_params_f16 && shader_params_f16 && slot_pts && slot_dt && slot_t &&
-                  slot_anchors && ray_counts && rays_d && bg && ticket && colors && disparity && depth && kept_counts,
-              "f2b_render_fwd_fused: null pointer");
-  F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "f2b_render_fwd_fused: bad n_volumes/local_size");
-  F2B_REQUIRE(slot_size > 0 && int64_t(n_rays) * slot_size < (int64_t(1) << 31), "f2b_render_fwd_fused: n_rays * slot_size overflows int32");
-  if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("f2b_render_fwd_fused: memset failed"); return F2B_ECUDA; }
-  cudaFuncSetAttribute(render_fwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem::BYTES);
-  const int grid = persistent_grid(n_rays, resident_per_sm(render_fwd_fused_kernel, kRT, FusedSmem::BYTES));
-  render_fwd_fused_kernel<<<grid, kRT, FusedSmem::BYTES, as_stream(stream)>>>(
-      (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,
-      (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,
-      total_all, ticket, colors, disparity, depth, kept_counts, weights_slots);
-  return check_launch("f2b_render_fwd_fused");
+  return launch_render_fwd_fused<false>("f2b_render_fwd_fused", table_f16, prim_pool, bias_pool, n_volumes, local_size,
+                                        field_params_f16, shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts,
+                                        rays_d, bg, n_rays, slot_size, total_all, ticket, colors, disparity, depth, kept_counts,
+                                        weights_slots, nullptr, stream);
+}
+
+extern "C" int f2b_render_fwd_fused_app(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
+                                        int local_size, const void* field_params_f16, const void* shader_params_f16,
+                                        const float* slot_pts, const float* slot_dt, const float* slot_t, const int* slot_anchors,
+                                        const int* ray_counts, const float* rays_d, const float* bg, int n_rays, int slot_size,
+                                        const int* total_all, int* ticket, float* colors, float* disparity, float* depth,
+                                        int* kept_counts, float* weights_slots, const float* app_emb, void* stream) {
+  return launch_render_fwd_fused<true>("f2b_render_fwd_fused_app", table_f16, prim_pool, bias_pool, n_volumes, local_size,
+                                       field_params_f16, shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts,
+                                       rays_d, bg, n_rays, slot_size, total_all, ticket, colors, disparity, depth, kept_counts,
+                                       weights_slots, app_emb, stream);
 }
 
 extern "C" int f2b_gather_kept_weights(const float* weights_slots, const int* new_bounds, int n_rays, int slot_size, float* weights,

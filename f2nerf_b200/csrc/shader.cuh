@@ -71,9 +71,11 @@ __device__ __forceinline__ void sh4_grad(float x, float y, float z, const float 
 }
 
 // Shader-MLP input row: fp16([1, feat[1..15]] + app_emb[cam] | SH4(dir)) (Renderer.cpp:179-187, SHShader.cpp:23-26,
-// identity-encoding cast).  feat[0..15] = the field output (fp16-rounded values), feat[0] is ignored.
-__device__ __forceinline__ void shade_row(const float feat[16], const float* __restrict__ emb_row /* nullable */,
-                                          float dx, float dy, float dz, uint4 row[4]) {
+// identity-encoding cast).  feat[0..15] = the field output (fp16-rounded values), feat[0] is ignored.  kSharedEmb: emb_row
+// points to shared memory (the fused forward stages its one row per CTA) and is read with plain loads; same adds, same bits.
+template <bool kSharedEmb>
+__device__ __forceinline__ void shade_row_t(const float feat[16], const float* __restrict__ emb_row /* nullable */,
+                                            float dx, float dy, float dz, uint4 row[4]) {
   float v[32];
 #pragma unroll
   for (int k = 0; k < 16; k++) v[k] = feat[k];
@@ -82,7 +84,7 @@ __device__ __forceinline__ void shade_row(const float feat[16], const float* __r
     const float4* e4 = reinterpret_cast<const float4*>(emb_row);
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      const float4 a = __ldg(e4 + q);
+      const float4 a = kSharedEmb ? e4[q] : __ldg(e4 + q);
       v[4 * q] = fadd(v[4 * q], a.x); v[4 * q + 1] = fadd(v[4 * q + 1], a.y);
       v[4 * q + 2] = fadd(v[4 * q + 2], a.z); v[4 * q + 3] = fadd(v[4 * q + 3], a.w);
     }
@@ -95,6 +97,11 @@ __device__ __forceinline__ void shade_row(const float feat[16], const float* __r
     for (int k = 0; k < 4; k++) h[k] = __floats2half2_rn(v[8 * q + 2 * k], v[8 * q + 2 * k + 1]);
     row[q] = *reinterpret_cast<uint4*>(h);
   }
+}
+
+__device__ __forceinline__ void shade_row(const float feat[16], const float* __restrict__ emb_row /* nullable */,
+                                          float dx, float dy, float dz, uint4 row[4]) {
+  shade_row_t<false>(feat, emb_row, dx, dy, dz, row);
 }
 
 // rgb = (1 + 2e-3) / (1 + exp(-o)) - 1e-3 on the fp16 MLP output (SHShader.cpp:27-28)

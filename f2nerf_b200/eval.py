@@ -36,10 +36,13 @@ def _to_dev(x, dev):
     return (x.contiguous().pin_memory() if torch.cuda.is_available() else x).to(dev, non_blocking=True)
 
 
-def _render_rays(renderer, o, d, ray_batch_size, dev):
+def _render_rays(renderer, o, d, ray_batch_size, dev, app=None):
     """The tiled VALIDATE-mode render of one image's rays (device [N,3] each) -> device (colors [N,3], first_oct_disp [N,1],
-    pred_disp [N,1]), normalised as ExpRunner.cpp:289-290.  No host sync on the fused path.  The caller sets VALIDATE mode."""
+    pred_disp [N,1]), normalised as ExpRunner.cpp:289-290.  No host sync on the fused path.  The caller sets VALIDATE mode.
+    ``app``: an appearance row [16] (``Renderer.appearance_row``) for every ray; only the fused kernel shades with one."""
     n_rays = d.shape[0]
+    if app is not None and not renderer._fused_forward_ok(n_rays) and n_rays > 0:
+        raise RuntimeError("appearance: rendering with an appearance row needs the fused forward (F2B_FUSED_FORWARD=1)")
     colors = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
     first = torch.full((n_rays, 1), 1., dtype=torch.float32, device=dev)
     disp = torch.zeros((n_rays, 1), dtype=torch.float32, device=dev)
@@ -60,7 +63,7 @@ def _render_rays(renderer, o, d, ray_batch_size, dev):
             if k < 2:
                 st.wait_event(ready)
             with torch.cuda.stream(st):
-                r = renderer.render_forward(o[i:j], d[i:j], out=(colors[i:j], disp_flat[i:j], depth[i:j]), lane=1 + k % 2)
+                r = renderer.render_forward(o[i:j], d[i:j], out=(colors[i:j], disp_flat[i:j], depth[i:j]), lane=1 + k % 2, app=app)
                 first[i:j] = r.first_oct_dis.reshape(-1, 1)
             alive.append(r)                                  # allocations of a lane stay referenced until the join below
         for st in lanes:
@@ -94,27 +97,34 @@ class _Validate:
         return False
 
 
+def resolve_appearance(renderer, appearance, view=None):
+    """``Renderer.appearance_row(appearance, view)``; None without asking the renderer when no appearance is given."""
+    return None if appearance is None else renderer.appearance_row(appearance, view=view)
+
+
 def _device_of(renderer, device):
     return torch.device(device) if device is not None else renderer.app_emb_.device
 
 
 @torch.no_grad()
-def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
     """-> (pred_colors [N,3], first_oct_disp [N,1], pred_disp [N,1]) CPU float32, like the reference.
     ``rays_o`` / ``rays_d``: [N,3] CPU or CUDA tensors; ``bounds`` is accepted and ignored (the sampler marches
-    [global_near_, 1e8], PersSampler.cu:322-323)."""
+    [global_near_, 1e8], PersSampler.cu:322-323).  ``appearance``: None, a training image's index or a [16] row
+    (``Renderer.appearance_row``, DESIGN.md §3m)."""
     dev = _device_of(renderer, device)
+    app = resolve_appearance(renderer, appearance)
     with _Validate(renderer):
-        colors, first, disp = _render_rays(renderer, _to_dev(rays_o, dev), _to_dev(rays_d, dev), ray_batch_size, dev)
+        colors, first, disp = _render_rays(renderer, _to_dev(rays_o, dev), _to_dev(rays_d, dev), ray_batch_size, dev, app)
     out = torch.cat([colors, first, disp], 1).cpu()              # the one device->host copy
     return out[:, :3].contiguous(), out[:, 3:4].contiguous(), out[:, 4:5].contiguous()
 
 
-def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None):
+def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None, app=None):
     """The tiled VALIDATE loop of ``RenderWholeImage`` with a kernel behind every chunk: ``render_forward`` of rays [i, j) on one of
     two lane streams, then ``each(result, i, j)`` on the same stream, over the chunk's slots.  ``out`` = (colors [N,3], disparity [N],
-    depth [N]) to write into, else per-lane scratch; ``bg``: render_forward's background override.  No host sync; the lanes are
-    joined to the current stream at the end.  The caller sets VALIDATE mode."""
+    depth [N]) to write into, else per-lane scratch; ``bg`` / ``app``: render_forward's background override and appearance row.
+    No host sync; the lanes are joined to the current stream at the end.  The caller sets VALIDATE mode."""
     n_rays = d.shape[0]
     main = torch.cuda.current_stream(dev)
     lanes = [renderer._side_stream(dev, 3), renderer._side_stream(dev, 4)]
@@ -131,7 +141,7 @@ def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None):
             st.wait_event(ready)
         with torch.cuda.stream(st):
             dst = tuple(u[:j - i] for u in unused[k % 2]) if out is None else tuple(u[i:j] for u in out)
-            r = renderer.render_forward(o[i:j], d[i:j], out=dst, lane=1 + k % 2, bg=bg)
+            r = renderer.render_forward(o[i:j], d[i:j], out=dst, lane=1 + k % 2, bg=bg, app=app)
             each(r, i, j)
         alive.append(r)                                      # allocations of a lane stay referenced until the join below
     for st in lanes:
@@ -260,7 +270,7 @@ def ImageMetrics(pred, gt):
 
 
 @torch.no_grad()
-def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
     """ExpRunner::TestImages (ExpRunner.cpp:343-391) on ``dataset.test_set_`` ->
     {"psnr": {idx: float}, "mean_psnr": float, "colors": [[H,W,3]], "disparity": [[H,W,1]], "first_oct_dis": [[H,W,1]],
      "psnr_8bit": {idx: float}, "mean_psnr_8bit": float, "ssim": {idx: float}, "mean_ssim": float}
@@ -268,15 +278,16 @@ def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
     accumulated in float64 on the device and PSNR = 20 log10(1 / sqrt(mse)) (:369).  "psnr_8bit" and "ssim" are what the
     reference's evaluation script reports for the written PNGs (``ImageMetrics``, scripts/eval.py:94-100), computed from the
     quantised colours behind each view's render.  The test images render back to back and all values come to the host in one
-    copy at the end."""
+    copy at the end.  ``appearance``: None, a training image's index or a [16] row for every view (``Renderer.appearance_row``)."""
     dev = _device_of(renderer, device)
+    app = resolve_appearance(renderer, appearance)
     H, W = dataset.height_, dataset.width_
     out = {"colors": [], "disparity": [], "first_oct_dis": []}
     psnrs, scores = [], []
     with _Validate(renderer):
         for idx in dataset.test_set_:
             rays_o, rays_d, _ = dataset.RaysOfCamera(idx)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev)
+            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app)
             q = quantify(colors.reshape(H, W, 3))
             gt = dataset.image_tensors_[idx].reshape(H, W, 3)
             mse = (q.double() - gt.double()).square().mean()
@@ -297,34 +308,51 @@ def TestImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
     return out
 
 
+def path_rows(renderer, appearance, n_frames):
+    """The appearance row of each of ``n_frames`` path frames: ``appearance`` as ``Renderer.appearance_row`` takes it for all frames,
+    or a [n_frames, 16] tensor with one row per frame (e.g. a blend of two looks along the path)."""
+    if isinstance(appearance, torch.Tensor) and appearance.dim() == 2:
+        if appearance.shape != (n_frames, 16):
+            raise ValueError(f"RenderPath: per-frame appearance rows must be [{n_frames}, 16], got {tuple(appearance.shape)}")
+        return [renderer.appearance_row(appearance[f]) for f in range(n_frames)]
+    return [resolve_appearance(renderer, appearance)] * n_frames
+
+
 @torch.no_grad()
-def RenderPath(renderer, dataset, reso_level=1, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def RenderPath(renderer, dataset, reso_level=1, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
     """ExpRunner::RenderPath (ExpRunner.cpp:322-341) over ``dataset.render_poses_`` -> list of device tuples
-    (colors [h,w,3], first_oct_dis [h,w,1], disparity [h,w,1]) with h, w = height // reso_level, width // reso_level."""
+    (colors [h,w,3], first_oct_dis [h,w,1], disparity [h,w,1]) with h, w = height // reso_level, width // reso_level.
+    ``appearance``: None, a training image's index or a [16] row for every frame, or a [F,16] tensor with one row per frame
+    (``path_rows``)."""
     if dataset.render_poses_ is None:
         raise ValueError("RenderPath: the dataset has no render_poses")
     dev = _device_of(renderer, device)
     h, w = dataset.height_ // int(reso_level), dataset.width_ // int(reso_level)
+    apps = path_rows(renderer, appearance, len(dataset.render_poses_))
     frames = []
     with _Validate(renderer):
-        for pose in dataset.render_poses_:
+        for pose, app in zip(dataset.render_poses_, apps):
             rays_o, rays_d, _ = dataset.RaysFromPose(pose, reso_level)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev)
+            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app)
             frames.append((colors.reshape(h, w, 3), first.reshape(h, w, 1), disp.reshape(h, w, 1)))
     return frames
 
 
 @torch.no_grad()
-def RenderAllImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def RenderAllImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
     """ExpRunner::RenderAllImages / VisualizeImage (ExpRunner.cpp:295-320): for every camera the device image
-    cat([GT | pred | first_oct_dis x3 | disparity x3], width) [H, 4W, 3] (GT zeros when the dataset holds no images)."""
+    cat([GT | pred | first_oct_dis x3 | disparity x3], width) [H, 4W, 3] (GT zeros when the dataset holds no images).
+    ``appearance``: None, a training image's index or a [16] row for every camera, or ``"own"``: each camera with its own row,
+    as its photo was trained (a camera outside the training set has an untrained row)."""
     dev = _device_of(renderer, device)
     H, W = dataset.height_, dataset.width_
     images = []
+    resolve_appearance(renderer, appearance, view=0)             # argument errors before any rendering
     with _Validate(renderer):
         for idx in range(dataset.n_images_):
             rays_o, rays_d, _ = dataset.RaysOfCamera(idx)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev)
+            app = resolve_appearance(renderer, appearance, view=idx)
+            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app)
             gt = (dataset.image_tensors_[idx].reshape(H, W, 3) if dataset.image_tensors_ is not None
                   else torch.zeros((H, W, 3), dtype=torch.float32, device=dev))
             images.append(torch.cat([gt, colors.reshape(H, W, 3), first.reshape(H, W, 1).expand(H, W, 3),

@@ -26,6 +26,7 @@ import torch
 
 from . import ops
 from ._lib import call, stream
+from .eval import resolve_appearance
 from .octree_build import TREE_NODE
 
 EMPTY_LOGIT = -1e4          # logit of a point outside every valid leaf: finite, and exp(EMPTY_LOGIT - 3) == 0 in fp32
@@ -123,9 +124,11 @@ def QueryNormal(renderer, pts):
     return unit_normals(QueryGradient(renderer, pts)[1])
 
 
-def QueryColor(renderer, pts, dirs):
-    """Colour [n,3] of world points [n,3] seen along unit directions ``dirs`` [n,3] (the way a ray travels), without the
-    appearance embedding, as the renderer's VALIDATE mode shades; 0 where no valid leaf holds the point."""
+def QueryColor(renderer, pts, dirs, appearance=None):
+    """Colour [n,3] of world points [n,3] seen along unit directions ``dirs`` [n,3] (the way a ray travels); 0 where no valid
+    leaf holds the point.  ``appearance`` (``Renderer.appearance_row``): None shades without the appearance embedding, as the
+    renderer's VALIDATE mode does; a training image's index or a [16] row is added to the shader input (DESIGN.md §3m)."""
+    app = resolve_appearance(renderer, appearance)
     pts = _points(pts, renderer)
     dirs = torch.as_tensor(dirs, dtype=torch.float32, device=pts.device).reshape(-1, 3).contiguous()
     warped, anchors = LocatePoints(renderer, pts)
@@ -140,7 +143,8 @@ def QueryColor(renderer, pts, dirs):
     d = dirs[rows].contiguous()
     logit = torch.empty((n,), dtype=torch.float32, device=pts.device)
     mlp_in = torch.empty((n, 32), dtype=torch.float16, device=pts.device)
-    call("f2b_field_shade_fwd", feat, fparams, d, None, None, n, logit, mlp_in, None, stream())
+    emb = (app[None], torch.zeros((n,), dtype=torch.int32, device=pts.device)) if app is not None else (None, None)
+    call("f2b_field_shade_fwd", feat, fparams, d, *emb, n, logit, mlp_in, None, stream())
     raw = torch.empty((n, 16), dtype=torch.float16, device=pts.device)
     out = torch.empty((n, 3), dtype=torch.float32, device=pts.device)
     call("f2b_shader_mlp_rgb_fwd", mlp_in, renderer.shader_.mlp_.params_f16(), n, raw, out, None, stream())
@@ -236,33 +240,36 @@ def vertex_normals(verts, faces):
     return n
 
 
-def VertexColors(renderer, verts, faces, normals=None):
+def VertexColors(renderer, verts, faces, normals=None, appearance=None):
     """Colour of each vertex seen from outside along its normal: ``QueryColor`` with view direction -n / |n|.  By default n is
     the area-weighted face normal (``vertex_normals``: sums of float atomics, so a colour can differ by an ulp from run to run);
-    ``normals`` [V,3] (unit or 0, e.g. ``QueryNormal``) replaces it wherever it is non-zero."""
+    ``normals`` [V,3] (unit or 0, e.g. ``QueryNormal``) replaces it wherever it is non-zero.  ``appearance``: as ``QueryColor``."""
     n = vertex_normals(verts, faces)
     if normals is not None:
         n = torch.where((normals != 0).any(1, keepdim=True), normals, n)
     d = -n / torch.linalg.norm(n, dim=1, keepdim=True).clamp_min(1e-30)
-    return QueryColor(renderer, verts, d)
+    return QueryColor(renderer, verts, d, appearance)
 
 
-def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, density=None, colors=True, normals=False):
+def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, density=None, colors=True, normals=False,
+                appearance=None):
     """The scene's surface as a ``Mesh`` on the device, in the normalised frame (``Mesh.to_data_frame`` maps it back).
     The level is the density that reaches opacity ``alpha`` over one VALIDATE march step (``level_from_alpha``), or
     ``density`` (per warp unit) when given; the lattice is ``DensityGrid(renderer, bbox_min, bbox_max, reso)``.
     ``normals``: the vertices get the field's normals (``QueryNormal``), and the colours are seen along them (the face normal
-    where the field normal is 0)."""
+    where the field normal is 0).  ``appearance``: the colours' appearance row, as ``QueryColor``."""
+    app = resolve_appearance(renderer, appearance)               # argument errors before the lattice is built
     level = math.log(float(density)) + 3. if density is not None else level_from_alpha(renderer, alpha)
     g = DensityGrid(renderer, bbox_min, bbox_max, reso)
     verts, faces = Isosurface(g.logit, level, g.origin, g.voxel)
     del g
     nrm = QueryNormal(renderer, verts) if normals else None
-    rgb = VertexColors(renderer, verts, faces, nrm) if colors and verts.shape[0] else None
+    rgb = VertexColors(renderer, verts, faces, nrm, app) if colors and verts.shape[0] else None
     return Mesh(verts, faces, rgb, nrm)
 
 
-def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0.9, min_views=2, rel_tol=0.01, normals=False):
+def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0.9, min_views=2, rel_tol=0.01, normals=False,
+                      appearance=None):
     """The scene's surface as a coloured ``PointCloud`` on the device, in the normalised frame (``to_data_frame`` maps it back).
     Pass 1, per view of ``views`` (default ``dataset.train_set_``): the VALIDATE render of the view's own camera on the
     (height // reso_level) x (width // reso_level) grid, with a black background, and the termination kernel on its slots (as
@@ -271,7 +278,9 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
     (as ``eval.RenderNormals``).  Pass 2, when ``min_views`` > 0: every candidate is projected into every other view of ``views``
     (``f2b_depth_consistency``) and kept when at least ``min_views`` of them see an opaque pixel (opacity >= ``min_opacity``)
     whose median depth is within ``rel_tol`` of the point's distance.  Points are ordered by (position of the view in ``views``,
-    cell); a run gives the same bits every time.  One host sync per view."""
+    cell); a run gives the same bits every time.  One host sync per view.  ``appearance`` colours the points
+    (``Renderer.appearance_row``): None, a training image's index, a [16] row, or ``"own"``: each view's own row.  The points
+    themselves do not depend on it (weights and density do not)."""
     from .eval import RAY_BATCH_SIZE, _slot_chunks, _Validate
     views = [int(v) for v in (dataset.train_set_ if views is None else views)]
     reso_level, min_views = int(reso_level), int(min_views)
@@ -285,6 +294,7 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
         raise ValueError(f"ExtractPointCloud: min_views {min_views} outside [0, {len(views) - 1}] (the other views of {len(views)})")
     if not float(rel_tol) >= 0.:
         raise ValueError("ExtractPointCloud: rel_tol must be >= 0")
+    apps = [resolve_appearance(renderer, appearance, view=b) for b in views]
     H, W = dataset.height_, dataset.width_
     h, w = H // reso_level, W // reso_level
     if h < 2 or w < 2:
@@ -297,7 +307,7 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
     f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
     maps, pts, cols, nrms, srcs = [], [], [], [], []
     with torch.no_grad(), _Validate(renderer):
-        for b in views:
+        for b, app in zip(views, apps):
             o, d = dataset._camera_rays(dataset.poses_[b], dataset.intri_[b], dataset.dist_params_[b], h, w)
             opa, med, point, rgb = f32(n), f32(n), f32(n, 3), f32(n, 3)
             nm = f32(n, 3) if normals else None
@@ -308,7 +318,7 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
                     ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
                                              f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=nm[i:j])
 
-            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black)
+            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black, app=app)
             cell = torch.nonzero(opa >= float(min_opacity)).squeeze(1)            # the host sync of the view; cells ascending
             maps.append((opa, med))
             pts.append(point[cell])

@@ -33,9 +33,10 @@ class _Batch:
     """The forward of one ray batch and every buffer the backward reads."""
 
 
-def _render(renderer, rays_o, rays_d_unit):
+def _render(renderer, rays_o, rays_d_unit, app=None):
     """VALIDATE render of unit-direction rays through the launch sequences: march into own scratch, early stop, compaction, field,
-    shader, composite.  One host sync (the survivor count)."""
+    shader, composite.  One host sync (the survivor count).  ``app``: an appearance row [16] for every ray, through phase 2's
+    embedding path (a [1,16] table, every ray on row 0)."""
     field, shader, sampler = renderer.scene_field_, renderer.shader_, renderer.pts_sampler_
     R, dev = rays_o.shape[0], rays_o.device
     S = MAX_SAMPLE_PER_RAY
@@ -66,6 +67,9 @@ def _render(renderer, rays_o, rays_d_unit):
                      a0=f32(R * S), keep=torch.empty((R * S,), dtype=torch.uint8, device=dev))
     ra.set(**b.scratch)
     b.keep_alive = [rays_o, rays_d_unit, heads, ra]
+    if app is not None:
+        b.app_table, b.ray_emb_idx = app.reshape(1, 16).contiguous(), torch.zeros((R,), dtype=torch.int32, device=dev)
+        ra.set(app_emb=b.app_table, n_emb=1, ray_emb_idx=b.ray_emb_idx)
     call("f2b_render_phase1", ra)
     n_kept, n_all, _ = heads.tolist()
     b.n_kept, b.n_all = n_kept, n_all
@@ -75,11 +79,28 @@ def _render(renderer, rays_o, rays_d_unit):
     T = dict(pts=f32(n_kept, 3), dirs=f32(n_kept, 3), dt=f32(n_kept), t=f32(n_kept), anchors=i32(n_kept, 3), feat_q=f16(n_kept, 32),
              logit=f32(n_kept), mlp_in=f16(n_kept, 32), raw=f16(n_kept, 16), rgb=f32(n_kept, 3), colors=f32(R, 3),
              disparity=f32(R), depth=f32(R), weights=f32(n_kept))
+    if app is not None:
+        T["pt_emb_idx"] = i32(n_kept)
     ra.set(n_kept=n_kept, n_edge_pairs=0, **T)
     call("f2b_render_phase2_fwd", ra)
     b.T, b.ra = T, ra
     b.colors = T["colors"]
     return b
+
+
+def _shader_input_bwd(b, d_colors, shader_scale):
+    """dL/dcolors -> (d_logit [P'], d_raw [P',16], d_in16 [P',32]) of the kept samples: the composite and colour-activation backward
+    and the shader MLP's backward to its input rows.  d_raw and d_in16 are fp16 and scaled by ``shader_scale``."""
+    nk, T, dev = b.n_kept, b.T, b.rays_o.device
+    d_colors = d_colors.to(device=dev, dtype=torch.float32).contiguous()
+    d_logit = torch.empty((nk,), dtype=torch.float32, device=dev)
+    d_raw, d_in16 = (torch.empty((nk, c), dtype=torch.float16, device=dev) for c in (16, 32))
+    d_sparams = torch.zeros((b.sparams16.numel(),), dtype=torch.float32, device=dev)       # scratch: the scene is not trained
+    if nk > 0:
+        call("f2b_composite_act_bwd", T["logit"], 1, T["rgb"], T["dt"], T["t"], b.new_bounds, b.bg, b.n_rays, d_colors, None, None, None,
+             1.0, T["raw"], float(shader_scale), d_logit, 1, d_raw, stream())
+        call("f2b_mlp_bwd2", d_raw, T["mlp_in"], None, None, b.sparams16, 1, nk, d_in16, d_sparams, stream())
+    return d_logit, d_raw, d_in16
 
 
 def _backprop(b, d_colors, shader_scale, field_scale, rows=False):
@@ -94,17 +115,13 @@ def _backprop(b, d_colors, shader_scale, field_scale, rows=False):
     nk, T, f = b.n_kept, b.T, b.renderer.scene_field_
     f16 = lambda *sh: torch.empty(sh, dtype=torch.float16, device=dev)
     f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
-    d_colors = d_colors.to(device=dev, dtype=torch.float32).contiguous()
-    d_logit, d_raw, d_in16, d_out16 = f32(nk), f16(nk, 16), f16(nk, 32), f16(nk, 16)
-    d_sparams = torch.zeros((b.sparams16.numel(),), dtype=torch.float32, device=dev)       # scratch: the scene is not trained
+    d_logit, d_raw, d_in16 = _shader_input_bwd(b, d_colors, shader_scale)
+    d_out16 = f16(nk, 16)
     work = f32(max(nk, 1), 6)
     d_pts = f32(nk, 3) if rows else None
     d_dirs = f32(nk, 3) if rows else None
     dfeat16 = f16(nk, 32) if rows else None
     if nk > 0:
-        call("f2b_composite_act_bwd", T["logit"], 1, T["rgb"], T["dt"], T["t"], b.new_bounds, b.bg, R, d_colors, None, None, None, 1.0,
-             T["raw"], float(shader_scale), d_logit, 1, d_raw, stream())
-        call("f2b_mlp_bwd2", d_raw, T["mlp_in"], None, None, b.sparams16, 1, nk, d_in16, d_sparams, stream())
         ops.shader_prep_bwd_f16(d_in16, d_logit, b.new_bounds, None, 1.0 / shader_scale, float(field_scale), d_out16, None)
     ops.ray_grad(b.renderer.pts_sampler_.pers_trans_gpu_, b.table16, f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
                  b.fparams16, T["feat_q"], d_out16, d_in16, T["pts"], T["t"], T["dirs"], T["anchors"], b.rays_o, b.new_bounds,
@@ -127,17 +144,24 @@ def _unit(rays_d):
     return (rays_d / torch.linalg.norm(rays_d, 2, -1, True)).contiguous()
 
 
+def backed_off(backward, finite, what):
+    """``backward(shader_scale, field_scale)`` at the fixed loss scales, backed off (both halved, as the trainer halves its scale)
+    only while ``finite(out)`` is False -> (out, shader_scale, field_scale)."""
+    sh, fs = SHADER_LOSS_SCALE, FIELD_LOSS_SCALE
+    for _ in range(_MAX_BACKOFF):
+        out = backward(sh, fs)
+        if finite(out):
+            return out, sh, fs
+        sh, fs = max(sh / 2., 1.), max(fs / 2., 1.)
+    raise FloatingPointError(f"{what} at every loss scale")
+
+
 def _vjp(b, d_colors, rays_d, rows=False):
     """Backward at the fixed loss scales, backed off (both halved, as the trainer halves its scale) only while the gradients are
     not finite."""
-    sh, fs = SHADER_LOSS_SCALE, FIELD_LOSS_SCALE
-    for _ in range(_MAX_BACKOFF):
-        out = _backprop(b, d_colors, sh, fs, rows)
-        if bool(torch.isfinite(out["d_o"]).all() & torch.isfinite(out["d_d"]).all()):
-            break
-        sh, fs = max(sh / 2., 1.), max(fs / 2., 1.)
-    else:
-        raise FloatingPointError("RayGradient: non-finite ray gradients at every loss scale")
+    out, sh, fs = backed_off(lambda sh, fs: _backprop(b, d_colors, sh, fs, rows),
+                             lambda out: bool(torch.isfinite(out["d_o"]).all() & torch.isfinite(out["d_d"]).all()),
+                             "RayGradient: non-finite ray gradients")
     d_dhat = out["d_d"]
     out.update(d_dhat=d_dhat, d_d=_chain_normalise(rays_d, d_dhat), shader_loss_scale=sh, field_loss_scale=fs)
     return out
@@ -287,18 +311,18 @@ def rays_from_pose(pose, dirs_cam):
     return o, d
 
 
-def _camera(camera, dataset, height, width):
+def _camera(camera, dataset, height, width, what="RefinePose"):
     if isinstance(camera, (int, np.integer)):
         if dataset is None:
-            raise ValueError("RefinePose: a camera given by index needs the dataset")
+            raise ValueError(f"{what}: a camera given by index needs the dataset")
         i = int(camera)
         if not 0 <= i < dataset.n_images_:
-            raise ValueError(f"RefinePose: camera index {i} outside [0, {dataset.n_images_})")
+            raise ValueError(f"{what}: camera index {i} outside [0, {dataset.n_images_})")
         if (dataset.height_, dataset.width_) != (height, width):
-            raise ValueError(f"RefinePose: the image is {height}x{width}, the dataset's cameras {dataset.height_}x{dataset.width_}")
+            raise ValueError(f"{what}: the image is {height}x{width}, the dataset's cameras {dataset.height_}x{dataset.width_}")
         return dataset.intri_[i], dataset.dist_params_[i]
     if not isinstance(camera, (tuple, list)) or len(camera) != 2:
-        raise ValueError("RefinePose: camera is (intrinsics [3,3], distortion [4]) or a dataset index")
+        raise ValueError(f"{what}: camera is (intrinsics [3,3], distortion [4]) or a dataset index")
     return camera
 
 

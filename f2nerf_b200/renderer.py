@@ -9,6 +9,7 @@ csrc/render.cu (f2b_render_phase1 / _phase2_fwd / _bwd / _grad_finalize), one fo
 shipped MLP shapes (field 32->64->16, shader 32->64->64->16) are supported.
 Host syncs per call: 2 (sample total, survivor total) against the reference's >= 11 ``.item()`` calls.
 """
+import numbers
 import os
 from dataclasses import dataclass
 from typing import Optional
@@ -267,14 +268,44 @@ class Renderer:
         (f2b_render_fwd_fused).  F2B_FUSED_FORWARD=0 keeps the operator pipeline (the launch sequences)."""
         return n_rays > 0 and os.environ.get("F2B_FUSED_FORWARD", "1") == "1"
 
-    def render_forward(self, rays_o, rays_d, out=None, lane=0, bg=None):
+    def appearance_row(self, appearance, view=None):
+        """The appearance row [16] (float32, on the renderer's device) that ``appearance`` names, or None (DESIGN.md §3m).  ``None``:
+        no embedding, the reference's VALIDATE shading.  An int: that image's row of ``app_emb_``.  A [16] tensor: used as given.
+        ``"own"``: the row of ``view`` (a dataset image index).  The shader adds the row to its input, [1, feat 1..15] + row, as
+        TRAIN mode does with the image's own row.  Raises ValueError on a renderer that trained no rows (``use_app_emb_`` False),
+        a bad shape, an index out of range, or ``"own"`` without a view."""
+        if appearance is None:
+            return None
+        if not self.use_app_emb_:
+            raise ValueError("appearance: this renderer has no trained appearance embedding (use_app_emb is False)")
+        n_rows = self.app_emb_.shape[0]
+        if isinstance(appearance, str):
+            if appearance != "own":
+                raise ValueError(f"appearance: unknown name {appearance!r} (None, an image index, a [16] row or 'own')")
+            if view is None:
+                raise ValueError("appearance: 'own' needs a view whose row to use")
+            appearance = view
+        if isinstance(appearance, bool):
+            raise ValueError("appearance: a bool is not an image index")
+        if isinstance(appearance, numbers.Integral):
+            i = int(appearance)
+            if not 0 <= i < n_rows:
+                raise ValueError(f"appearance: image index {i} outside [0, {n_rows})")
+            return self.app_emb_.detach()[i].clone()
+        row = torch.as_tensor(appearance)
+        if row.shape != (16,):
+            raise ValueError(f"appearance: a row has 16 entries, got shape {tuple(row.shape)}")
+        return row.detach().to(device=self.app_emb_.device, dtype=torch.float32).contiguous()
+
+    def render_forward(self, rays_o, rays_d, out=None, lane=0, bg=None, app=None):
         """Renderer::Render (Renderer.cpp:52-213) for a batch that takes no gradient (VALIDATE mode): the march, then hash encode
         -> field MLP -> early stop -> SH + shader MLP -> composite in ONE kernel that walks each ray front to back and stops at
         the first opaque sample (csrc/fused_fwd.cu).  No host sync, no per-sample tensor in HBM; values bit-identical to the
         operator pipeline.  ``out`` = (colors [R,3], disparity [R], depth [R]) views to write into (whole-image rendering writes
         its image buffers directly); ``lane`` > 0 uses that extra scratch set so two chunks can be in flight on two streams.
         ``bg``: a background colour [3] or [R,3] in place of the renderer's own; with a zero background the colour is exactly the
-        composite sum_i w_i c_i of the kept samples.
+        composite sum_i w_i c_i of the kept samples.  ``app``: an appearance row [16] (``appearance_row``) added to every ray's
+        shader input (``f2b_render_fwd_fused_app``); None shades without one.
         Not reproduced: the reference's torch::rand draws for the MLP outputs (rng.py) — their sizes would need the host sync."""
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
@@ -297,12 +328,18 @@ class Renderer:
             w_slots = self._buf(f"w_fwd{lane}", (n_rays * S,), torch.float32, dev)
             stamps = self.__dict__.setdefault("_fwd_stamp", {})
             stamps[lane] = stamps.get(lane, 0) + 1
-            call("f2b_render_fwd_fused", table16, field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_),
-                 fparams16, sparams16, slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors, slots.counts, slots.rays_d, bg, n_rays, S,
-                 slots.totals, ticket, colors, disparity, depth, kept, w_slots, stream())
+            args = (table16, field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_), fparams16, sparams16,
+                    slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors, slots.counts, slots.rays_d, bg, n_rays, S, slots.totals, ticket,
+                    colors, disparity, depth, kept, w_slots)
+            if app is None:
+                call("f2b_render_fwd_fused", *args, stream())
+            else:
+                if app.shape != (16,) or app.dtype != torch.float32 or not app.is_contiguous() or app.device != torch.device(dev):
+                    raise ValueError("render_forward: app must be a contiguous float32 [16] row on the rays' device")
+                call("f2b_render_fwd_fused_app", *args, app, stream())
         res = ForwardRenderResult(colors, slots.first_oct_dis, disparity, depth, kept, w_slots, S, self, (lane, stamps[lane]),
                                   slots.totals)
-        res._keep = (slots, table16, fparams16, sparams16, bg, ticket)          # alive until the result dies (stream-ordered reuse)
+        res._keep = (slots, table16, fparams16, sparams16, bg, ticket, app)     # alive until the result dies (stream-ordered reuse)
         return res
 
     def set_next_rays(self, rays_o, rays_d):

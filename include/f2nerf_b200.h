@@ -517,8 +517,8 @@ int f2b_set_trace(f2b_trace_fn fn);
  * hash encode -> field MLP -> early stop (T > 1e-4, Renderer.cpp:125) -> shading-feature assembly + SH4 -> shader MLP ->
  * colour activation -> composite, one CTA walking one ray front to back over the march's slot layout
  * (slot_pts [R*slot,3], slot_dt / slot_t [R*slot], slot_anchors [R*slot,2], ray_counts [R] as f2b_sampler_march leaves them)
- * and stopping at the first opaque sample — the samples behind it are never encoded.  No app embedding (Renderer.cpp:184
- * applies it in TRAIN mode only).  rays_d normalised, bg [R,3].  total_all: device int, the batch's sample total (NULL or
+ * and stopping at the first opaque sample — the samples behind it are never encoded.  No app embedding here (Renderer.cpp:184
+ * applies it in TRAIN mode only); f2b_render_fwd_fused_app shades with one.  rays_d normalised, bg [R,3].  total_all: device int, the batch's sample total (NULL or
  * > 0: normal; <= 0: the reference's empty-batch result, depth = 512, Renderer.cpp:83-97).  ticket: [1] device int scratch.
  * Outputs: colors [R,3], disparity [R], depth [R], kept_counts [R] (survivors per ray), and — nullable — weights_slots
  * [R*slot]: the kept samples' weights at their slots (f2b_gather_kept_weights packs them into RenderResult.weights order).
@@ -528,6 +528,17 @@ int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool, const floa
                          const float* slot_t, const int* slot_anchors, const int* ray_counts, const float* rays_d, const float* bg,
                          int n_rays, int slot_size, const int* total_all, int* ticket, float* colors, float* disparity,
                          float* depth, int* kept_counts, float* weights_slots, void* stream);
+/* f2b_render_fwd_fused with an appearance row (DESIGN.md §3m): app_emb [16] (device) is added to the shader input of every ray
+ * of the call, in shade_row's order: v[0] = 1 + app_emb[0], v[k] = feat[k] + app_emb[k] (k = 1..15), then fp16.  Colours,
+ * disparity, depth, kept_counts and weights_slots are bit-identical to f2b_render_phase1 + f2b_render_phase2_fwd with the
+ * [1,16] table app_emb (n_emb = 1) and ray_emb_idx = zeros.  The row is staged in shared memory once per CTA (64 B); the kernel
+ * keeps f2b_render_fwd_fused's 128 threads and 3 CTAs per SM.  Kept counts and weights do not depend on the row. */
+int f2b_render_fwd_fused_app(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                             const void* field_params_f16, const void* shader_params_f16, const float* slot_pts,
+                             const float* slot_dt, const float* slot_t, const int* slot_anchors, const int* ray_counts,
+                             const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all, int* ticket,
+                             float* colors, float* disparity, float* depth, int* kept_counts, float* weights_slots,
+                             const float* app_emb /* [16] */, void* stream);
 /* weights_slots [R*slot] + new_bounds [R,2] (f2b_count_scan of kept_counts) -> weights [P'] in the packed ray order. */
 int f2b_gather_kept_weights(const float* weights_slots, const int* new_bounds, int n_rays, int slot_size, float* weights,
                             void* stream);

@@ -3,8 +3,11 @@ trained into: checkpoints/latest/{renderer,scalars}.pt, test_images/), ``checkpo
 views.  Per view: the render time (CUDA events around a one-view TestImages: rays, tiled fused render, metrics; medians over
 --reps after a warm-up pass over all views), PSNR, 8-bit PSNR and SSIM, the PSNR the program wrote to test_images/info.yaml,
 and how far this path's colour PNG bytes are from the program's own PNG of that view.  Records the GPU and its power limit.
+``--appearance`` adds ``appearance.TestAppearance``'s numbers (DESIGN.md §3m): the right half of each test view scored with no
+appearance row, the training views' mean row and a row fitted on the left half.
 
     python scripts/eval_trained.py /tmp/f2b_train_ref /tmp/f2b_train_b200 [--config oracle/ref_config_ngp_fox.yaml] [--reps 3]
+        [--appearance]
 
 Run from the directory the program trained in: the config's dataset.data_path is relative to it.
 """
@@ -27,7 +30,7 @@ def power_limit():
         return None
 
 
-def evaluate(exp, config, reps):
+def evaluate(exp, config, reps, appearance=False):
     import numpy as np
     import torch
     import yaml
@@ -69,10 +72,16 @@ def evaluate(exp, config, reps):
                                        mean_abs_levels=float(d.mean()))
         views.append(v)
     mean = lambda key: float(np.mean([v[key] for v in views]))
-    return dict(experiment=exp, iter_step=scene.iter_step, ray_march_fineness=scene.global_data_pool.ray_march_fineness_,
-                image_hw=[ds.height_, ds.width_], n_test_views=len(views), ms_per_view=mean("ms"), mean_psnr=out["mean_psnr"],
-                mean_psnr_8bit=out["mean_psnr_8bit"], mean_ssim=out["mean_ssim"], program_mean_psnr=info.get("mean_psnr"),
-                views=views)
+    rec = dict(experiment=exp, iter_step=scene.iter_step, ray_march_fineness=scene.global_data_pool.ray_march_fineness_,
+               image_hw=[ds.height_, ds.width_], n_test_views=len(views), ms_per_view=mean("ms"), mean_psnr=out["mean_psnr"],
+               mean_psnr_8bit=out["mean_psnr_8bit"], mean_ssim=out["mean_ssim"], program_mean_psnr=info.get("mean_psnr"),
+               views=views)
+    if appearance:
+        from f2nerf_b200 import TestAppearance
+        res = TestAppearance(renderer, ds)
+        rec["appearance"] = {k: {m: res[k][m] for m in ("psnr", "psnr_8bit", "ssim", "mean_psnr", "mean_psnr_8bit", "mean_ssim")}
+                             for k in ("none", "mean", "fit")}
+    return rec
 
 
 def main():
@@ -81,11 +90,12 @@ def main():
     ap.add_argument("--config", default=os.path.join(ROOT, "oracle", "ref_config_ngp_fox.yaml"))
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--appearance", action="store_true", help="also run TestAppearance (fit on the left half, score the right)")
     args = ap.parse_args()
     import torch
     torch.cuda.set_device(0)
     rec = dict(probe="eval_trained", gpu=torch.cuda.get_device_name(0), power_limit_w=power_limit(), config=args.config,
-               reps=args.reps, experiments=[evaluate(e, args.config, args.reps) for e in args.experiments])
+               reps=args.reps, experiments=[evaluate(e, args.config, args.reps, args.appearance) for e in args.experiments])
     text = json.dumps(rec, indent=1)
     if args.out:
         with open(args.out, "w") as f:

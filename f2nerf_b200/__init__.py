@@ -7,6 +7,7 @@ this package is the thin host-side mirror of the reference's operator surface
 """
 from . import _lib  # noqa: F401  (fails loudly when the CUDA extension is missing)
 from .appearance import FitAppearance, TestAppearance
+from .crop import Crop
 from .checkpoint import Scene, gradient_scaling_progress, load_scene, load_states
 from .dataset import RayGenerator, load_dataset
 from .octree_build import build_edge_pool, build_tree_nodes, initial_octree
@@ -19,6 +20,6 @@ from .renderer import Renderer, RenderResult, check_backward_nan
 from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultFlex
 from .shader import SHShader
 
-__all__ = ["FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
+__all__ = ["Crop", "FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
            "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderDepth", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

@@ -102,6 +102,9 @@ SIGNATURES = {
     "f2b_render_fwd_fused": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P],
     "f2b_render_fwd_fused_app": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P,
                                  _P],
+    "f2b_render_fwd_fused_crop": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P,
+                                  _P, _P, _P, c_int, _P],
+    "f2b_crop_mask": [_P, c_int, _P, c_int, _P, _P],
     "f2b_gather_kept_weights": [_P, _P, c_int, c_int, _P, _P],
 }
 TRACE_FN = ctypes.CFUNCTYPE(None, ctypes.c_char_p, c_int, c_void_p)      # f2b_trace_fn

@@ -20,7 +20,11 @@
 // out bit-identical to f2b_render_phase1 + _phase2_fwd (tests/test_gpu_render.py::test_fused_forward_matches_unfused).
 // f2b_render_fwd_fused_app is the same kernel with one appearance row added to every ray's shader input (DESIGN.md §3m), bit-identical
 // to the launch sequences with that row as a [1,16] table (tests/test_gpu_appearance.py).
+// f2b_render_fwd_fused_crop renders only what a crop box keeps (DESIGN.md §3n): a sample whose world point fma(t, d, o) the box
+// removes has density 0 (tau = alpha = weight = +0) and is never encoded, and a tile the box removes whole skips both MLPs.  The result is
+// bit-identical to the same kernel over a slot layout with the removed samples deleted (tests/test_gpu_crop.py).
 #include "common.cuh"
+#include "crop.cuh"
 #include "hash.cuh"
 #include "shader.cuh"
 #include "tc.cuh"
@@ -66,7 +70,9 @@ __device__ __forceinline__ int walker_sync_count(bool pred) {
 
 // 3 CTAs per SM, <= 168 registers: the wgmma accumulators live in registers.  kApp: every ray is shaded with the one appearance
 // row app_emb [16], staged in shared memory once per CTA (read there by the shading-input assembly, not held in registers).
-template <bool kApp>
+// kCrop: samples whose world point fma(t, d, o) `crop` does not keep have density 0 (crop.cuh); the box stays in the parameter
+// bank.  (slot_pts are the warped coordinates the encode reads, so the point is formed from the slot's t and the ray, rays_o [R,3].)
+template <bool kApp, bool kCrop>
 __global__ void __launch_bounds__(kRT, 3)
 render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict__ prim_pool, const float* __restrict__ bias_pool,
                         int n_volumes, int local_size, const __half* __restrict__ fparams, const __half* __restrict__ sparams,
@@ -75,7 +81,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
                         const float* __restrict__ bg, int n_rays, int slot, const int* __restrict__ total_all,
                         int* __restrict__ ticket, float* __restrict__ colors, float* __restrict__ disparity,
                         float* __restrict__ depth, int* __restrict__ kept_counts, float* __restrict__ weights_slots,
-                        const float* __restrict__ app_emb) {
+                        const float* __restrict__ app_emb, const CropBox crop, const float* __restrict__ rays_o) {
   using S = FusedSmem;
   unsigned char* sm = smem_base();
   const int tid = threadIdx.x;                                   // thread == sample
@@ -137,10 +143,25 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       const int nv = min(kRT, cnt - t0);
       const bool valid = tid < nv;
       const size_t p = base + t0 + tid;
+      // ---- crop: a removed sample is a padding lane with density 0 -----------------------------------------------
+      bool in_crop = true;                                       // (kCrop) my sample is kept by the box
+      if (kCrop) {
+        if (valid) {
+          const float t = __ldg(s_t + p);
+          in_crop = crop_keep(crop, ffma(t, dx, __ldg(rays_o + ray * 3)), ffma(t, dy, __ldg(rays_o + ray * 3 + 1)),
+                              ffma(t, dz, __ldg(rays_o + ray * 3 + 2)));
+        }
+        if (walker_sync_count(valid && in_crop) == 0) {          // the box removes the whole tile: every sample has T = exp(-run),
+          if (walker_sync_count(tid == 0 && expf(-run) > 1e-4f) == 0) break;   // so all of them are kept (weight 0), or none
+          if (valid && weights_slots) weights_slots[p] = 0.f;
+          n_kept += nv;                                          // run and run_end stay: the tile adds no optical depth
+          continue;
+        }
+      }
       // ---- encode my sample -> operand row ------------------------------------------------------------------------
       uint32_t enc[16];
       float dt_i = 0.f;
-      if (valid) {
+      if (valid && in_crop) {
         encode_point(table, prim_pool, bias_pool, n_volumes, local_size, s_scale, __ldg(s_pts + p * 3), __ldg(s_pts + p * 3 + 1),
                      __ldg(s_pts + p * 3 + 2), __ldg(s_anchors + p * 2), enc);
         dt_i = __ldg(s_dt + p);
@@ -168,8 +189,8 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       }
       // ---- early stop: optical depth in serial order, transmittance, keep = T > 1e-4 (Renderer.cpp:115-126) ----------
       // (H0 is dead from here to the shader MLP's first epilogue: tau / acc live in it)
-      float tau = 0.f, alpha = 0.f;
-      if (valid) {
+      float tau = 0.f, alpha = 0.f;                              // +0 for padding lanes and removed samples
+      if (valid && in_crop) {
         const float dens = expf(fsub(feat[0], 3.f));             // TruncExp(x - 3)
         tau = fmul(dens, dt_i);
         alpha = fsub(1.f, expf(-tau));
@@ -192,7 +213,7 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
       // ---- shader MLP input: [1, feat 1..15 | SH4(dir)] -> 64 -> 64 -> 16, colour activation --------------------------
       {
         uint4 row[4] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-        if (valid) shade_row_t<true>(feat, kApp ? s_emb : nullptr, dx, dy, dz, row);
+        if (valid && in_crop) shade_row_t<true>(feat, kApp ? s_emb : nullptr, dx, dy, dz, row);
 #pragma unroll
         for (int c = 0; c < 4; c++) *reinterpret_cast<uint4*>(wsm + S::A0 + sw64_off(tid, c)) = row[c];
       }
@@ -248,6 +269,13 @@ render_fwd_fused_kernel(const __half* __restrict__ table, const int* __restrict_
 #undef F2B_OUT_ROW
 }
 
+// kept[i] = crop_keep(pts[i]) for n points (f2b_crop_mask)
+__global__ void __launch_bounds__(256)
+crop_mask_kernel(const float* __restrict__ pts, int n, const CropBox crop, uint8_t* __restrict__ kept) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) kept[i] = crop_keep(crop, __ldg(pts + size_t(i) * 3), __ldg(pts + size_t(i) * 3 + 1), __ldg(pts + size_t(i) * 3 + 2));
+}
+
 // weights of the kept samples out of the slot layout into the reference's packed layout (RenderResult.weights, Renderer.h:24)
 __global__ void __launch_bounds__(256)
 gather_kept_weights_kernel(const float* __restrict__ w_slots, const int* __restrict__ new_bounds, int n_rays, int slot,
@@ -265,28 +293,28 @@ gather_kept_weights_kernel(const float* __restrict__ w_slots, const int* __restr
 using namespace f2b;
 
 namespace {
-template <bool kApp>
+template <bool kApp, bool kCrop>
 int launch_render_fwd_fused(const char* name, const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
                             int local_size, const void* field_params_f16, const void* shader_params_f16, const float* slot_pts,
                             const float* slot_dt, const float* slot_t, const int* slot_anchors, const int* ray_counts,
                             const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all, int* ticket,
                             float* colors, float* disparity, float* depth, int* kept_counts, float* weights_slots,
-                            const float* app_emb, void* stream) {
+                            const float* app_emb, const CropBox& crop, const float* rays_o, void* stream) {
   if (n_rays <= 0) return F2B_OK;
   F2B_REQUIRE(table_f16 && prim_pool && bias_pool && field_params_f16 && shader_params_f16 && slot_pts && slot_dt && slot_t &&
                   slot_anchors && ray_counts && rays_d && bg && ticket && colors && disparity && depth && kept_counts &&
-                  (!kApp || app_emb),
+                  (!kApp || app_emb) && (!kCrop || rays_o),
               "%s: null pointer", name);
   F2B_REQUIRE(n_volumes > 0 && local_size > 0 && (local_size % 2) == 0, "%s: bad n_volumes/local_size", name);
   F2B_REQUIRE(slot_size > 0 && int64_t(n_rays) * slot_size < (int64_t(1) << 31), "%s: n_rays * slot_size overflows int32", name);
   if (cudaMemsetAsync(ticket, 0, sizeof(int), as_stream(stream)) != cudaSuccess) { set_error("%s: memset failed", name); return F2B_ECUDA; }
   const int smem = kApp ? FusedSmem::BYTES_APP : FusedSmem::BYTES;
-  cudaFuncSetAttribute(render_fwd_fused_kernel<kApp>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  const int grid = persistent_grid(n_rays, resident_per_sm(render_fwd_fused_kernel<kApp>, kRT, smem));
-  render_fwd_fused_kernel<kApp><<<grid, kRT, smem, as_stream(stream)>>>(
+  cudaFuncSetAttribute(render_fwd_fused_kernel<kApp, kCrop>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const int grid = persistent_grid(n_rays, resident_per_sm(render_fwd_fused_kernel<kApp, kCrop>, kRT, smem));
+  render_fwd_fused_kernel<kApp, kCrop><<<grid, kRT, smem, as_stream(stream)>>>(
       (const __half*)table_f16, prim_pool, bias_pool, n_volumes, local_size, (const __half*)field_params_f16,
       (const __half*)shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size,
-      total_all, ticket, colors, disparity, depth, kept_counts, weights_slots, app_emb);
+      total_all, ticket, colors, disparity, depth, kept_counts, weights_slots, app_emb, crop, rays_o);
   return check_launch(name);
 }
 }  // namespace
@@ -297,10 +325,10 @@ extern "C" int f2b_render_fwd_fused(const void* table_f16, const int* prim_pool,
                                     const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all,
                                     int* ticket, float* colors, float* disparity, float* depth, int* kept_counts,
                                     float* weights_slots, void* stream) {
-  return launch_render_fwd_fused<false>("f2b_render_fwd_fused", table_f16, prim_pool, bias_pool, n_volumes, local_size,
+  return launch_render_fwd_fused<false, false>("f2b_render_fwd_fused", table_f16, prim_pool, bias_pool, n_volumes, local_size,
                                         field_params_f16, shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts,
                                         rays_d, bg, n_rays, slot_size, total_all, ticket, colors, disparity, depth, kept_counts,
-                                        weights_slots, nullptr, stream);
+                                        weights_slots, nullptr, CropBox{}, nullptr, stream);
 }
 
 extern "C" int f2b_render_fwd_fused_app(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
@@ -309,10 +337,37 @@ extern "C" int f2b_render_fwd_fused_app(const void* table_f16, const int* prim_p
                                         const int* ray_counts, const float* rays_d, const float* bg, int n_rays, int slot_size,
                                         const int* total_all, int* ticket, float* colors, float* disparity, float* depth,
                                         int* kept_counts, float* weights_slots, const float* app_emb, void* stream) {
-  return launch_render_fwd_fused<true>("f2b_render_fwd_fused_app", table_f16, prim_pool, bias_pool, n_volumes, local_size,
+  return launch_render_fwd_fused<true, false>("f2b_render_fwd_fused_app", table_f16, prim_pool, bias_pool, n_volumes, local_size,
                                        field_params_f16, shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts,
                                        rays_d, bg, n_rays, slot_size, total_all, ticket, colors, disparity, depth, kept_counts,
-                                       weights_slots, app_emb, stream);
+                                       weights_slots, app_emb, CropBox{}, nullptr, stream);
+}
+
+extern "C" int f2b_render_fwd_fused_crop(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes,
+                                         int local_size, const void* field_params_f16, const void* shader_params_f16,
+                                         const float* slot_pts, const float* slot_dt, const float* slot_t, const int* slot_anchors,
+                                         const int* ray_counts, const float* rays_d, const float* bg, int n_rays, int slot_size,
+                                         const int* total_all, int* ticket, float* colors, float* disparity, float* depth,
+                                         int* kept_counts, float* weights_slots, const float* app_emb, const float* rays_o,
+                                         const float* box12, int invert, void* stream) {
+  F2B_REQUIRE(box12, "f2b_render_fwd_fused_crop: null box");
+  CropBox crop;
+  for (int k = 0; k < 12; k++) crop.m[k] = box12[k];
+  crop.invert = invert != 0;
+  const auto launch = app_emb ? launch_render_fwd_fused<true, true> : launch_render_fwd_fused<false, true>;
+  return launch("f2b_render_fwd_fused_crop", table_f16, prim_pool, bias_pool, n_volumes, local_size, field_params_f16,
+                shader_params_f16, slot_pts, slot_dt, slot_t, slot_anchors, ray_counts, rays_d, bg, n_rays, slot_size, total_all, ticket,
+                colors, disparity, depth, kept_counts, weights_slots, app_emb, crop, rays_o, stream);
+}
+
+extern "C" int f2b_crop_mask(const float* pts, int n, const float* box12, int invert, uint8_t* kept, void* stream) {
+  if (n <= 0) return F2B_OK;
+  F2B_REQUIRE(pts && box12 && kept, "f2b_crop_mask: null pointer");
+  CropBox crop;
+  for (int k = 0; k < 12; k++) crop.m[k] = box12[k];
+  crop.invert = invert != 0;
+  crop_mask_kernel<<<div_up(n, 256), 256, 0, as_stream(stream)>>>(pts, n, crop, kept);
+  return check_launch("f2b_crop_mask");
 }
 
 extern "C" int f2b_gather_kept_weights(const float* weights_slots, const int* new_bounds, int n_rays, int slot_size, float* weights,

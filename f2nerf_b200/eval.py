@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from ._lib import call, stream
+from .crop import resolve_crop
 from .sampler import VALIDATE
 
 RAY_BATCH_SIZE = 8192          # ExpRunner.cpp:268
@@ -36,13 +37,19 @@ def _to_dev(x, dev):
     return (x.contiguous().pin_memory() if torch.cuda.is_available() else x).to(dev, non_blocking=True)
 
 
-def _render_rays(renderer, o, d, ray_batch_size, dev, app=None):
+def _render_rays(renderer, o, d, ray_batch_size, dev, app=None, crop=None, bg=None):
     """The tiled VALIDATE-mode render of one image's rays (device [N,3] each) -> device (colors [N,3], first_oct_disp [N,1],
     pred_disp [N,1]), normalised as ExpRunner.cpp:289-290.  No host sync on the fused path.  The caller sets VALIDATE mode.
-    ``app``: an appearance row [16] (``Renderer.appearance_row``) for every ray; only the fused kernel shades with one."""
+    ``app``: an appearance row [16] (``Renderer.appearance_row``) for every ray; ``crop``: a ``Crop``; ``bg``: a background
+    colour [3] in place of the renderer's own.  Only the fused kernel renders with any of them."""
     n_rays = d.shape[0]
-    if app is not None and not renderer._fused_forward_ok(n_rays) and n_rays > 0:
-        raise RuntimeError("appearance: rendering with an appearance row needs the fused forward (F2B_FUSED_FORWARD=1)")
+    if not renderer._fused_forward_ok(n_rays) and n_rays > 0:
+        if app is not None:
+            raise RuntimeError("appearance: rendering with an appearance row needs the fused forward (F2B_FUSED_FORWARD=1)")
+        if crop is not None:
+            raise RuntimeError("crop: rendering with a crop box needs the fused forward (F2B_FUSED_FORWARD=1)")
+        if bg is not None:
+            raise RuntimeError("background: rendering on a given background needs the fused forward (F2B_FUSED_FORWARD=1)")
     colors = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
     first = torch.full((n_rays, 1), 1., dtype=torch.float32, device=dev)
     disp = torch.zeros((n_rays, 1), dtype=torch.float32, device=dev)
@@ -63,7 +70,8 @@ def _render_rays(renderer, o, d, ray_batch_size, dev, app=None):
             if k < 2:
                 st.wait_event(ready)
             with torch.cuda.stream(st):
-                r = renderer.render_forward(o[i:j], d[i:j], out=(colors[i:j], disp_flat[i:j], depth[i:j]), lane=1 + k % 2, app=app)
+                r = renderer.render_forward(o[i:j], d[i:j], out=(colors[i:j], disp_flat[i:j], depth[i:j]), lane=1 + k % 2, bg=bg,
+                                            app=app, crop=crop)
                 first[i:j] = r.first_oct_dis.reshape(-1, 1)
             alive.append(r)                                  # allocations of a lane stay referenced until the join below
         for st in lanes:
@@ -106,24 +114,37 @@ def _device_of(renderer, device):
     return torch.device(device) if device is not None else renderer.app_emb_.device
 
 
+def _background(background, dev):
+    """A background colour [3] as a float32 device tensor, or None (the renderer's own)."""
+    if background is None:
+        return None
+    bg = torch.as_tensor(background, dtype=torch.float32).reshape(-1)
+    if bg.shape != (3,):
+        raise ValueError(f"background: a colour has 3 entries, got {bg.numel()}")
+    return bg.to(dev)
+
+
 @torch.no_grad()
-def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
+def RenderWholeImage(renderer, rays_o, rays_d, bounds=None, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None, crop=None,
+                     background=None):
     """-> (pred_colors [N,3], first_oct_disp [N,1], pred_disp [N,1]) CPU float32, like the reference.
     ``rays_o`` / ``rays_d``: [N,3] CPU or CUDA tensors; ``bounds`` is accepted and ignored (the sampler marches
     [global_near_, 1e8], PersSampler.cu:322-323).  ``appearance``: None, a training image's index or a [16] row
-    (``Renderer.appearance_row``, DESIGN.md §3m)."""
+    (``Renderer.appearance_row``, DESIGN.md §3m).  ``crop``: a ``Crop`` (DESIGN.md §3n): what its box does not keep is empty
+    space.  ``background``: a colour [3] in place of the renderer's own (e.g. white or black to isolate a cropped object)."""
     dev = _device_of(renderer, device)
-    app = resolve_appearance(renderer, appearance)
+    app, crop, bg = resolve_appearance(renderer, appearance), resolve_crop(crop), _background(background, dev)
     with _Validate(renderer):
-        colors, first, disp = _render_rays(renderer, _to_dev(rays_o, dev), _to_dev(rays_d, dev), ray_batch_size, dev, app)
+        colors, first, disp = _render_rays(renderer, _to_dev(rays_o, dev), _to_dev(rays_d, dev), ray_batch_size, dev, app, crop, bg)
     out = torch.cat([colors, first, disp], 1).cpu()              # the one device->host copy
     return out[:, :3].contiguous(), out[:, 3:4].contiguous(), out[:, 4:5].contiguous()
 
 
-def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None, app=None):
+def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None, app=None, crop=None):
     """The tiled VALIDATE loop of ``RenderWholeImage`` with a kernel behind every chunk: ``render_forward`` of rays [i, j) on one of
     two lane streams, then ``each(result, i, j)`` on the same stream, over the chunk's slots.  ``out`` = (colors [N,3], disparity [N],
-    depth [N]) to write into, else per-lane scratch; ``bg`` / ``app``: render_forward's background override and appearance row.
+    depth [N]) to write into, else per-lane scratch; ``bg`` / ``app`` / ``crop``: render_forward's background override, appearance
+    row and crop box.
     No host sync; the lanes are joined to the current stream at the end.  The caller sets VALIDATE mode."""
     n_rays = d.shape[0]
     main = torch.cuda.current_stream(dev)
@@ -141,7 +162,7 @@ def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None, a
             st.wait_event(ready)
         with torch.cuda.stream(st):
             dst = tuple(u[:j - i] for u in unused[k % 2]) if out is None else tuple(u[i:j] for u in out)
-            r = renderer.render_forward(o[i:j], d[i:j], out=dst, lane=1 + k % 2, bg=bg, app=app)
+            r = renderer.render_forward(o[i:j], d[i:j], out=dst, lane=1 + k % 2, bg=bg, app=app, crop=crop)
             each(r, i, j)
         alive.append(r)                                      # allocations of a lane stay referenced until the join below
     for st in lanes:
@@ -150,16 +171,17 @@ def _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=None, bg=None, a
 
 
 @torch.no_grad()
-def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None, crop=None):
     """-> normals [N,3] CPU float32: the normal map of the rays in the normalised scene frame (DESIGN.md §3j).  Per ray,
     N = sum_i w_i n_i over the samples the VALIDATE render keeps, with n_i = -g_i / |g_i| the outward density normal and w_i the
     render's weights; the result is N / |N|, 0 where N = 0 (rays that miss the scene included).  The rays are rendered in the
     tiled loop of ``RenderWholeImage`` (two streams, ``render_forward`` per chunk), each chunk followed on its stream by the
     normals kernel over the chunk's slots; one device->host copy at the end.  The sums run in a fixed order, so a view gets the
     same bits on every run and for any ``ray_batch_size``.  Turning the map into camera coordinates is one rotation by the
-    camera's pose, left to the caller."""
+    camera's pose, left to the caller.  ``crop``: a ``Crop``; the weights are the cropped render's (DESIGN.md §3n)."""
     from . import ops
     dev = _device_of(renderer, device)
+    crop = resolve_crop(crop)
     o, d = _to_dev(rays_o, dev), _to_dev(rays_d, dev)
     n_rays = d.shape[0]
     normals = torch.zeros((n_rays, 3), dtype=torch.float32, device=dev)
@@ -173,21 +195,23 @@ def RenderNormals(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, devic
                                  r._keep[0], r.kept_counts, r._w_slots, out=normals[i:j])
 
     with _Validate(renderer):
-        _slot_chunks(renderer, o, d, ray_batch_size, dev, each)
+        _slot_chunks(renderer, o, d, ray_batch_size, dev, each, crop=crop)
     return normals.cpu()                                         # the one device->host copy
 
 
 @torch.no_grad()
-def RenderDepth(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None):
+def RenderDepth(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=None, crop=None):
     """-> (opacity [N], median_depth [N], depth [N]) CPU float32, in normalised scene units along the unit ray direction (times
     ``dataset.radius_`` for data units; DESIGN.md §3l).  Per ray, over the samples the VALIDATE render keeps, with w_i the render's
     weights: opacity W = sum_i w_i (fp32, serially in sample order); median_depth = t_m of the first sample m whose running sum
     reaches W / 2 (a sample's own t: no interpolation, no offset); 0 for both where W = 0 (rays that miss included).  ``depth`` is
     the renderer's own expectation sum_i w_i (t_i + 0.01) / (1 - T + 1e-4), bit for bit.  The rays are rendered in the tiled loop
     of ``RenderNormals``, each chunk followed on its stream by the termination kernel over the chunk's slots; one device->host
-    copy at the end.  The same bits on every run and for any ``ray_batch_size``."""
+    copy at the end.  The same bits on every run and for any ``ray_batch_size``.  ``crop``: a ``Crop``; the weights are the
+    cropped render's, so a pixel sees only what the box keeps (DESIGN.md §3n)."""
     from . import ops
     dev = _device_of(renderer, device)
+    crop = resolve_crop(crop)
     o, d = _to_dev(rays_o, dev), _to_dev(rays_d, dev)
     n_rays = d.shape[0]
     res = torch.zeros((3, n_rays), dtype=torch.float32, device=dev)          # opacity, median depth, depth
@@ -199,7 +223,7 @@ def RenderDepth(renderer, rays_o, rays_d, ray_batch_size=RAY_BATCH_SIZE, device=
         ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=res[0, i:j], median_t=res[1, i:j])
 
     with _Validate(renderer):
-        _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=(colors, disp, res[2]))
+        _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=(colors, disp, res[2]), crop=crop)
     return tuple(res.cpu())                                      # the one device->host copy
 
 
@@ -319,32 +343,36 @@ def path_rows(renderer, appearance, n_frames):
 
 
 @torch.no_grad()
-def RenderPath(renderer, dataset, reso_level=1, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
+def RenderPath(renderer, dataset, reso_level=1, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None, crop=None,
+               background=None):
     """ExpRunner::RenderPath (ExpRunner.cpp:322-341) over ``dataset.render_poses_`` -> list of device tuples
     (colors [h,w,3], first_oct_dis [h,w,1], disparity [h,w,1]) with h, w = height // reso_level, width // reso_level.
     ``appearance``: None, a training image's index or a [16] row for every frame, or a [F,16] tensor with one row per frame
-    (``path_rows``)."""
+    (``path_rows``).  ``crop`` / ``background``: as ``RenderWholeImage``, for every frame."""
     if dataset.render_poses_ is None:
         raise ValueError("RenderPath: the dataset has no render_poses")
     dev = _device_of(renderer, device)
+    crop, bg = resolve_crop(crop), _background(background, dev)
     h, w = dataset.height_ // int(reso_level), dataset.width_ // int(reso_level)
     apps = path_rows(renderer, appearance, len(dataset.render_poses_))
     frames = []
     with _Validate(renderer):
         for pose, app in zip(dataset.render_poses_, apps):
             rays_o, rays_d, _ = dataset.RaysFromPose(pose, reso_level)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app)
+            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app, crop, bg)
             frames.append((colors.reshape(h, w, 3), first.reshape(h, w, 1), disp.reshape(h, w, 1)))
     return frames
 
 
 @torch.no_grad()
-def RenderAllImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None):
+def RenderAllImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None, crop=None, background=None):
     """ExpRunner::RenderAllImages / VisualizeImage (ExpRunner.cpp:295-320): for every camera the device image
     cat([GT | pred | first_oct_dis x3 | disparity x3], width) [H, 4W, 3] (GT zeros when the dataset holds no images).
     ``appearance``: None, a training image's index or a [16] row for every camera, or ``"own"``: each camera with its own row,
-    as its photo was trained (a camera outside the training set has an untrained row)."""
+    as its photo was trained (a camera outside the training set has an untrained row).  ``crop`` / ``background``: as
+    ``RenderWholeImage``, for every camera."""
     dev = _device_of(renderer, device)
+    crop, bg = resolve_crop(crop), _background(background, dev)
     H, W = dataset.height_, dataset.width_
     images = []
     resolve_appearance(renderer, appearance, view=0)             # argument errors before any rendering
@@ -352,7 +380,7 @@ def RenderAllImages(renderer, dataset, ray_batch_size=RAY_BATCH_SIZE, device=Non
         for idx in range(dataset.n_images_):
             rays_o, rays_d, _ = dataset.RaysOfCamera(idx)
             app = resolve_appearance(renderer, appearance, view=idx)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app)
+            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app, crop, bg)
             gt = (dataset.image_tensors_[idx].reshape(H, W, 3) if dataset.image_tensors_ is not None
                   else torch.zeros((H, W, 3), dtype=torch.float32, device=dev))
             images.append(torch.cat([gt, colors.reshape(H, W, 3), first.reshape(H, W, 1).expand(H, W, 3),

@@ -17,6 +17,9 @@ A point cloud (DESIGN.md §3l) samples the surface where the views see it rather
 unbounded scene near and far: ``ExtractPointCloud`` renders every view on a grid, puts a point at each opaque pixel's median
 sample (``eval.RenderDepth``'s termination kernel), coloured by the pixel's foreground colour, and keeps the points whose depth
 the other views confirm (``f2b_depth_consistency``).
+
+A crop box (``crop.Crop``, DESIGN.md §3n) restricts the lattice, the mesh and the point cloud to what the box keeps: lattice points
+it does not keep read ``EMPTY_LOGIT``, so the mesh stays closed and caps the cut, and the point cloud's renders are cropped.
 """
 import math
 from typing import NamedTuple, Optional
@@ -26,12 +29,14 @@ import torch
 
 from . import ops
 from ._lib import call, stream
+from .crop import resolve_crop
 from .eval import resolve_appearance
 from .octree_build import TREE_NODE
 
 EMPTY_LOGIT = -1e4          # logit of a point outside every valid leaf: finite, and exp(EMPTY_LOGIT - 3) == 0 in fp32
 SLAB_POINTS = 1 << 23       # Isosurface: owner points per z-slab; scratch <= 25 B x (SLAB_POINTS + one layer), ~210 MB
 GRID_SLAB_POINTS = 1 << 30  # DensityGrid: lattice points per kernel launch (the kernel indexes a slab with int32)
+CROP_MASK_POINTS = 1 << 24  # DensityGrid(crop=): lattice points masked per f2b_crop_mask launch (12 B of points each)
 
 
 class Grid(NamedTuple):
@@ -162,11 +167,34 @@ def leaf_bounds(renderer):
     return tuple(float(x) for x in (c - h).min(0)), tuple(float(x) for x in (c + h).max(0))
 
 
-def DensityGrid(renderer, bbox_min=None, bbox_max=None, reso=256):
+def _crop_lattice(crop, logit, origin, voxel, z0):
+    """Lattice layers [z0, z0 + nz) of ``logit`` [nz, ny, nx] read ``EMPTY_LOGIT`` where ``crop`` does not keep the lattice point
+    origin + voxel * (i, j, k), formed as the grid kernel forms it: fadd(origin, fmul(voxel, i)) per axis (one fp32 op each)."""
+    nz, ny, nx = logit.shape
+    dev = logit.device
+    o = [torch.tensor(float(x), dtype=torch.float32, device=dev) for x in origin]
+    v = [torch.tensor(float(x), dtype=torch.float32, device=dev) for x in voxel]
+    axis = lambda a, n, i0: o[a] + v[a] * torch.arange(i0, i0 + n, dtype=torch.float32, device=dev)
+    xs, ys = axis(0, nx, 0), axis(1, ny, 0)
+    layers = max(1, CROP_MASK_POINTS // (nx * ny))
+    for k0 in range(0, nz, layers):
+        n = min(layers, nz - k0)
+        zs = axis(2, n, z0 + k0)
+        pts = torch.stack([xs.expand(n, ny, nx), ys[:, None].expand(n, ny, nx), zs[:, None, None].expand(n, ny, nx)], -1)
+        logit[k0:k0 + n].masked_fill_(~crop.mask(pts).view(n, ny, nx), EMPTY_LOGIT)
+
+
+def DensityGrid(renderer, bbox_min=None, bbox_max=None, reso=256, crop=None):
     """The density logit on a lattice over the box [bbox_min, bbox_max] (default: ``leaf_bounds``) with cubic voxels, ``reso``
-    points along the box's longest axis -> ``Grid``.  The lattice points are generated in the kernel, in z-slabs."""
+    points along the box's longest axis -> ``Grid``.  The lattice points are generated in the kernel, in z-slabs.
+    ``crop``: a ``Crop``; lattice points it does not keep read ``EMPTY_LOGIT`` (its predicate, ``f2b_crop_mask``, over each slab's
+    points), and when the box is not given and the crop is not inverted it defaults to ``crop.aabb()`` within ``leaf_bounds``."""
+    crop = resolve_crop(crop)
     if bbox_min is None or bbox_max is None:
         lo, hi = leaf_bounds(renderer)
+        if crop is not None and not crop.invert:
+            clo, chi = crop.aabb()
+            lo, hi = tuple(max(a, b) for a, b in zip(lo, clo)), tuple(min(a, b) for a, b in zip(hi, chi))
         bbox_min = lo if bbox_min is None else bbox_min
         bbox_max = hi if bbox_max is None else bbox_max
     lo, hi = np.asarray(bbox_min, np.float64).reshape(3), np.asarray(bbox_max, np.float64).reshape(3)
@@ -183,6 +211,8 @@ def DensityGrid(renderer, bbox_min=None, bbox_max=None, reso=256):
     for z0 in range(0, nz, step):
         n = min(step, nz - z0)
         ops.query_logit_grid(nodes, trans, *fargs, origin, (voxel,) * 3, nx, ny, z0, n, EMPTY_LOGIT, logit[z0:z0 + n])
+        if crop is not None:
+            _crop_lattice(crop, logit[z0:z0 + n], origin, (voxel,) * 3, z0)
     return Grid(logit, origin, (voxel,) * 3)
 
 
@@ -252,15 +282,16 @@ def VertexColors(renderer, verts, faces, normals=None, appearance=None):
 
 
 def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, density=None, colors=True, normals=False,
-                appearance=None):
+                appearance=None, crop=None):
     """The scene's surface as a ``Mesh`` on the device, in the normalised frame (``Mesh.to_data_frame`` maps it back).
     The level is the density that reaches opacity ``alpha`` over one VALIDATE march step (``level_from_alpha``), or
     ``density`` (per warp unit) when given; the lattice is ``DensityGrid(renderer, bbox_min, bbox_max, reso)``.
     ``normals``: the vertices get the field's normals (``QueryNormal``), and the colours are seen along them (the face normal
-    where the field normal is 0).  ``appearance``: the colours' appearance row, as ``QueryColor``."""
+    where the field normal is 0).  ``appearance``: the colours' appearance row, as ``QueryColor``.  ``crop``: a ``Crop``
+    (``DensityGrid``): the surface of what the box keeps, closed where the box cuts it."""
     app = resolve_appearance(renderer, appearance)               # argument errors before the lattice is built
     level = math.log(float(density)) + 3. if density is not None else level_from_alpha(renderer, alpha)
-    g = DensityGrid(renderer, bbox_min, bbox_max, reso)
+    g = DensityGrid(renderer, bbox_min, bbox_max, reso, crop)
     verts, faces = Isosurface(g.logit, level, g.origin, g.voxel)
     del g
     nrm = QueryNormal(renderer, verts) if normals else None
@@ -269,7 +300,7 @@ def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, den
 
 
 def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0.9, min_views=2, rel_tol=0.01, normals=False,
-                      appearance=None):
+                      appearance=None, crop=None):
     """The scene's surface as a coloured ``PointCloud`` on the device, in the normalised frame (``to_data_frame`` maps it back).
     Pass 1, per view of ``views`` (default ``dataset.train_set_``): the VALIDATE render of the view's own camera on the
     (height // reso_level) x (width // reso_level) grid, with a black background, and the termination kernel on its slots (as
@@ -280,8 +311,10 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
     whose median depth is within ``rel_tol`` of the point's distance.  Points are ordered by (position of the view in ``views``,
     cell); a run gives the same bits every time.  One host sync per view.  ``appearance`` colours the points
     (``Renderer.appearance_row``): None, a training image's index, a [16] row, or ``"own"``: each view's own row.  The points
-    themselves do not depend on it (weights and density do not)."""
+    themselves do not depend on it (weights and density do not).  ``crop``: a ``Crop``; every render is cropped (DESIGN.md §3n), so
+    the candidates and the consistency pass see only what the box keeps."""
     from .eval import RAY_BATCH_SIZE, _slot_chunks, _Validate
+    crop = resolve_crop(crop)
     views = [int(v) for v in (dataset.train_set_ if views is None else views)]
     reso_level, min_views = int(reso_level), int(min_views)
     if not views:
@@ -318,7 +351,7 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
                     ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
                                              f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=nm[i:j])
 
-            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black, app=app)
+            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black, app=app, crop=crop)
             cell = torch.nonzero(opa >= float(min_opacity)).squeeze(1)            # the host sync of the view; cells ascending
             maps.append((opa, med))
             pts.append(point[cell])

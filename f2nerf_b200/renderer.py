@@ -18,6 +18,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import call, stream
+from .crop import resolve_crop
 from .rng import burn_mlp_output, burn_rand
 from .sampler import TRAIN, LazySampleResult
 
@@ -297,7 +298,7 @@ class Renderer:
             raise ValueError(f"appearance: a row has 16 entries, got shape {tuple(row.shape)}")
         return row.detach().to(device=self.app_emb_.device, dtype=torch.float32).contiguous()
 
-    def render_forward(self, rays_o, rays_d, out=None, lane=0, bg=None, app=None):
+    def render_forward(self, rays_o, rays_d, out=None, lane=0, bg=None, app=None, crop=None):
         """Renderer::Render (Renderer.cpp:52-213) for a batch that takes no gradient (VALIDATE mode): the march, then hash encode
         -> field MLP -> early stop -> SH + shader MLP -> composite in ONE kernel that walks each ray front to back and stops at
         the first opaque sample (csrc/fused_fwd.cu).  No host sync, no per-sample tensor in HBM; values bit-identical to the
@@ -305,7 +306,8 @@ class Renderer:
         its image buffers directly); ``lane`` > 0 uses that extra scratch set so two chunks can be in flight on two streams.
         ``bg``: a background colour [3] or [R,3] in place of the renderer's own; with a zero background the colour is exactly the
         composite sum_i w_i c_i of the kept samples.  ``app``: an appearance row [16] (``appearance_row``) added to every ray's
-        shader input (``f2b_render_fwd_fused_app``); None shades without one.
+        shader input (``f2b_render_fwd_fused_app``); None shades without one.  ``crop``: a ``crop.Crop``; samples whose world point
+        fma(t, d, o) it does not keep get density 0 (``f2b_render_fwd_fused_crop``, DESIGN.md §3n); None renders the whole scene.
         Not reproduced: the reference's torch::rand draws for the MLP outputs (rng.py) — their sizes would need the host sync."""
         field, shader, sampler = self.scene_field_, self.shader_, self.pts_sampler_
         n_rays, dev = rays_o.shape[0], rays_o.device
@@ -331,15 +333,20 @@ class Renderer:
             args = (table16, field.prim_pool_, field.bias_pool_, int(field.n_volumes_), int(field.local_size_), fparams16, sparams16,
                     slots.s_pts, slots.s_dt, slots.s_t, slots.s_anchors, slots.counts, slots.rays_d, bg, n_rays, S, slots.totals, ticket,
                     colors, disparity, depth, kept, w_slots)
-            if app is None:
+            if app is not None and (app.shape != (16,) or app.dtype != torch.float32 or not app.is_contiguous()
+                                    or app.device != torch.device(dev)):
+                raise ValueError("render_forward: app must be a contiguous float32 [16] row on the rays' device")
+            box = None
+            if crop is not None:
+                box = resolve_crop(crop).box12()
+                call("f2b_render_fwd_fused_crop", *args, app, slots.rays_o, box.ctypes.data, int(crop.invert), stream())
+            elif app is None:
                 call("f2b_render_fwd_fused", *args, stream())
             else:
-                if app.shape != (16,) or app.dtype != torch.float32 or not app.is_contiguous() or app.device != torch.device(dev):
-                    raise ValueError("render_forward: app must be a contiguous float32 [16] row on the rays' device")
                 call("f2b_render_fwd_fused_app", *args, app, stream())
         res = ForwardRenderResult(colors, slots.first_oct_dis, disparity, depth, kept, w_slots, S, self, (lane, stamps[lane]),
                                   slots.totals)
-        res._keep = (slots, table16, fparams16, sparams16, bg, ticket, app)     # alive until the result dies (stream-ordered reuse)
+        res._keep = (slots, table16, fparams16, sparams16, bg, ticket, app, box)  # alive until the result dies (stream-ordered reuse)
         return res
 
     def set_next_rays(self, rays_o, rays_d):

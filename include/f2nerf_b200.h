@@ -539,6 +539,26 @@ int f2b_render_fwd_fused_app(const void* table_f16, const int* prim_pool, const 
                              const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all, int* ticket,
                              float* colors, float* disparity, float* depth, int* kept_counts, float* weights_slots,
                              const float* app_emb /* [16] */, void* stream);
+/* Crop boxes (DESIGN.md §3n).  box12: host array, the 3x4 fp32 matrix box_from_scene M, row-major, mapping the normalised scene
+ * frame to the box's frame.  A point p is inside when |b_k| <= 1 for k = 0, 1, 2, with
+ * b_k = fma(M[k][0], x, fma(M[k][1], y, fma(M[k][2], z, M[k][3]))) in this fp32 order (a NaN point is not inside), and it is
+ * kept when it is inside, or, with invert != 0, when it is not.
+ * f2b_render_fwd_fused_crop: f2b_render_fwd_fused (app_emb NULL) or f2b_render_fwd_fused_app (app_emb [16], device) where every
+ * sample whose world point fma(slot_t, rays_d, rays_o) (per component, as f2b_ray_termination_slots forms it; rays_o [R,3] the
+ * march's origins, slot_pts being warped coordinates) the box does not keep has density 0: tau, alpha and its weight are +0, it
+ * is not encoded, and it still counts towards the kept prefix (T > 1e-4).  Colours, disparity and depth are bit-identical to the uncropped entry over
+ * the slot layout with the removed samples deleted (the same total_all); weights_slots holds those weights at the kept-by-crop
+ * slots and +0 at the other kept slots.  The background, the march and total_all are unchanged. */
+int f2b_render_fwd_fused_crop(const void* table_f16, const int* prim_pool, const float* bias_pool, int n_volumes, int local_size,
+                              const void* field_params_f16, const void* shader_params_f16, const float* slot_pts,
+                              const float* slot_dt, const float* slot_t, const int* slot_anchors, const int* ray_counts,
+                              const float* rays_d, const float* bg, int n_rays, int slot_size, const int* total_all, int* ticket,
+                              float* colors, float* disparity, float* depth, int* kept_counts, float* weights_slots,
+                              const float* app_emb /* [16] or NULL */, const float* rays_o /* [R,3] */,
+                              const float* box12 /* host, 12 floats */, int invert, void* stream);
+/* kept[i] = 1 when the box keeps pts[i] (the predicate above, the same device function as the render's), else 0. */
+int f2b_crop_mask(const float* pts /* [n,3] */, int n, const float* box12 /* host, 12 floats */, int invert,
+                  uint8_t* kept /* [n] */, void* stream);
 /* weights_slots [R*slot] + new_bounds [R,2] (f2b_count_scan of kept_counts) -> weights [P'] in the packed ray order. */
 int f2b_gather_kept_weights(const float* weights_slots, const int* new_bounds, int n_rays, int slot_size, float* weights,
                             void* stream);

@@ -1,10 +1,11 @@
 """Extract a trained scene's surface as a coloured PLY mesh on the device.
 
     python scripts/extract_mesh.py <runtime_config.yaml> <checkpoint_dir> [--reso 512] [--alpha 0.5]
-                                   [--bbox x0 y0 z0 x1 y1 z1] --out scene.ply
+                                   [--bbox x0 y0 z0 x1 y1 z1] [--crop x0 y0 z0 x1 y1 z1 [--crop-invert]] --out scene.ply
 
 load_scene -> DensityGrid -> Isosurface -> VertexColors (f2nerf_b200/geometry.py); the mesh is written in the data's own world
-frame (Mesh.to_data_frame).  --bbox is in the normalised scene frame (default: the valid leaves' bounding box).  Prints one
+frame (Mesh.to_data_frame).  --bbox is in the normalised scene frame (default: the valid leaves' bounding box, or with --crop
+the crop box within it).  --crop keeps only what an axis-aligned box of the scene frame holds (DESIGN.md §3n).  Prints one
 JSON line: lattice size, grid-query time and rate, extraction time, colour time, vertex and face counts, and the GPU.
 """
 import argparse
@@ -25,16 +26,20 @@ def main(argv=None):
     ap.add_argument("--alpha", type=float, default=0.5)
     ap.add_argument("--bbox", type=float, nargs=6, default=None)
     ap.add_argument("--out", required=True)
+    ap.add_argument("--crop", type=float, nargs=6, default=None, metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"),
+                    help="keep only the axis-aligned box [x0, x1] x [y0, y1] x [z0, z1] of the normalised scene frame")
+    ap.add_argument("--crop-invert", action="store_true", help="keep everything but the --crop box")
     ap.add_argument("--normals", action="store_true", help="field normals on the vertices (written as nx ny nz; colours seen along them)")
     ap.add_argument("--repeat", type=int, default=1, help="time the grid query and the extraction this many times (median)")
     a = ap.parse_args(argv)
 
     import torch
-    from f2nerf_b200 import geometry as G, load_scene
+    from f2nerf_b200 import Crop, geometry as G, load_scene
 
     scene = load_scene(a.config, a.checkpoint_dir, device="cuda")
     r = scene.renderer
     lo, hi = (a.bbox[:3], a.bbox[3:]) if a.bbox else (None, None)
+    crop = Crop.box(a.crop[:3], a.crop[3:], invert=a.crop_invert) if a.crop else None
     level = G.level_from_alpha(r, a.alpha)
 
     def timed(fn):
@@ -44,8 +49,8 @@ def main(argv=None):
         torch.cuda.synchronize()
         return out, time.perf_counter() - t0
 
-    G.DensityGrid(r, lo, hi, reso=16)                                # warm-up: module load, shadow table, allocator
-    grids, t_grid = zip(*(timed(lambda: G.DensityGrid(r, lo, hi, reso=a.reso)) for _ in range(a.repeat)))
+    G.DensityGrid(r, lo, hi, reso=16, crop=crop)                                # warm-up: module load, shadow table, allocator
+    grids, t_grid = zip(*(timed(lambda: G.DensityGrid(r, lo, hi, reso=a.reso, crop=crop)) for _ in range(a.repeat)))
     g = grids[-1]
     del grids
     meshes, t_iso = zip(*(timed(lambda: G.Isosurface(g.logit, level, g.origin, g.voxel)) for _ in range(a.repeat)))
@@ -59,7 +64,7 @@ def main(argv=None):
     G.write_ply(a.out, mesh)
     med = lambda x: sorted(x)[len(x) // 2]
     props = torch.cuda.get_device_properties(0)
-    print(json.dumps(dict(reso=a.reso, alpha=a.alpha, level=level, lattice_points=n_pts, grid_query_s=med(t_grid),
+    print(json.dumps(dict(reso=a.reso, alpha=a.alpha, crop=a.crop, crop_invert=a.crop_invert, level=level, lattice_points=n_pts, grid_query_s=med(t_grid),
                           grid_points_per_s=n_pts / med(t_grid), extract_s=med(t_iso), colors_s=t_col, normals_s=t_nrm, verts=int(verts.shape[0]),
                           faces=int(faces.shape[0]), gpu=props.name, out=a.out)))
 

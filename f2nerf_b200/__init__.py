@@ -11,8 +11,9 @@ from .crop import Crop
 from .checkpoint import Scene, gradient_scaling_progress, load_scene, load_states
 from .dataset import RayGenerator, load_dataset
 from .octree_build import build_edge_pool, build_tree_nodes, initial_octree
-from .eval import ImageMetrics, RenderAllImages, RenderDepth, RenderNormals, RenderPath, RenderWholeImage, TestImages
+from .eval import ImageMetrics, RenderAllImages, RenderDepth, RenderLens, RenderNormals, RenderPath, RenderWholeImage, TestImages
 from .field import Hash3DAnchored, TCNNWP
+from .lens import Lens, level_pose
 from .ops import CustomOps, FlexOps
 from .optim import FusedAdam
 from .pose import RayGradient, RefinePose
@@ -20,6 +21,6 @@ from .renderer import Renderer, RenderResult, check_backward_nan
 from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultFlex
 from .shader import SHShader
 
-__all__ = ["Crop", "FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
+__all__ = ["Crop", "Lens", "level_pose", "RenderLens", "FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
            "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderDepth", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

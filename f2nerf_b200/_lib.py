@@ -85,6 +85,7 @@ SIGNATURES = {
     "f2b_octree_mark_invisible": [_P, c_int, _P, _P, _P, c_int, _P],
     "f2b_img2world_rays": [_P, _P, _P, _P, _P, c_int, _P, _P, _P],
     "f2b_camera_rays": [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P],
+    "f2b_lens_rays": [c_int, _P, c_int, c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double, _P, _P, _P, _P],
     "f2b_gather_pixels": [_P, _P, _P, c_int, c_int, c_int, _P, _P],
     "f2b_image_metrics": [_P, _P, c_int, c_int, _P, _P, _P, _P, _P],
     "f2b_adam_step": [_P, _P, _P, _P, c_i64, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,

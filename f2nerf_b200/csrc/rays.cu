@@ -105,9 +105,98 @@ gather_pixels_kernel(int n, const float* __restrict__ images, const int* __restr
   out[size_t(r) * 3 + 2] = __ldg(images + px * 3 + 2);
 }
 
+// Lens rays (DESIGN.md §3o).  Angles are carried in half-turns so that sincospi never rounds pi; everything up to the stores is
+// float64, with the fmas written out, and each output is rounded to fp32 once.  The equirectangular directions are one function
+// that the ODS model calls with the same arguments, so ODS at ipd 0 reproduces them bit for bit.
+__device__ __forceinline__ void equirect_dir(int a, int b, int height, int width, double hfov, double vfov, double& x, double& y,
+                                             double& z, double& sin_lam, double& cos_lam) {
+  const double lam = __ddiv_rn(__dmul_rn(hfov, double(2 * b + 1 - width)), __dmul_rn(360., double(width)));    // half-turns
+  const double phi = __ddiv_rn(__dmul_rn(vfov, double(height - 2 * a - 1)), __dmul_rn(360., double(height)));
+  double sin_phi, cos_phi;
+  sincospi(lam, &sin_lam, &cos_lam);
+  sincospi(phi, &sin_phi, &cos_phi);
+  x = __dmul_rn(cos_phi, sin_lam);
+  y = sin_phi;
+  z = -__dmul_rn(cos_phi, cos_lam);
+}
+
+template <int Model>
+__global__ void __launch_bounds__(128)
+lens_rays_kernel(int n, int height, int width, double p0, double p1, double p2, const float* __restrict__ pose,
+                 float* __restrict__ rays_o, float* __restrict__ rays_d, uint8_t* __restrict__ valid) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const int hw = height * width;
+  const int eye = Model == F2B_LENS_ODS ? r / hw : 0;                 // ODS: 0 = left (top half), 1 = right
+  const int q = r - eye * hw;
+  const int a = q / width, b = q - a * width;
+  double x, y, z, sin_lam = 0., cos_lam = 1.;
+  bool ok = true;
+  if (Model == F2B_LENS_FISHEYE) {
+    // twice the pixel offset, an integer: the circle test r <= min(H, W) / 2 (theta <= fov / 2) is exact
+    const int64_t X = 2 * int64_t(b) + 1 - width, Y = 2 * int64_t(a) + 1 - height, m = height < width ? height : width;
+    ok = uint64_t(X * X) + uint64_t(Y * Y) <= uint64_t(m * m);
+    const double px = 0.5 * double(X), py = 0.5 * double(Y);
+    const double rad = sqrt(__fma_rn(px, px, __dmul_rn(py, py)));
+    if (rad == 0.) {
+      x = 0.; y = 0.; z = -1.;
+    } else {
+      double s, c;
+      sincospi(__ddiv_rn(__dmul_rn(rad, p0), __dmul_rn(180., double(m))), &s, &c);   // theta = r / f in half-turns
+      x = __dmul_rn(s, __ddiv_rn(px, rad));
+      y = -__dmul_rn(s, __ddiv_rn(py, rad));
+      z = -c;
+    }
+  } else {
+    equirect_dir(a, b, height, width, p0, p1, x, y, z, sin_lam, cos_lam);
+  }
+  double off[3] = {0., 0., 0.};
+  if (Model == F2B_LENS_ODS) {
+    const double h = eye ? 0.5 * p2 : -0.5 * p2;                      // s ipd / 2, the eye on the viewing circle
+    off[0] = __dmul_rn(h, cos_lam);
+    off[2] = __dmul_rn(h, sin_lam);
+  }
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const double r0 = __ldg(pose + 4 * k), r1 = __ldg(pose + 4 * k + 1), r2 = __ldg(pose + 4 * k + 2);
+    const double t = __ldg(pose + 4 * k + 3);
+    const double d = __fma_rn(r0, x, __fma_rn(r1, y, __dmul_rn(r2, z)));
+    rays_d[size_t(r) * 3 + k] = ok ? __double2float_rn(d) : 0.f;
+    rays_o[size_t(r) * 3 + k] =
+        Model == F2B_LENS_ODS && p2 != 0. ? __double2float_rn(__dadd_rn(t, __fma_rn(r0, off[0], __dmul_rn(r2, off[2])))) : float(t);
+  }
+  valid[r] = ok;
+}
+
 }  // namespace f2b
 
 using namespace f2b;
+
+extern "C" int f2b_lens_rays(int model, const float* pose, int height, int width, double p0, double p1, double p2,
+                             float* rays_o, float* rays_d, uint8_t* valid, void* stream) {
+  F2B_REQUIRE(pose && rays_o && rays_d && valid, "f2b_lens_rays: null pointer");
+  F2B_REQUIRE(model == F2B_LENS_EQUIRECT || model == F2B_LENS_FISHEYE || model == F2B_LENS_ODS, "f2b_lens_rays: unknown model %d",
+              model);
+  F2B_REQUIRE(height >= 1 && width >= 1, "f2b_lens_rays: size %dx%d", height, width);
+  const int64_t n = int64_t(model == F2B_LENS_ODS ? 2 : 1) * height * width;
+  F2B_REQUIRE(n < (int64_t(1) << 31), "f2b_lens_rays: %lld rays overflow int32", (long long)n);
+  if (model == F2B_LENS_FISHEYE) {
+    F2B_REQUIRE(isfinite(p0) && p0 > 0. && p0 <= 360., "f2b_lens_rays: fisheye fov %g outside (0, 360]", p0);
+  } else {
+    F2B_REQUIRE(isfinite(p0) && p0 > 0. && p0 <= 360., "f2b_lens_rays: hfov %g outside (0, 360]", p0);
+    F2B_REQUIRE(isfinite(p1) && p1 > 0. && p1 <= 180., "f2b_lens_rays: vfov %g outside (0, 180]", p1);
+  }
+  if (model == F2B_LENS_ODS) F2B_REQUIRE(isfinite(p2) && p2 >= 0., "f2b_lens_rays: ipd %g must be finite and >= 0", p2);
+  const int grid = div_up(n, 128);
+  cudaStream_t st = as_stream(stream);
+  if (model == F2B_LENS_EQUIRECT)
+    lens_rays_kernel<F2B_LENS_EQUIRECT><<<grid, 128, 0, st>>>(int(n), height, width, p0, p1, p2, pose, rays_o, rays_d, valid);
+  else if (model == F2B_LENS_FISHEYE)
+    lens_rays_kernel<F2B_LENS_FISHEYE><<<grid, 128, 0, st>>>(int(n), height, width, p0, p1, p2, pose, rays_o, rays_d, valid);
+  else
+    lens_rays_kernel<F2B_LENS_ODS><<<grid, 128, 0, st>>>(int(n), height, width, p0, p1, p2, pose, rays_o, rays_d, valid);
+  return check_launch("f2b_lens_rays");
+}
 
 extern "C" int f2b_img2world_rays(const float* poses, const float* intri, const float* dist_params, const int* cam_indices,
                                   const int* ij, int n_rays, float* rays_o, float* rays_d, void* stream) {

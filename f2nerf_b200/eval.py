@@ -344,24 +344,95 @@ def path_rows(renderer, appearance, n_frames):
 
 @torch.no_grad()
 def RenderPath(renderer, dataset, reso_level=1, ray_batch_size=RAY_BATCH_SIZE, device=None, appearance=None, crop=None,
-               background=None):
+               background=None, lens=None):
     """ExpRunner::RenderPath (ExpRunner.cpp:322-341) over ``dataset.render_poses_`` -> list of device tuples
     (colors [h,w,3], first_oct_dis [h,w,1], disparity [h,w,1]) with h, w = height // reso_level, width // reso_level.
     ``appearance``: None, a training image's index or a [16] row for every frame, or a [F,16] tensor with one row per frame
-    (``path_rows``).  ``crop`` / ``background``: as ``RenderWholeImage``, for every frame."""
+    (``path_rows``).  ``crop`` / ``background``: as ``RenderWholeImage``, for every frame.  ``lens``: a ``Lens`` (DESIGN.md §3o)
+    through which every frame is rendered instead, at (h, w) = ``lens.shape`` (``reso_level`` is then not used; an ODS ipd is in
+    scene units, the frame of ``render_poses_``).  The two normalisations run over the lens's valid pixels; the others are 0."""
     if dataset.render_poses_ is None:
         raise ValueError("RenderPath: the dataset has no render_poses")
     dev = _device_of(renderer, device)
     crop, bg = resolve_crop(crop), _background(background, dev)
-    h, w = dataset.height_ // int(reso_level), dataset.width_ // int(reso_level)
+    h, w = (dataset.height_ // int(reso_level), dataset.width_ // int(reso_level)) if lens is None else lens.shape
     apps = path_rows(renderer, appearance, len(dataset.render_poses_))
     frames = []
     with _Validate(renderer):
         for pose, app in zip(dataset.render_poses_, apps):
-            rays_o, rays_d, _ = dataset.RaysFromPose(pose, reso_level)
-            colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app, crop, bg)
+            if lens is None:
+                rays_o, rays_d, _ = dataset.RaysFromPose(pose, reso_level)
+                colors, first, disp = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app, crop, bg)
+            else:
+                rays_o, rays_d, _, idx = _lens_rays(lens, pose, None, dev)
+                if idx is not None:
+                    rays_o, rays_d = rays_o[idx], rays_d[idx]
+                res = _render_rays(renderer, rays_o, rays_d, ray_batch_size, dev, app, crop, bg)
+                colors, first, disp = (res if idx is None else
+                                       tuple(torch.zeros((h * w, x.shape[1]), dtype=x.dtype, device=dev).index_copy_(0, idx, x)
+                                             for x in res))
             frames.append((colors.reshape(h, w, 3), first.reshape(h, w, 1), disp.reshape(h, w, 1)))
     return frames
+
+
+def _lens_rays(lens, pose, dataset, dev):
+    """``lens.rays`` -> (rays_o, rays_d, valid, idx): idx the indices of the valid pixels (one host sync) for a lens that can leave
+    pixels without a ray, else None (every ray is rendered)."""
+    from .lens import Lens
+    if not isinstance(lens, Lens):
+        raise ValueError(f"lens: expected a Lens, got {type(lens).__name__}")
+    o, d, valid = lens.rays(pose, dataset=dataset, device=dev)
+    return o, d, valid, (valid.nonzero().squeeze(1) if lens.may_be_invalid else None)
+
+
+@torch.no_grad()
+def RenderLens(renderer, lens, pose, dataset=None, depth=False, normals=False, appearance=None, crop=None, background=None,
+               ray_batch_size=RAY_BATCH_SIZE, device=None):
+    """One image through a ``Lens`` (DESIGN.md §3o) -> dict of CPU float32 tensors at (h, w) = ``lens.shape``:
+    "colors" [h,w,3] and "valid" [h,w] bool; with ``depth``, "opacity" and "median_depth" [h,w] as ``RenderDepth`` defines them
+    (along the unit ray, so a panorama's median depth is the radial distance from its centre); with ``normals``, "normals" [h,w,3]
+    as ``RenderNormals``.  ``pose``: [3,4] camera to world, in the normalised scene frame or, with ``dataset``, in the data's own
+    frame (``Lens.rays``).  Pixels that are not valid (outside a fisheye's circle) are 0 in every output.
+    Each chunk of rays is rendered once, whatever is asked for: ``render_forward`` writes the colours, and the termination and
+    normals kernels read the same chunk's slots on its stream.  The values equal ``RenderWholeImage`` / ``RenderDepth`` /
+    ``RenderNormals`` on ``lens.rays()``'s valid rays bit for bit; one device->host copy at the end (and one host sync before
+    rendering for a fisheye).  ``appearance`` / ``crop`` / ``background``: as ``RenderWholeImage``."""
+    from . import ops
+    dev = _device_of(renderer, device)
+    app, crop, bg = resolve_appearance(renderer, appearance), resolve_crop(crop), _background(background, dev)
+    o, d, valid, idx = _lens_rays(lens, pose, dataset, dev)
+    if idx is not None:
+        o, d = o[idx], d[idx]
+    n = d.shape[0]
+    names = ["colors"] * 3 + (["opacity", "median_depth"] if depth else []) + (["normals"] * 3 if normals else [])
+    res = torch.zeros((len(names), n), dtype=torch.float32, device=dev)             # planes; transposed once at the end
+    colors = torch.zeros((n, 3), dtype=torch.float32, device=dev)
+    nrm = torch.zeros((n, 3), dtype=torch.float32, device=dev) if normals else None
+    scratch = torch.empty((2, n), dtype=torch.float32, device=dev)                     # disparity and depth, not returned
+    f, trans = renderer.scene_field_, renderer.pts_sampler_.pers_trans_gpu_
+
+    def each(r, i, j):
+        if depth:
+            ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=res[3, i:j], median_t=res[4, i:j])
+        if normals:
+            ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_, f.mlp_.params_f16(),
+                                     r._keep[0], r.kept_counts, r._w_slots, out=nrm[i:j])
+
+    if n > 0:
+        with _Validate(renderer):
+            _slot_chunks(renderer, o, d, ray_batch_size, dev, each, out=(colors, scratch[0], scratch[1]), bg=bg, app=app, crop=crop)
+    res[0:3] = colors.T
+    if normals:
+        res[-3:] = nrm.T
+    h, w = lens.shape
+    full = res if idx is None else torch.zeros((len(names), h * w), dtype=torch.float32, device=dev).index_copy_(1, idx, res)
+    full = torch.cat([full, valid.to(torch.float32)[None]]).cpu()                     # the one device->host copy
+    out = {"colors": full[0:3].T.reshape(h, w, 3).contiguous(), "valid": full[-1].reshape(h, w).bool()}
+    if depth:
+        out["opacity"], out["median_depth"] = full[3].reshape(h, w).contiguous(), full[4].reshape(h, w).contiguous()
+    if normals:
+        out["normals"] = full[-4:-1].T.reshape(h, w, 3).contiguous()
+    return out
 
 
 @torch.no_grad()

@@ -363,6 +363,25 @@ int f2b_img2world_rays(const float* poses, const float* intri, const float* dist
  * 1 <= out_h <= height, 1 <= out_w <= width, out_h*out_w < 2^31. */
 int f2b_camera_rays(const float* pose, const float* intri, const float* dist_params, int height, int width, int out_h,
                     int out_w, float* rays_o /* [out_h*out_w,3] */, float* rays_d /* [out_h*out_w,3] */, void* stream);
+/* Lens rays (DESIGN.md §3o): the rays of a panoramic or fisheye image through the camera pose [3,4] (camera to world, device, the
+ * normalised scene frame).  Ray a*width + b passes through the centre (a + 0.5, b + 0.5) of pixel (a, b), row 0 at the top.  Camera
+ * frame as f2b_camera_rays (OpenGL: x right, y up, looking down -z); longitude lam from -z, positive towards +x; latitude phi
+ * positive towards +y.
+ * - F2B_LENS_EQUIRECT, p0 = hfov in (0, 360], p1 = vfov in (0, 180] (degrees): lam = hfov ((b + .5) / width - .5),
+ *   phi = vfov (.5 - (a + .5) / height), d_cam = (cos phi sin lam, sin phi, -cos phi cos lam).
+ * - F2B_LENS_FISHEYE (equidistant), p0 = fov in (0, 360]: offset (x, y) = (b + .5 - width / 2, a + .5 - height / 2), r = |(x, y)|,
+ *   f = (min(height, width) / 2) / (fov / 2 in radians), theta = r / f, d_cam = (sin theta x / r, -sin theta y / r, -cos theta),
+ *   (0, 0, -1) at r = 0.  valid = theta <= fov / 2, decided exactly (r <= min(height, width) / 2); rays_d = 0 where not valid.
+ * - F2B_LENS_ODS (omnidirectional stereo), p0, p1 as F2B_LENS_EQUIRECT, p2 = ipd >= 0 (scene units): 2*height x width rays, the
+ *   left eye's image on top of the right's, directions those of the equirectangular image, origin
+ *   t + R (s ipd / 2 (cos lam, 0, sin lam)) with s = -1 for the left eye and +1 for the right (the horizontal viewing direction
+ *   crossed with up).  At ipd = 0 the origins are t and the directions the equirectangular ones, bit for bit.
+ * World rays: rays_d = R d_cam, rays_o = t (ODS: plus its offset).  Angles, trig (sincospi on half-turns), the rotation and the
+ * offset are float64; each output is rounded to fp32 once (within 1 ulp of the exact value).  valid [N] is 1 except outside
+ * the fisheye's circle.  height, width >= 1 and N < 2^31. */
+enum { F2B_LENS_EQUIRECT = 0, F2B_LENS_FISHEYE = 1, F2B_LENS_ODS = 2 };
+int f2b_lens_rays(int model, const float* pose /* device [3,4] */, int height, int width, double p0, double p1, double p2,
+                  float* rays_o /* [N,3] */, float* rays_d /* [N,3] */, uint8_t* valid /* [N] */, void* stream);
 /* out[r] = images[cam_indices[r], ij[r,0], ij[r,1], 0:3]; images fp32 [n_img, height, width, 3] resident on the device. */
 int f2b_gather_pixels(const float* images, const int* cam_indices, const int* ij, int height, int width, int n,
                       float* out /* [n,3] */, void* stream);

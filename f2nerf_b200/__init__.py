@@ -13,6 +13,7 @@ from .dataset import RayGenerator, load_dataset
 from .octree_build import build_edge_pool, build_tree_nodes, initial_octree
 from .eval import ImageMetrics, RenderAllImages, RenderDepth, RenderLens, RenderNormals, RenderPath, RenderWholeImage, TestImages
 from .field import Hash3DAnchored, TCNNWP
+from .geometry import ExtractTSDFMesh, FuseTSDF, TSDFGrid, TSDFSurface
 from .lens import Lens, level_pose
 from .ops import CustomOps, FlexOps
 from .optim import FusedAdam
@@ -21,6 +22,6 @@ from .renderer import Renderer, RenderResult, check_backward_nan
 from .sampler import TRAIN, VALIDATE, GlobalDataPool, PersSampler, SampleResultFlex
 from .shader import SHShader
 
-__all__ = ["Crop", "Lens", "level_pose", "RenderLens", "FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
+__all__ = ["ExtractTSDFMesh", "FuseTSDF", "TSDFGrid", "TSDFSurface", "Crop", "Lens", "level_pose", "RenderLens", "FitAppearance", "TestAppearance", "FusedAdam", "RayGradient", "RefinePose", "RayGenerator", "load_dataset", "load_scene", "load_states", "Scene", "gradient_scaling_progress",
            "build_tree_nodes", "build_edge_pool", "initial_octree", "RenderWholeImage", "RenderDepth", "RenderNormals", "TestImages", "ImageMetrics", "RenderPath", "RenderAllImages", "Hash3DAnchored", "TCNNWP", "CustomOps", "FlexOps", "Renderer", "RenderResult", "check_backward_nan",
            "TRAIN", "VALIDATE", "GlobalDataPool", "PersSampler", "SampleResultFlex", "SHShader"]

@@ -61,6 +61,9 @@ SIGNATURES = {
     "f2b_render_normals_slots": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P],
     "f2b_ray_termination_slots": [_P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P],
     "f2b_depth_consistency": [_P, _P, c_int, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, c_float, c_float, _P, _P, _P],
+    "f2b_tsdf_integrate": [_P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, _P, c_float, c_int, c_int, c_int, c_int, c_int, c_float,
+                           c_float, c_int, _P, _P, _P, _P],
+    "f2b_tsdf_colors": [_P, c_int, _P, _P, c_int, c_int, c_int, _P, c_float, _P, _P],
     "f2b_ray_grad": [_P, _P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, c_float, _P, _P, _P,
                      _P, _P, _P, _P],
     "f2b_iso_count": [_P, c_int, c_int, c_int, c_float, c_float, c_int, c_int, _P, _P, _P, _P],

@@ -254,32 +254,97 @@ depth_consistency_kernel(const float* __restrict__ pts, const int* __restrict__ 
     if (cell) cell[i] = -1;
     return;
   }
-  const float dx = fsub(__ldg(pts + 3 * size_t(i)), __ldg(pose + 3));
-  const float dy = fsub(__ldg(pts + 3 * size_t(i) + 1), __ldg(pose + 7));
-  const float dz = fsub(__ldg(pts + 3 * size_t(i) + 2), __ldg(pose + 11));
-  float xc[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++)                                     // R^T (p - o): column k of R
-    xc[k] = ffma(__ldg(pose + 8 + k), dz, ffma(__ldg(pose + 4 + k), dy, fmul(__ldg(pose + k), dx)));
-  int idx = -1;
-  if (xc[2] < 0.f) {
-    const float u = fdiv(xc[0], -xc[2]), v = fdiv(xc[1], xc[2]);  // dir = (u, -v, -1) in the camera frame
-    const float u2 = fmul(u, u), uv = fmul(u, v), v2 = fmul(v, v);
-    float du, dv;
-    distort(load_dist(dist_params), u, v, u2, uv, v2, fadd(u2, v2), du, dv);
-    const float x = ffma(__ldg(intri), fadd(u, du), __ldg(intri + 2));        // fx u_d + cx
-    const float y = ffma(__ldg(intri + 4), fadd(v, dv), __ldg(intri + 5));    // fy v_d + cy
-    const float fb = fdiv(fsub(x, .5f), step_j), fa = fdiv(fsub(y, .5f), step_i);   // the grid's pixel centres sit at +.5
-    if (fb > -1.f && fb < float(out_w) && fa > -1.f && fa < float(out_h)) {
-      const int b = __float2int_rn(fb), a = __float2int_rn(fa);
-      if (b >= 0 && b < out_w && a >= 0 && a < out_h) idx = a * out_w + b;
-    }
-  }
+  float dx, dy, dz;
+  const int idx = project_cell(LdgLoad(), pose, intri, dist_params, [&](int k) { return __ldg(pts + 3 * size_t(i) + k); }, out_h, out_w,
+                               step_i, step_j, dx, dy, dz);
   if (cell) cell[i] = idx;
   if (idx < 0 || !(__ldg(opacity + idx) >= min_opacity)) return;
   const float tb = __ldg(median_t + idx);
   const float dist = fsqrt(fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz)));
   if (fabsf(fsub(dist, tb)) <= fmul(rel_tol, tb)) count[i] += 1;
+}
+
+
+// ---- TSDF fusion (DESIGN §3p) ----------------------------------------------------------------------------------------
+// One thread per lattice point of a z-slab, over a group of views whose camera table (kTsdfCam floats per view: pose 12, rows
+// 0-1 of K 6, distortion 4) is staged in shared memory.  The point's sums are read once (unless the group is the first), carried
+// in registers across the group's views in order, and written once; every addition is one fp32 op in view order, so the bits do
+// not depend on how the views are split into groups.
+constexpr int kTsdfCam = 22;
+constexpr int kTsdfMaxViews = 64;
+constexpr int kTsdfThreads = 128;
+
+__global__ void __launch_bounds__(kTsdfThreads)
+tsdf_integrate_kernel(const float* __restrict__ cams, int n_views, const float* __restrict__ opacity, const float* __restrict__ median_t,
+                      const float* __restrict__ colors, int out_h, int out_w, float step_i, float step_j, float ox, float oy,
+                      float oz, float vox, int nx, int ny, int z0, int n_layers, float mu, float min_opacity, int first,
+                      float* __restrict__ sdf_sum, float* __restrict__ weight, float* __restrict__ color_sum) {
+  __shared__ float s_cam[kTsdfMaxViews * kTsdfCam];
+  for (int k = threadIdx.x; k < n_views * kTsdfCam; k += blockDim.x) s_cam[k] = __ldg(cams + k);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nx * ny * n_layers) return;
+  const int ix = i % nx, iy = (i / nx) % ny, iz = z0 + i / (nx * ny);
+  const float p[3] = {fadd(ox, fmul(vox, float(ix))), fadd(oy, fmul(vox, float(iy))), fadd(oz, fmul(vox, float(iz)))};
+  const size_t g = size_t(iz) * nx * ny + size_t(iy) * nx + ix;
+  float s = 0.f, w = 0.f, r = 0.f, gr = 0.f, b = 0.f;
+  if (!first) {
+    s = sdf_sum[g]; w = weight[g];
+    r = color_sum[3 * g]; gr = color_sum[3 * g + 1]; b = color_sum[3 * g + 2];
+  }
+  const size_t n_cells = size_t(out_h) * out_w;
+  const float neg_mu = -mu;
+  for (int v = 0; v < n_views; v++) {
+    const float* cam = s_cam + v * kTsdfCam;
+    float dx, dy, dz;
+    const int idx = project_cell(PlainLoad(), cam, cam + 12, cam + 18, [&](int k) { return p[k]; }, out_h, out_w, step_i, step_j, dx, dy, dz);
+    if (idx < 0) continue;
+    const size_t c = v * n_cells + idx;
+    if (!(__ldg(opacity + c) >= min_opacity)) continue;
+    const float dist = fsqrt(fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz)));
+    const float sdf = fsub(__ldg(median_t + c), dist);
+    if (!(sdf >= neg_mu)) continue;
+    s = fadd(s, fminf(1.f, fdiv(sdf, mu)));
+    w = fadd(w, 1.f);
+    r = fadd(r, __ldg(colors + 3 * c)); gr = fadd(gr, __ldg(colors + 3 * c + 1)); b = fadd(b, __ldg(colors + 3 * c + 2));
+  }
+  sdf_sum[g] = s; weight[g] = w;
+  color_sum[3 * g] = r; color_sum[3 * g + 1] = gr; color_sum[3 * g + 2] = b;
+}
+
+// One thread per vertex: trilinear interpolation of color_sum / weight over the observed corners of the vertex's cell (weight > 0
+// and not on the lattice's outermost layer), their trilinear weights renormalised; 0 where no corner is observed.
+__global__ void __launch_bounds__(128)
+tsdf_colors_kernel(const float* __restrict__ verts, int n_verts, const float* __restrict__ weight, const float* __restrict__ color_sum,
+                   int nx, int ny, int nz, float ox, float oy, float oz, float vox, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_verts) return;
+  const int n[3] = {nx, ny, nz};
+  const float o[3] = {ox, oy, oz};
+  int i0[3];
+  float f[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const float u = fdiv(fsub(__ldg(verts + 3 * size_t(i) + k), o[k]), vox);
+    const int c = min(max(int(floorf(u)), 0), n[k] - 2);
+    i0[k] = c;
+    f[k] = fminf(fmaxf(fsub(u, float(c)), 0.f), 1.f);
+  }
+  float acc[3] = {0.f, 0.f, 0.f}, tw = 0.f;
+#pragma unroll
+  for (int q = 0; q < 8; q++) {
+    const int x = i0[0] + (q & 1), y = i0[1] + (q >> 1 & 1), z = i0[2] + (q >> 2);
+    if (x == 0 || y == 0 || z == 0 || x == nx - 1 || y == ny - 1 || z == nz - 1) continue;
+    const size_t g = size_t(z) * nx * ny + size_t(y) * nx + x;
+    const float wg = __ldg(weight + g);
+    if (!(wg > 0.f)) continue;
+    const float t = fmul(fmul(q & 1 ? f[0] : fsub(1.f, f[0]), q & 2 ? f[1] : fsub(1.f, f[1])), q & 4 ? f[2] : fsub(1.f, f[2]));
+#pragma unroll
+    for (int k = 0; k < 3; k++) acc[k] = ffma(t, fdiv(__ldg(color_sum + 3 * g + k), wg), acc[k]);
+    tw = fadd(tw, t);
+  }
+#pragma unroll
+  for (int k = 0; k < 3; k++) out[3 * size_t(i) + k] = tw > 0.f ? fdiv(acc[k], tw) : 0.f;
 }
 
 }  // namespace f2b
@@ -358,4 +423,37 @@ extern "C" int f2b_iso_emit(const float* logit, int nx, int ny, int nz, float le
                                                                  origin3[2], voxel3[0], voxel3[1], voxel3[2], ez0, ez1 - ez0, vert_base,
                                                                  edge_mask, vert_bounds, tri_bounds, verts, faces);
   return check_launch("f2b_iso_emit");
+}
+
+extern "C" int f2b_tsdf_integrate(const float* cams, int n_views, const float* opacity, const float* median_t, const float* colors,
+                                  int height, int width, int out_h, int out_w, const float* origin3, float voxel, int nx, int ny,
+                                  int nz, int z0, int n_layers, float mu, float min_opacity, int first, float* sdf_sum,
+                                  float* weight, float* color_sum, void* stream) {
+  F2B_REQUIRE(cams && opacity && median_t && colors && origin3 && sdf_sum && weight && color_sum, "f2b_tsdf_integrate: null pointer");
+  F2B_REQUIRE(n_views >= 1 && n_views <= kTsdfMaxViews, "f2b_tsdf_integrate: %d views outside [1, %d] per launch", n_views, kTsdfMaxViews);
+  F2B_REQUIRE(out_h >= 2 && out_h <= height && out_w >= 2 && out_w <= width, "f2b_tsdf_integrate: grid %dx%d outside image %dx%d",
+              out_h, out_w, height, width);
+  F2B_REQUIRE(int64_t(out_h) * out_w < (int64_t(1) << 31), "f2b_tsdf_integrate: %d x %d cells overflow int32", out_h, out_w);
+  F2B_REQUIRE(nx >= 1 && ny >= 1 && nz >= 1 && z0 >= 0 && n_layers >= 1 && z0 + n_layers <= nz,
+              "f2b_tsdf_integrate: bad lattice %d x %d x %d or slab [%d, %d)", nx, ny, nz, z0, z0 + n_layers);
+  F2B_REQUIRE(int64_t(nx) * ny * n_layers < (int64_t(1) << 31), "f2b_tsdf_integrate: the slab's points overflow int32");
+  F2B_REQUIRE(isfinite(voxel) && voxel > 0.f, "f2b_tsdf_integrate: voxel must be finite and > 0");
+  F2B_REQUIRE(isfinite(mu) && mu > 0.f, "f2b_tsdf_integrate: mu must be finite and > 0");
+  F2B_REQUIRE(min_opacity > 0.f && min_opacity <= 1.f, "f2b_tsdf_integrate: min_opacity must lie in (0, 1]");
+  const int64_t n = int64_t(nx) * ny * n_layers;
+  tsdf_integrate_kernel<<<div_up(n, kTsdfThreads), kTsdfThreads, 0, as_stream(stream)>>>(
+      cams, n_views, opacity, median_t, colors, out_h, out_w, linspace_step(height, out_h), linspace_step(width, out_w), origin3[0],
+      origin3[1], origin3[2], voxel, nx, ny, z0, n_layers, mu, min_opacity, first, sdf_sum, weight, color_sum);
+  return check_launch("f2b_tsdf_integrate");
+}
+
+extern "C" int f2b_tsdf_colors(const float* verts, int n_verts, const float* weight, const float* color_sum, int nx, int ny, int nz,
+                               const float* origin3, float voxel, float* colors, void* stream) {
+  if (n_verts <= 0) return F2B_OK;
+  F2B_REQUIRE(verts && weight && color_sum && origin3 && colors, "f2b_tsdf_colors: null pointer");
+  F2B_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "f2b_tsdf_colors: lattice %d x %d x %d has an axis under 2 points", nx, ny, nz);
+  F2B_REQUIRE(isfinite(voxel) && voxel > 0.f, "f2b_tsdf_colors: voxel must be finite and > 0");
+  tsdf_colors_kernel<<<div_up(n_verts, 128), 128, 0, as_stream(stream)>>>(verts, n_verts, weight, color_sum, nx, ny, nz, origin3[0],
+                                                                        origin3[1], origin3[2], voxel, colors);
+  return check_launch("f2b_tsdf_colors");
 }

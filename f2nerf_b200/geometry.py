@@ -18,6 +18,11 @@ unbounded scene near and far: ``ExtractPointCloud`` renders every view on a grid
 sample (``eval.RenderDepth``'s termination kernel), coloured by the pixel's foreground colour, and keeps the points whose depth
 the other views confirm (``f2b_depth_consistency``).
 
+A TSDF mesh (DESIGN.md §3p) meshes the surface the views' median depths agree on rather than a density level: ``FuseTSDF``
+averages, per lattice point, the truncated signed distances to the depth maps of the views that see it (``f2b_tsdf_integrate``),
+``TSDFSurface`` extracts their zero level set over the observed lattice points and colours it (``f2b_tsdf_colors``), and
+``ExtractTSDFMesh`` renders the maps of the training views (``ExtractPointCloud``'s pass 1) and does both.
+
 A crop box (``crop.Crop``, DESIGN.md §3n) restricts the lattice, the mesh and the point cloud to what the box keeps: lattice points
 it does not keep read ``EMPTY_LOGIT``, so the mesh stays closed and caps the cut, and the point cloud's renders are cropped.
 """
@@ -37,6 +42,7 @@ EMPTY_LOGIT = -1e4          # logit of a point outside every valid leaf: finite,
 SLAB_POINTS = 1 << 23       # Isosurface: owner points per z-slab; scratch <= 25 B x (SLAB_POINTS + one layer), ~210 MB
 GRID_SLAB_POINTS = 1 << 30  # DensityGrid: lattice points per kernel launch (the kernel indexes a slab with int32)
 CROP_MASK_POINTS = 1 << 24  # DensityGrid(crop=): lattice points masked per f2b_crop_mask launch (12 B of points each)
+TSDF_SLAB_POINTS = 1 << 30  # FuseTSDF: lattice points per kernel launch (the kernel indexes a slab with int32)
 
 
 class Grid(NamedTuple):
@@ -59,6 +65,16 @@ class Mesh(NamedTuple):
         differ by a uniform scale and a translation, so the normals carry over unchanged."""
         center = torch.as_tensor(dataset.center_, dtype=torch.float32, device=self.verts.device)
         return Mesh(self.verts * float(dataset.radius_) + center, self.faces, self.colors, self.normals)
+
+
+class TSDFGrid(NamedTuple):
+    """The sums of a TSDF fusion (DESIGN.md §3p), fp32 on the device: ``sdf_sum`` and ``weight`` [nz, ny, nx], ``color_sum``
+    [nz, ny, nx, 3]; lattice point (i, j, k) at origin + voxel * (i, j, k), ``voxel`` one float (cubic voxels)."""
+    sdf_sum: torch.Tensor
+    weight: torch.Tensor
+    color_sum: torch.Tensor
+    origin: tuple
+    voxel: float
 
 
 class PointCloud(NamedTuple):
@@ -184,6 +200,18 @@ def _crop_lattice(crop, logit, origin, voxel, z0):
         logit[k0:k0 + n].masked_fill_(~crop.mask(pts).view(n, ny, nx), EMPTY_LOGIT)
 
 
+def _lattice(bbox_min, bbox_max, reso, who):
+    """(origin, voxel, (nx, ny, nz)) of the lattice over [bbox_min, bbox_max] with cubic voxels, ``reso`` points along the box's
+    longest axis; origin and voxel rounded to fp32."""
+    lo, hi = np.asarray(bbox_min, np.float64).reshape(3), np.asarray(bbox_max, np.float64).reshape(3)
+    ext = hi - lo
+    if int(reso) < 2 or not (ext > 0).all():
+        raise ValueError(f"{who}: reso must be >= 2 and the box must have a positive extent on every axis")
+    voxel = float(np.float32(ext.max() / (int(reso) - 1)))
+    shape = tuple(min(int(reso), int(math.ceil(e / voxel - 1e-6)) + 1) for e in ext)
+    return tuple(float(np.float32(v)) for v in lo), voxel, shape
+
+
 def DensityGrid(renderer, bbox_min=None, bbox_max=None, reso=256, crop=None):
     """The density logit on a lattice over the box [bbox_min, bbox_max] (default: ``leaf_bounds``) with cubic voxels, ``reso``
     points along the box's longest axis -> ``Grid``.  The lattice points are generated in the kernel, in z-slabs.
@@ -197,13 +225,7 @@ def DensityGrid(renderer, bbox_min=None, bbox_max=None, reso=256, crop=None):
             lo, hi = tuple(max(a, b) for a, b in zip(lo, clo)), tuple(min(a, b) for a, b in zip(hi, chi))
         bbox_min = lo if bbox_min is None else bbox_min
         bbox_max = hi if bbox_max is None else bbox_max
-    lo, hi = np.asarray(bbox_min, np.float64).reshape(3), np.asarray(bbox_max, np.float64).reshape(3)
-    ext = hi - lo
-    if int(reso) < 2 or not (ext > 0).all():
-        raise ValueError("DensityGrid: reso must be >= 2 and the box must have a positive extent on every axis")
-    voxel = float(np.float32(ext.max() / (int(reso) - 1)))
-    nx, ny, nz = (min(int(reso), int(math.ceil(e / voxel - 1e-6)) + 1) for e in ext)
-    origin = tuple(float(np.float32(v)) for v in lo)
+    origin, voxel, (nx, ny, nz) = _lattice(bbox_min, bbox_max, reso, "DensityGrid")
     nodes, trans = _octree(renderer)
     fargs = _field_args(renderer)
     logit = torch.empty((nz, ny, nx), dtype=torch.float32, device=nodes.device)
@@ -299,6 +321,33 @@ def ExtractMesh(renderer, bbox_min=None, bbox_max=None, reso=512, alpha=0.5, den
     return Mesh(verts, faces, rgb, nrm)
 
 
+def _view_maps(renderer, dataset, views, h, w, apps, crop, normals=False):
+    """Pass 1 of ``ExtractPointCloud`` and ``ExtractTSDFMesh``: per view of ``views`` (with its appearance row of ``apps``), the
+    VALIDATE render of the view's own camera on the h x w grid with a black background, cropped by ``crop``, and the termination
+    kernel (with ``normals`` the normals kernel) on its slots -> yields (opacity [n], median_t [n], point [n,3], rgb [n,3],
+    normals [n,3] or None), n = h * w.  The caller holds ``torch.no_grad()`` and ``eval._Validate(renderer)``."""
+    from .eval import RAY_BATCH_SIZE, _slot_chunks
+    n = h * w
+    dev = dataset.poses_.device
+    f = renderer.scene_field_
+    trans = renderer.pts_sampler_.pers_trans_gpu_
+    black = torch.zeros((3,), dtype=torch.float32, device=dev)
+    f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
+    for b, app in zip(views, apps):
+        o, d = dataset._camera_rays(dataset.poses_[b], dataset.intri_[b], dataset.dist_params_[b], h, w)
+        opa, med, point, rgb = f32(n), f32(n), f32(n, 3), f32(n, 3)
+        nm = f32(n, 3) if normals else None
+
+        def each(r, i, j):
+            ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=opa[i:j], median_t=med[i:j], point=point[i:j])
+            if normals:
+                ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
+                                         f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=nm[i:j])
+
+        _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black, app=app, crop=crop)
+        yield opa, med, point, rgb, nm
+
+
 def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0.9, min_views=2, rel_tol=0.01, normals=False,
                       appearance=None, crop=None):
     """The scene's surface as a coloured ``PointCloud`` on the device, in the normalised frame (``to_data_frame`` maps it back).
@@ -313,7 +362,7 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
     (``Renderer.appearance_row``): None, a training image's index, a [16] row, or ``"own"``: each view's own row.  The points
     themselves do not depend on it (weights and density do not).  ``crop``: a ``Crop``; every render is cropped (DESIGN.md §3n), so
     the candidates and the consistency pass see only what the box keeps."""
-    from .eval import RAY_BATCH_SIZE, _slot_chunks, _Validate
+    from .eval import _Validate
     crop = resolve_crop(crop)
     views = [int(v) for v in (dataset.train_set_ if views is None else views)]
     reso_level, min_views = int(reso_level), int(min_views)
@@ -332,26 +381,10 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
     h, w = H // reso_level, W // reso_level
     if h < 2 or w < 2:
         raise ValueError(f"ExtractPointCloud: reso_level {reso_level} leaves a {h} x {w} grid of a {H} x {W} image")
-    n = h * w
     dev = dataset.poses_.device
-    f = renderer.scene_field_
-    trans = renderer.pts_sampler_.pers_trans_gpu_
-    black = torch.zeros((3,), dtype=torch.float32, device=dev)
-    f32 = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
     maps, pts, cols, nrms, srcs = [], [], [], [], []
     with torch.no_grad(), _Validate(renderer):
-        for b, app in zip(views, apps):
-            o, d = dataset._camera_rays(dataset.poses_[b], dataset.intri_[b], dataset.dist_params_[b], h, w)
-            opa, med, point, rgb = f32(n), f32(n), f32(n, 3), f32(n, 3)
-            nm = f32(n, 3) if normals else None
-
-            def each(r, i, j):
-                ops.ray_termination_slots(r._keep[0], r.kept_counts, r._w_slots, opacity=opa[i:j], median_t=med[i:j], point=point[i:j])
-                if normals:
-                    ops.render_normals_slots(trans, f.table_f16(), f.prim_pool_, f.bias_pool_, f.n_volumes_, f.local_size_,
-                                             f.mlp_.params_f16(), r._keep[0], r.kept_counts, r._w_slots, out=nm[i:j])
-
-            _slot_chunks(renderer, o, d, RAY_BATCH_SIZE, dev, each, out=(rgb, f32(n), f32(n)), bg=black, app=app, crop=crop)
+        for b, (opa, med, point, rgb, nm) in zip(views, _view_maps(renderer, dataset, views, h, w, apps, crop, normals)):
             cell = torch.nonzero(opa >= float(min_opacity)).squeeze(1)            # the host sync of the view; cells ascending
             maps.append((opa, med))
             pts.append(point[cell])
@@ -370,6 +403,149 @@ def ExtractPointCloud(renderer, dataset, views=None, reso_level=1, min_opacity=0
             points, colors, source = points[keep], colors[keep], source[keep]
             nrm = nrm[keep] if normals else None
     return PointCloud(points, colors, nrm, source)
+
+
+def _tsdf_args(trunc, min_opacity, who):
+    if not (math.isfinite(float(trunc)) and float(trunc) > 0.):
+        raise ValueError(f"{who}: trunc must be finite and > 0")
+    if not 0. < float(min_opacity) <= 1.:
+        raise ValueError(f"{who}: min_opacity must lie in (0, 1]")
+
+
+def FuseTSDF(poses, intri, dist_params, height, width, opacity, median_t, colors, bbox_min, bbox_max, reso=512, trunc=4., min_opacity=0.9):
+    """TSDF fusion of V views' depth maps into a lattice over [bbox_min, bbox_max] (cubic voxels, ``reso`` points along the
+    longest axis, as ``DensityGrid``) -> ``TSDFGrid`` (DESIGN.md §3p).  View v: camera ``poses[v]`` [3,4] camera-to-world,
+    ``intri[v]`` [3,3], ``dist_params[v]`` (k1, k2, p1, p2) of a ``height`` x ``width`` image, and its maps on the h x w grid
+    ``f2b_camera_rays`` renders: ``opacity`` and ``median_t`` (along the unit ray) [V,h,w], ``colors`` [V,h,w,3] (fp32 CUDA tensors).
+    Per lattice point and view, in view order: where the point projects into the grid (``f2b_depth_consistency``'s projection) on
+    a pixel with opacity >= ``min_opacity`` and sdf = median_t - |p - o| >= -mu, mu = fp32(trunc * voxel): sdf_sum += min(1, sdf
+    / mu), weight += 1, color_sum += the pixel's colour.  The views go through ``f2b_tsdf_integrate`` in groups of
+    ``ops.TSDF_MAX_VIEWS``; the bits do not depend on the grouping."""
+    if not (isinstance(opacity, torch.Tensor) and opacity.dim() == 3):
+        raise ValueError("FuseTSDF: opacity must be a [V, h, w] tensor")
+    V, h, w = opacity.shape
+    shapes = ((poses, (V, 3, 4), "poses"), (intri, (V, 3, 3), "intri"), (dist_params, (V, 4), "dist_params"),
+              (median_t, (V, h, w), "median_t"), (colors, (V, h, w, 3), "colors"))
+    for t, shape, name in shapes:
+        if tuple(torch.as_tensor(t).shape) != shape:
+            raise ValueError(f"FuseTSDF: {name} has shape {tuple(torch.as_tensor(t).shape)}, expected {shape}")
+    if V < 1 or not (2 <= h <= int(height) and 2 <= w <= int(width)):
+        raise ValueError(f"FuseTSDF: {V} views of a {h} x {w} grid of a {height} x {width} image")
+    _tsdf_args(trunc, min_opacity, "FuseTSDF")
+    if not (np.isfinite(np.asarray(bbox_min, np.float64)).all() and np.isfinite(np.asarray(bbox_max, np.float64)).all()):
+        raise ValueError("FuseTSDF: the box must be finite")
+    origin, voxel, (nx, ny, nz) = _lattice(bbox_min, bbox_max, reso, "FuseTSDF")
+    for t, name in ((opacity, "opacity"), (median_t, "median_t"), (colors, "colors")):
+        ops._chk(t, torch.float32, f"FuseTSDF: {name}")
+    dev = opacity.device
+    cam = lambda t, k: torch.as_tensor(t, dtype=torch.float32, device=dev).reshape(V, -1)[:, :k]
+    cams = torch.cat([cam(poses, 12), cam(intri, 6), cam(dist_params, 4)], 1).contiguous()      # pose, rows 0-1 of K, distortion
+    mu = float(np.float32(float(trunc) * voxel))
+    sdf_sum = torch.empty((nz, ny, nx), dtype=torch.float32, device=dev)
+    weight, color_sum = torch.empty_like(sdf_sum), torch.empty((nz, ny, nx, 3), dtype=torch.float32, device=dev)
+    step = max(1, TSDF_SLAB_POINTS // (nx * ny))
+    for z0 in range(0, nz, step):
+        n = min(step, nz - z0)
+        for g0 in range(0, V, ops.TSDF_MAX_VIEWS):
+            g = slice(g0, min(g0 + ops.TSDF_MAX_VIEWS, V))
+            ops.tsdf_integrate(cams[g], opacity[g], median_t[g], colors[g], height, width, origin, voxel, z0, n, mu, min_opacity, g0 == 0,
+                               sdf_sum, weight, color_sum)
+    return TSDFGrid(sdf_sum, weight, color_sum, origin, voxel)
+
+
+def TSDFSurface(grid):
+    """The zero level set of a ``TSDFGrid`` as a coloured ``Mesh`` (no normals), in the grid's frame (DESIGN.md §3p).  A lattice point
+    is observed when its weight is > 0 and it is not on the lattice's outermost layer; the surface is the marching-tetrahedra
+    surface of -sdf_sum / weight at 0 over the tetrahedra whose corners are all observed, outward towards free space.  It is
+    ``Isosurface`` of a lattice holding NaN where a point is not observed: every face of a tetrahedron with a NaN corner has a
+    vertex on an edge to it, whose position is NaN, so dropping the faces with a non-finite vertex and then the unreferenced
+    vertices (renumbered in order) leaves the fully observed tetrahedra.  Vertex colours: ``f2b_tsdf_colors``."""
+    wt = grid.weight
+    obs = wt > 0
+    for a in range(3):
+        obs.narrow(a, 0, 1).fill_(False)
+        obs.narrow(a, obs.shape[a] - 1, 1).fill_(False)
+    value = torch.where(obs, -grid.sdf_sum / wt, torch.full_like(wt, float("nan")))
+    verts, faces = Isosurface(value, 0., grid.origin, (grid.voxel,) * 3, empty_logit=-1.)
+    del value, obs
+    f = faces.long()
+    f = f[torch.isfinite(verts).all(1)[f].all(1)]
+    used = torch.zeros((verts.shape[0],), dtype=torch.bool, device=verts.device)
+    used[f.reshape(-1)] = True
+    renum = torch.cumsum(used, 0, dtype=torch.int32) - 1
+    verts, faces = verts[used], renum[f]
+    return Mesh(verts, faces, ops.tsdf_colors(verts, wt, grid.color_sum, grid.origin, grid.voxel), None)
+
+
+def _tsdf_maps(renderer, dataset, views, reso_level, bbox_min, bbox_max, min_opacity, apps, crop):
+    """Pass 1 of ``ExtractTSDFMesh`` -> (opacity, median_t [V,h,w], colors [V,h,w,3], h, w, bbox_min, bbox_max), the box completed
+    by its default where not given."""
+    from .eval import _Validate
+    h, w = dataset.height_ // reso_level, dataset.width_ // reso_level
+    need_box = bbox_min is None or bbox_max is None
+    pct = need_box and (crop is None or crop.invert)
+    opas, meds, cols, pts = [], [], [], []
+    with torch.no_grad(), _Validate(renderer):
+        for opa, med, point, rgb, _ in _view_maps(renderer, dataset, views, h, w, apps, crop):
+            opas.append(opa.view(h, w))
+            meds.append(med.view(h, w))
+            cols.append((rgb / opa[:, None]).clamp_(0., 1.).view(h, w, 3))     # only read where opa >= min_opacity > 0
+            if pct:
+                pts.append(point[opa >= float(min_opacity)])
+    opacity, median_t, colors = torch.stack(opas), torch.stack(meds), torch.stack(cols)
+    del opas, meds, cols
+    if need_box:
+        lo, hi = leaf_bounds(renderer)
+        if pct:
+            p = torch.cat(pts)
+            if p.shape[0] == 0:
+                raise ValueError("ExtractTSDFMesh: no pixel reaches min_opacity, so there is no default box; pass bbox_min and bbox_max")
+            s = torch.sort(p, dim=0).values                       # per axis (torch.quantile refuses more than 2^24 elements)
+            n = s.shape[0]
+            p1, p99 = s[int(math.floor(.01 * (n - 1)))].double(), s[int(math.ceil(.99 * (n - 1)))].double()
+            pad = (p99 - p1) * .05
+            clo, chi = (p1 - pad).tolist(), (p99 + pad).tolist()
+            del p, s
+        else:
+            clo, chi = crop.aabb()
+        lo, hi = tuple(max(a, b) for a, b in zip(lo, clo)), tuple(min(a, b) for a, b in zip(hi, chi))
+        bbox_min = lo if bbox_min is None else bbox_min
+        bbox_max = hi if bbox_max is None else bbox_max
+    return opacity, median_t, colors, bbox_min, bbox_max
+
+
+def ExtractTSDFMesh(renderer, dataset, views=None, reso_level=1, reso=512, bbox_min=None, bbox_max=None, trunc=4., min_opacity=0.9,
+                    appearance=None, crop=None):
+    """The scene's surface as a coloured ``Mesh`` on the device fused from the views' depth maps, in the normalised frame
+    (``Mesh.to_data_frame`` maps it back; DESIGN.md §3p).  Pass 1 is ``ExtractPointCloud``'s: every view of ``views`` (default
+    ``dataset.train_set_``) rendered on the (height // reso_level) x (width // reso_level) grid, its opacity, median depth and
+    foreground colour C / W.  Then ``FuseTSDF`` over the box [bbox_min, bbox_max] at ``reso`` with ``trunc`` and ``min_opacity``,
+    and ``TSDFSurface``.  The default box: with a crop that is not inverted, ``crop.aabb()``; otherwise, per axis, the 1st to 99th
+    percentile of the median points of the pixels with opacity >= ``min_opacity``, widened by 5 % of its extent; both within
+    ``leaf_bounds``.  ``appearance`` (including ``"own"``) colours the mesh only; ``crop`` crops every render (DESIGN.md §3n).
+    The result has the same bits every run."""
+    crop = resolve_crop(crop)
+    views = [int(v) for v in (dataset.train_set_ if views is None else views)]
+    reso_level = int(reso_level)
+    if not views:
+        raise ValueError("ExtractTSDFMesh: no views")
+    if reso_level < 1:
+        raise ValueError("ExtractTSDFMesh: reso_level must be >= 1")
+    _tsdf_args(trunc, min_opacity, "ExtractTSDFMesh")
+    if int(reso) < 2:
+        raise ValueError("ExtractTSDFMesh: reso must be >= 2")
+    if bbox_min is not None and bbox_max is not None:
+        _lattice(bbox_min, bbox_max, reso, "ExtractTSDFMesh")
+    H, W = dataset.height_, dataset.width_
+    if H // reso_level < 2 or W // reso_level < 2:
+        raise ValueError(f"ExtractTSDFMesh: reso_level {reso_level} leaves a {H // reso_level} x {W // reso_level} grid of a {H} x {W} image")
+    apps = [resolve_appearance(renderer, appearance, view=b) for b in views]
+    opacity, median_t, colors, lo, hi = _tsdf_maps(renderer, dataset, views, reso_level, bbox_min, bbox_max, min_opacity, apps, crop)
+    idx = torch.as_tensor(views, device=dataset.poses_.device)
+    grid = FuseTSDF(dataset.poses_[idx], dataset.intri_[idx], dataset.dist_params_[idx], H, W, opacity, median_t, colors, lo, hi, reso,
+                    trunc, min_opacity)
+    del opacity, median_t, colors
+    return TSDFSurface(grid)
 
 
 def write_ply(path, mesh):

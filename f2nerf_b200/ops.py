@@ -255,6 +255,39 @@ def depth_consistency(pts, source, view, pose, intri, dist_params, height, width
     return count
 
 
+TSDF_MAX_VIEWS = 64      # f2b_tsdf_integrate: views per launch (their camera table is staged in shared memory)
+
+
+def tsdf_integrate(cams, opacity, median_t, colors, height, width, origin, voxel, z0, n_layers, mu, min_opacity, first, sdf_sum, weight,
+                   color_sum):
+    """f2b_tsdf_integrate: the views of ``cams`` [G,22] (their maps opacity / median_t [G,h,w], colors [G,h,w,3]) into layers
+    [z0, z0 + n_layers) of the sums sdf_sum / weight [nz,ny,nx] and color_sum [nz,ny,nx,3] (DESIGN §3p); ``first`` starts them
+    from 0."""
+    import ctypes
+    for t, name in ((cams, "cams"), (opacity, "opacity"), (median_t, "median_t"), (colors, "colors"), (sdf_sum, "sdf_sum"),
+                    (weight, "weight"), (color_sum, "color_sum")):
+        _chk(t, F32, f"tsdf_integrate: {name}")
+    G, h, w = opacity.shape
+    nz, ny, nx = sdf_sum.shape
+    if cams.shape != (G, 22) or median_t.shape != (G, h, w) or colors.shape != (G, h, w, 3) or weight.shape != (nz, ny, nx) \
+            or color_sum.shape != (nz, ny, nx, 3):
+        raise ValueError("tsdf_integrate: inconsistent shapes")
+    o3 = _host3(origin)
+    call("f2b_tsdf_integrate", cams, G, opacity, median_t, colors, int(height), int(width), h, w, ctypes.addressof(o3), float(voxel), nx,
+         ny, nz, int(z0), int(n_layers), float(mu), float(min_opacity), int(bool(first)), sdf_sum, weight, color_sum, stream())
+
+
+def tsdf_colors(verts, weight, color_sum, origin, voxel):
+    """f2b_tsdf_colors: colours [V,3] of vertices [V,3] of a fused lattice (DESIGN §3p)."""
+    import ctypes
+    _chk(verts, F32, "tsdf_colors: verts")
+    nz, ny, nx = weight.shape
+    out = dev_empty((verts.shape[0], 3), F32, verts)
+    o3 = _host3(origin)
+    call("f2b_tsdf_colors", verts, int(verts.shape[0]), weight, color_sum, nx, ny, nz, ctypes.addressof(o3), float(voxel), out, stream())
+    return out
+
+
 def ray_grad(trans, table_f16, prim_pool, bias_pool, n_volumes, local_size, params_f16, feat_f16, d_field_out_f16, d_mlp_in_f16, pts,
              t, dirs, anchors, rays_o, bounds, inv_field_loss_scale, inv_shader_loss_scale, row_work, d_rays_o, d_rays_d, d_pts=None,
              d_dirs=None, dfeat16=None):

@@ -233,6 +233,23 @@ int f2b_depth_consistency(const float* pts, const int* source, int n_pts, int vi
                           const float* dist_params, int height, int width, int out_h, int out_w, const float* opacity,
                           const float* median_t, float min_opacity, float rel_tol, int* count /* [n_pts], in/out */,
                           int* cell, void* stream);
+/* TSDF integration of a group of views into a lattice (DESIGN.md §3p).  cams [n_views,22] (device): per view pose [3,4]
+ * camera-to-world, rows 0-1 of K (6 floats) and (k1, k2, p1, p2); opacity, median_t [n_views,out_h,out_w] and colors
+ * [n_views,out_h,out_w,3], the views' maps on the grid of f2b_depth_consistency.  Lattice point (i, j, k) of the nx x ny x nz
+ * lattice (x fastest) is fadd(origin, fmul(voxel, index)) per axis; the launch covers layers [z0, z0 + n_layers).  Per point and
+ * view, in view order, with the projection of f2b_depth_consistency: where the cell is inside the grid, opacity >= min_opacity
+ * and sdf = median_t - |p - o| >= -mu, sdf_sum += min(1, sdf / mu), weight += 1 and color_sum += the cell's colour, each one
+ * fp32 addition.  first != 0 starts the sums from 0 instead of reading them.  n_views <= 64; mu finite and > 0; min_opacity in
+ * (0, 1].  origin3: host array of 3 floats. */
+int f2b_tsdf_integrate(const float* cams, int n_views, const float* opacity, const float* median_t, const float* colors, int height,
+                       int width, int out_h, int out_w, const float* origin3, float voxel, int nx, int ny, int nz, int z0,
+                       int n_layers, float mu, float min_opacity, int first, float* sdf_sum /* [nz,ny,nx] */,
+                       float* weight /* [nz,ny,nx] */, float* color_sum /* [nz,ny,nx,3] */, void* stream);
+/* Colours [n_verts,3] of vertices of a fused lattice: trilinear interpolation of color_sum / weight at each vertex over the corners
+ * of its cell that are observed (weight > 0, not on the lattice's outermost layer), their weights renormalised; 0 where no corner
+ * is observed.  origin3: host array of 3 floats; nx, ny, nz >= 2. */
+int f2b_tsdf_colors(const float* verts, int n_verts, const float* weight, const float* color_sum, int nx, int ny, int nz,
+                    const float* origin3, float voxel, float* colors, void* stream);
 /* Gradient of the rendered colour with respect to the rays of a VALIDATE batch (DESIGN.md §3k), behind the composite, shader-MLP and
  * input-assembly backward: rows p < n_pts are the compacted survivors f2b_render_phase2_fwd leaves (pts, t, dirs, anchors [P,3], feat
  * [P,32] fp16), d_field_out [P,16] fp16 = f2b_shader_prep_bwd_f16's dL/dout of the field MLP and d_mlp_in [P,32] fp16 = f2b_mlp_bwd2's

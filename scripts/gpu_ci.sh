@@ -14,19 +14,20 @@
 # And the appearance module (tests/test_gpu_appearance.py): float64 render twins on the device, and a 300-iteration ngp_fox training.
 # And the crop module (tests/test_gpu_crop.py): the cropped render against compacted layouts, and a 300-iteration ngp_fox training.
 # And the lens module (tests/test_gpu_lens.py): lens rays against their float64 twin, and a 300-iteration ngp_fox training.
+# And the TSDF module (tests/test_gpu_tsdf.py): the fusion kernel against its float64 twin, and a 300-iteration ngp_fox training.
 # And the reference-configs module (tests/test_gpu_ref_configs.py): both reference binaries, three arms on free, big20 and big22.
 P=tests/test_gpu_parity.py
 OWN=("$P::test_mlp_fwd_bwd" "$P::test_mlp_tc_tiles_and_f32_output" "$P::test_mlp_bwd_recompute_equals_saved"
      "$P::test_fused_epilogues_match_operator_sequence" "$P::test_fused_field_matches_unfused" "$P::test_shader_prep_bwd_f16"
      tests/test_gpu_bwd_fused.py tests/test_gpu_shade_fused.py tests/test_gpu_checkpoint.py tests/test_gpu_train_maintenance.py
      tests/test_gpu_cpp_host_steps.py tests/test_gpu_grad_autograd.py tests/test_gpu_cpp_ops_reference.py tests/test_gpu_geometry.py tests/test_gpu_normals.py
-     tests/test_gpu_pose.py tests/test_gpu_points.py tests/test_gpu_appearance.py tests/test_gpu_crop.py tests/test_gpu_lens.py)
+     tests/test_gpu_pose.py tests/test_gpu_points.py tests/test_gpu_appearance.py tests/test_gpu_crop.py tests/test_gpu_lens.py tests/test_gpu_tsdf.py)
 MAIN=(tests -m gpu --ignore=tests/test_ref_parity.py --ignore=tests/test_gpu_bwd_reference.py --ignore=tests/test_gpu_fwd_reference.py
       --ignore=tests/test_gpu_mlp_fwd_reference.py --ignore=tests/test_gpu_bwd_fused.py --ignore=tests/test_gpu_shade_fused.py --ignore=tests/test_gpu_checkpoint.py
       --ignore=tests/test_gpu_train_maintenance.py --ignore=tests/test_gpu_cpp_host_steps.py --ignore=tests/test_gpu_grad_autograd.py
       --ignore=tests/test_gpu_cpp_ops_reference.py --ignore=tests/test_gpu_geometry.py --ignore=tests/test_gpu_normals.py
       --ignore=tests/test_gpu_pose.py --ignore=tests/test_gpu_points.py --ignore=tests/test_gpu_appearance.py --ignore=tests/test_gpu_crop.py
-      --ignore=tests/test_gpu_lens.py --ignore=tests/test_gpu_ref_configs.py)
+      --ignore=tests/test_gpu_lens.py --ignore=tests/test_gpu_tsdf.py --ignore=tests/test_gpu_ref_configs.py)
 for T in "${OWN[@]}"; do case "$T" in *::*) MAIN+=(--deselect "$T");; esac; done
 if [ "${1:-}" = "--list" ]; then                 # print each pytest selection, one per line (collect with -m gpu --collect-only)
   echo "${MAIN[*]}"; for T in "${OWN[@]}"; do echo "$T"; done; echo tests/test_gpu_bwd_reference.py; echo tests/test_gpu_fwd_reference.py

@@ -26,6 +26,13 @@
 //       probes mean the iteration consumed the same draws.  Per iteration, <out_dir>/it<k>/ holds the state before the
 //       step, the Render outputs, the loss, the gradients (d_weights: dL/dweights as the loss hands it to Render's backward,
 //       the var-loss term through the reference's WeightVar), the octree after the step and the probes.
+//   ref_driver --march <runtime_config.yaml> <dir>
+//       PersSampler::GetSamples alone on trees and rays a test wrote.  Every subdirectory <case> of dir holding params.npy is one
+//       case, run in name order: tree_nodes.npy and pers_trans.npy (u8 blobs) replace the scene's octree and warps, rays_o /
+//       rays_d [n,3] f32 are the rays (GetSamples normalises rays_d itself; rays_d_used is what it marched), params [6] f32 =
+//       [train, near, sample_l, scale_by_dis, max_oct_intersect_per_ray, seed].  VALIDATE (train 0) marches with noise 1; TRAIN
+//       seeds the CUDA generator with `seed` and dumps the noise GetSamples draws (fineness 1).  <case> gets pts, dirs, dt, t,
+//       anchors [n,2] (the reference leaves the third column unwritten), bounds and first_oct_dis.
 //   ref_driver --ops <runtime_config.yaml> <in_dir> <out_dir>
 //       the two MLP operators alone, on inputs a test wrote: Hash3DAnchored::AnchoredQuery and SHShader::Query, each followed
 //       by (out * g).sum().backward().  In ref_driver these are the reference's own (tiny-cuda-nn); in ref_driver_b200 always
@@ -181,8 +188,10 @@ static void dump_scene(const Scene& sc, int n_rays) {
 
 static int run_steps(const std::string& conf_path, const std::string& out_root, int n_iters, int fixed_batch);
 static int run_ops(const std::string& conf_path, const std::string& in_dir, const std::string& out_root);
+static int run_march(const std::string& conf_path, const std::string& dir);
 
 int main(int argc, char** argv) {
+  if (argc >= 4 && std::string(argv[1]) == "--march") return run_march(argv[2], argv[3]);
   if (argc >= 5 && std::string(argv[1]) == "--ops") return run_ops(argv[2], argv[3], argv[4]);
   if (argc >= 3 && std::string(argv[1]) == "--train") {     // main.cpp:6-13 verbatim in behaviour
     torch::manual_seed(2022);
@@ -195,7 +204,8 @@ int main(int argc, char** argv) {
   if (argc < 4) {
     std::fprintf(stderr, "usage: ref_driver <config.yaml> <out_dir> <n_rays> [n_time_iters] [dump_full_grads] [fineness] [gs_progress]\n"
                          "       ref_driver --steps <config.yaml> <out_dir> <n_iters> [fixed_batch]\n"
-                         "       ref_driver --ops <config.yaml> <in_dir> <out_dir>\n");
+                         "       ref_driver --ops <config.yaml> <in_dir> <out_dir>\n"
+                         "       ref_driver --march <config.yaml> <dir>\n");
     return 1;
   }
   const std::string conf_path = argv[1];
@@ -644,5 +654,52 @@ static int run_ops(const std::string& conf_path, const std::string& in_dir, cons
                 sf[1].item<float>(), sf[2].item<float>());
   }
   std::printf("ref_driver: done, %d operator cases in %s\n", int(cases.size()), out_root.c_str());
+  return 0;
+}
+
+// ==================================================================================================== --march ===
+static int run_march(const std::string& conf_path, const std::string& root) {
+  Scene sc = make_scene(conf_path, true);
+  GlobalDataPool* gdp = sc.gdp.get();
+  PersSampler* sampler = sc.sampler;
+  std::vector<std::string> cases;
+  for (const auto& e : fs::directory_iterator(root))
+    if (fs::is_directory(e.path()) && fs::exists(e.path() / "params.npy")) cases.push_back(e.path().string());
+  std::sort(cases.begin(), cases.end());
+  for (const auto& dir : cases) {
+    const auto in = [&](const std::string& name, torch::TensorOptions opts) {
+      cnpy::NpyArray a = cnpy::npy_load(dir + "/" + name + ".npy");
+      CHECK(!a.fortran_order && a.word_size == size_t(opts.dtype().itemsize())) << name;
+      std::vector<int64_t> shape(a.shape.begin(), a.shape.end());
+      return torch::from_blob(a.data<char>(), shape, opts).clone().to(torch::kCUDA).contiguous();
+    };
+    sampler->pers_octree_->tree_nodes_gpu_ = in("tree_nodes", CPUUInt8).reshape({-1});
+    sampler->pers_octree_->pers_trans_gpu_ = in("pers_trans", CPUUInt8).reshape({-1});
+    Tensor rays_o = in("rays_o", CPUFloat), rays_d = in("rays_d", CPUFloat);
+    Tensor params = in("params", CPUFloat).to(torch::kCPU);
+    const bool train = params[0].item<float>() != 0.f;
+    sampler->global_near_ = params[1].item<float>();
+    sampler->sample_l_ = params[2].item<float>();
+    sampler->scale_by_dis_ = params[3].item<float>() != 0.f;
+    sampler->max_oct_intersect_per_ray_ = int(params[4].item<float>());
+    const int64_t seed = int64_t(params[5].item<float>());
+    gdp->ray_march_fineness_ = 1.f;
+    gdp->mode_ = train ? RunningMode::TRAIN : RunningMode::VALIDATE;
+    g_out = dir;
+    const int n_rays = int(rays_o.size(0));
+    torch::NoGradGuard ng;
+    dump("rays_d_used", rays_d / torch::linalg_norm(rays_d, 2, -1, true));
+    if (train) {   // the draw GetSamples makes first (PersSampler.cu:377, MAX_SAMPLE_PER_RAY 1024), replayed from the same seed
+      torch::manual_seed(seed);
+      dump("noise", (torch::rand({ 1024 + n_rays + 10 }, CUDAFloat) - .5f) + 1.f);
+      torch::manual_seed(seed);
+    }
+    auto s = sampler->GetSamples(rays_o, rays_d, Tensor());
+    dump("pts", s.pts); dump("dirs", s.dirs); dump("dt", s.dt); dump("t", s.t);
+    dump("anchors", s.anchors.index({Slc(), Slc(0, 2)}).contiguous());
+    dump("bounds", s.pts_idx_bounds); dump("first_oct_dis", s.first_oct_dis);
+    std::printf("{\"march_case\": \"%s\", \"rays\": %d, \"samples\": %d}\n", dir.c_str(), n_rays, int(s.pts.size(0)));
+  }
+  std::printf("ref_driver: done, %d march cases in %s\n", int(cases.size()), root.c_str());
   return 0;
 }

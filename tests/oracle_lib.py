@@ -68,6 +68,22 @@ def sampler(tree_nodes, trans, rays_o, rays_d, noise, near, far, sample_l, scale
     return out
 
 
+SAMPLER_COVER = ("guard", "guard_zero", "guard_plane", "guard_decides", "empty_eq", "near_past", "step0", "hop", "hop_inf",
+                 "hop_nan", "hop_sat", "stack_stop", "near_entry")
+
+
+def sampler_cover(tree_nodes, trans, rays_o, rays_d, noise, near, far, sample_l, scale_by_dis, max_hits):
+    """How often the march of this batch takes each branch of SAMPLER_COVER (orc_sampler_cover in oracle/f2_oracle.c)
+    -> dict name -> count."""
+    R = rays_o.shape[0]
+    bounds, totals = np.zeros((R, 2), np.int32), np.zeros(2, np.int32)
+    cov = np.zeros(len(SAMPLER_COVER), np.int64)
+    lib().orc_sampler_cover(_p(c(tree_nodes, np.uint8)), _p(c(trans, np.uint8)), _p(c(rays_o, np.float32)),
+                            _p(c(rays_d, np.float32)), _p(c(noise, np.float32)), I(R), F(near), F(far), F(sample_l),
+                            I(int(scale_by_dis)), I(max_hits), _p(bounds), _p(totals), _p(cov))
+    return dict(zip(SAMPLER_COVER, cov.tolist()))
+
+
 def edge_samples(edge_pool, trans, edge_idx, coord):
     n = edge_idx.shape[0]
     out_pts, out_idx = np.zeros((n, 2, 3), np.float32), np.zeros((n, 2), np.int32)

@@ -53,11 +53,11 @@ def hops(ref):
     return best
 
 
-def check_all_modes(scene, oracle, o, dn, noise, sample_l, scale_by_dis, max_hits=CAP):
+def check_all_modes(scene, oracle, o, dn, noise, sample_l, scale_by_dis, max_hits=CAP, near=0.05, far=1e8):
     from f2nerf_b200 import ops
-    ref = oracle.sampler(scene["nodes"], scene["trans"], o, dn, noise, 0.05, 1e8, sample_l, scale_by_dis, max_hits)
+    ref = oracle.sampler(scene["nodes"], scene["trans"], o, dn, noise, near, far, sample_l, scale_by_dis, max_hits)
     n = o.shape[0]
-    args = (T(scene["nodes"]), T(scene["trans"]), T(o), T(dn), T(noise), 0.05, 1e8, sample_l, scale_by_dis, max_hits)
+    args = (T(scene["nodes"]), T(scene["trans"]), T(o), T(dn), T(noise), near, far, sample_l, scale_by_dis, max_hits)
     # MODE 0 (count), with and without count_all_hits, then MODE 1 (fill)
     bounds, totals = ops.sampler_count(*args, count_all_hits=True)
     n_pts, n_hits = (int(v) for v in totals.tolist())
@@ -65,7 +65,7 @@ def check_all_modes(scene, oracle, o, dn, noise, sample_l, scale_by_dis, max_hit
     np.testing.assert_array_equal(N(bounds), ref["bounds"])
     b2, tot2 = ops.sampler_count(*args, count_all_hits=False)
     np.testing.assert_array_equal(N(b2), ref["bounds"])
-    assert int(tot2[0]) == n_pts and 0 < int(tot2[1]) <= n_hits
+    assert int(tot2[0]) == n_pts and min(n_hits, 1) <= int(tot2[1]) <= n_hits
     pts, dirs, dt, t, anchors, first = ops.sampler_fill(*args, bounds, n_pts)
     got = dict(pts=N(pts), dirs=N(dirs), dt=N(dt), t=N(t), first_oct_dis=N(first))
     for k in ("first_oct_dis", "t", "dt", "dirs", "pts"):
@@ -78,12 +78,13 @@ def check_all_modes(scene, oracle, o, dn, noise, sample_l, scale_by_dis, max_hit
         b3, tot3, first3 = ops.sampler_march(*args, scratch, count_all_hits=cah)
         np.testing.assert_array_equal(N(b3), ref["bounds"])
         assert int(tot3[0]) == n_pts
-        assert int(tot3[1]) == n_hits if cah else 0 < int(tot3[1]) <= n_hits
+        assert int(tot3[1]) == n_hits if cah else min(n_hits, 1) <= int(tot3[1]) <= n_hits
         np.testing.assert_array_equal(N(first3).view(np.uint32), ref["first_oct_dis"].view(np.uint32))
     # nothing was written past a ray's count in its slot
     cnt = np.diff(ref["bounds"], axis=1)[:, 0]
-    s_dt = N(scratch[1]).reshape(n, CAP)
-    assert np.isnan(s_dt[np.arange(CAP)[None, :] >= cnt[:, None]]).all()
+    past = np.arange(CAP)[None, :] >= cnt[:, None]
+    assert np.isnan(N(scratch[1]).reshape(n, CAP)[past]).all() and np.isnan(N(scratch[2]).reshape(n, CAP)[past]).all()
+    assert np.isnan(N(scratch[0]).reshape(n, CAP, 3)[past]).all() and (N(scratch[3]).reshape(n, CAP, 2)[past] == -7).all()
     g = ops.sampler_gather(T(dn), b3, n_pts, scratch)
     for k, v in zip(("pts", "dirs", "dt", "t"), g[:4]):
         np.testing.assert_array_equal(N(v).view(np.uint32), ref[k].view(np.uint32), err_msg=f"march {k}")
